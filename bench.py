@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- diffusion iter/s of the b200sd hot path on N B200s (one process per GPU).
+"""bench.py -- diffusion iter/s of the b200sd hot path on N H100s (one process per GPU).
 
 A "step" is one denoising iteration of BASELINE.json configs[1] (SD-2.1-base txt2img, 512x512, 20 DDIM
 steps, CFG 7.5, fp16): UNet forward at batch 2 (uncond, cond) + the fused CFG/scheduler-step kernel,
@@ -9,7 +9,12 @@ resident in HBM; `e2e` is the same iteration driven through the reference-facing
 pinned HOST buffers, host<->device copies inside the timed region.  Extra keys report 512^2 images/s
 (20 steps + VAE decode), the tensor-core roofline of the dominant kernel and the CPU baseline.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed as float32 DIR/<name>.npy:
+latents.npy, the updated latents [1, 4, 64, 64] (NCHW, what the pipeline's loop hands on), and noise_pred.npy, the
+UNet noise prediction [2, 4, 64, 64] (NCHW, uncond then cond: the layout UNetModel.__call__ returns).  The inputs are
+seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -36,7 +41,7 @@ def CONFIG(world):
     return {"workload": WORKLOAD, "unet_batch": 2, "latent": "4x64x64", "text_tokens": 77,
             "weights": "random-init SD-2.1-base (865.9 M params)",
             "parallelism": f"replicas x{world}, independent prompts per rank, no data-path collective",
-            "cache": "inputs larger than L2: every step streams 1.73 GB of fp16 weights through the 126 MB L2"}
+            "cache": "inputs larger than L2: every step streams 1.73 GB of fp16 weights through the 50 MB L2"}
 
 
 def _peaks():
@@ -45,11 +50,11 @@ def _peaks():
         with open(p) as f:
             d = json.load(f)
         return d["bf16_tflops"], d["bf16_tflops_sustained"], d["hbm_gbs"], "measured"
-    return 1590.0, 1400.0, 6650.0, "fallback"
+    return 989.0, 989.0, 3350.0, "H100 SXM data-sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -304,16 +309,9 @@ def class_breakdown(loop, barrier, peaks, pipe):
     burst, sustained, _, how = peaks
     ms = out["gemm_conv"]
     achieved = flops / (ms * 1e-3) / 1e12
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic_r2.json")) as f:
-            traffic = round(json.load(f)["dram_bytes_per_launch"])
-    except (OSError, KeyError, ValueError):
-        pass
-    roof = {"bound": "tensor", "kernel": "umma_gemm_kernel + halo_conv_kernel (every conv3x3 / 1x1 / linear launch of one UNet forward)",
+    roof = {"bound": "tensor", "kernel": "wgmma_gemm_kernel + halo_conv_kernel (every conv3x3 / 1x1 / linear launch of one UNet forward)",
             "achieved": round(achieved, 1), "peak": sustained, "unit": "TFLOP/s", "frac": round(achieved / sustained, 4),
-            "peak_kind": f"{how} sustained bf16 dense (kernels timed inside a long step)", "traffic": traffic,
-            "traffic_unit": "DRAM bytes per launch (ncu; algorithmic = weights 1.73e9 B / forward)",
+            "peak_kind": f"{how} sustained bf16 dense (kernels timed inside a long step)",
             "launches": launches, "algorithmic_tflop": round(flops / 1e12, 4), "kernel_ms_sum": ms,
             "how": "CUDA-graph replay of the loop with only the GEMM / convolution class launching (same buffers, no "
                    "event gaps), divided by the steps"}
@@ -345,6 +343,13 @@ def extra_config(name, dev, barrier, peaks, steps=N_STEPS_IMG):
             "launches_per_step": round(loop.launches_per_image / N_STEPS_IMG, 1),
             "step_roofline": {"algorithmic_tflop": tflop, "achieved": round(tflop / (ms * 1e-3), 1), "peak": sustained,
                               "unit": "TFLOP/s", "frac": round(tflop / (ms * 1e-3) / sustained, 4)}}
+
+
+def dump_outputs(out_dir, arrays):
+    """What the timed path handed back in its last step, as float32 .npy files (a few hundred KB in all)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def run_gpu_arm(args, rank, local_rank, world):
@@ -390,6 +395,9 @@ def run_gpu_arm(args, rank, local_rank, world):
     e1.record()
     barrier()
     ms_dev = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        # the engine keeps the noise prediction NHWC; a caller of UNetModel receives it NCHW
+        dump_outputs(args.dump_outputs, {"latents": pipe._latents, "noise_pred": unet._out_nhwc.permute(0, 3, 1, 2)})
     if args.quick:
         if rank == 0:
             print(json.dumps({"quick": True, "iter_per_s": round(world * args.steps / (ms_dev * 1e-3), 2),
@@ -539,6 +547,8 @@ def main():
     ap.add_argument("--no-batched", action="store_true", help="skip the 8-prompts-per-GPU images/s measurement")
     ap.add_argument("--quick", action="store_true", help="device-resident iter/s only (tuning runs; not a bench line)")
     ap.add_argument("--no-extra", action="store_true", help="skip the SDXL-768 / ControlNet configs (N = 1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's latents and noise prediction as float32 .npy")
     ap.add_argument("--profile-step", action="store_true",
                     help="run ONE eager denoising iteration between cudaProfilerStart/Stop (for ncu --profile-from-start off)")
     args = ap.parse_args()
@@ -553,6 +563,8 @@ def main():
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}",
                "--master-addr", "127.0.0.1", "--master-port", "29517", os.path.abspath(__file__), "--gpus",
                str(args.gpus), "--steps", str(args.steps), "--warmup", str(args.warmup)]
+        if args.dump_outputs:
+            cmd += ["--dump-outputs", os.path.abspath(args.dump_outputs)]
         sys.exit(subprocess.call(cmd))
     if not torch.cuda.is_available():
         print(json.dumps({"error": "no CUDA device: b200sd has no CPU fallback; use --impl reference for the CPU arm"}))

@@ -1,4 +1,4 @@
-/* b200sd -- C-ABI of the Blackwell-native Stable Diffusion hot path.
+/* b200sd -- C-ABI of the Hopper-native Stable Diffusion hot path.
  *
  * Drop-in boundary.  The reference (apple/ml-stable-diffusion) is pure Python; its device
  * boundary is `CoreMLModel.__call__(**np.ndarray) -> dict` (python_coreml_stable_diffusion/
@@ -41,8 +41,8 @@ void b200sd_set_launch_classes(uint32_t mask);
 uint64_t b200sd_launch_count(void);
 
 /* ---- tensor-core GEMM / implicit-GEMM convolution --------------------------------------
- * out[M, N] = epilogue( A[M, K] * W[N, K]^T ),  fp16 operands, fp32 accumulate (tcgen05.mma
- * kind::f16, accumulators in TMEM, operands TMA-staged with 128B swizzle).
+ * out[M, N] = epilogue( A[M, K] * W[N, K]^T ),  fp16 operands, fp32 accumulate (wgmma
+ * m64nNk16, accumulators in registers, operands TMA-staged with 128B swizzle).
  *
  *   mode 0  "linear"  : every nn.Conv2d(k=1) of the reference (unet.py:74-84 q/k/v/out,
  *                       :533-551 proj_in/out, :613 GEGLU proj, :601 FF out, :464 conv_shortcut,

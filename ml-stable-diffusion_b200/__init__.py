@@ -1,4 +1,4 @@
-"""b200sd -- Blackwell-native Stable Diffusion hot path (UNet denoising loop, CFG + scheduler
+"""b200sd -- Hopper-native Stable Diffusion hot path (UNet denoising loop, CFG + scheduler
 step, VAE decoder) behind the reference's model-call / pipeline interface.
 
 The directory is named ``ml-stable-diffusion_b200`` (not importable as-is); import it as

@@ -1,4 +1,4 @@
-"""In-tree build of ``libb200sd.so`` (sm_100a only) with nvcc.  No JIT cache, no torch extension:
+"""In-tree build of ``libb200sd.so`` (sm_90a only) with nvcc.  No JIT cache, no torch extension:
 the library is a plain C-ABI shared object (``include/b200sd.h``) loaded with ctypes."""
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ LIB = os.path.join(HERE, "libb200sd.so")
 STAMP = os.path.join(HERE, ".libb200sd.stamp")
 SOURCES = ["runtime.cu", "gemm_conv.cu", "attention.cu", "norm.cu", "elementwise.cu", "model.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math_placeholder",
 ]
 
@@ -38,7 +38,7 @@ def _digest():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a and link ``libb200sd.so``.  Returns its path."""
+    """Compile every CUDA source for sm_90a and link ``libb200sd.so``.  Returns its path."""
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(STAMP):
         with open(STAMP) as f:
@@ -63,7 +63,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
         if verbose and out.strip():
             print(out, file=sys.stderr)
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

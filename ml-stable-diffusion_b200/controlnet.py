@@ -1,4 +1,4 @@
-"""ControlNet on the sm_100a kernels: the UNet encoder half + mid block + 1x1 "zero convs" and the
+"""ControlNet on the sm_90a kernels: the UNet encoder half + mid block + 1x1 "zero convs" and the
 8-conv conditioning embedder (reference ``python_coreml_stable_diffusion/controlnet.py:15-250``), with the
 reference's model-call contract (``pipeline.py:259-284``: ``sample, timestep, encoder_hidden_states,
 controlnet_cond`` -> ``additional_residual_i``).  Re-uses ``UNetEngine``'s packed blocks; the conditioning

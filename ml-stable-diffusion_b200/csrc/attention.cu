@@ -1,16 +1,15 @@
-// b200sd -- flash-style attention for sm_100a: S = Q K^T and O += P V on tcgen05 tensor cores
-// (accumulators in TMEM), Q/K/V tiles staged by TMA (SWIZZLE_128B), online softmax (exp2 domain)
-// in registers, P handed back to the tensor core through shared memory.
+// b200sd -- flash-style attention for sm_90a: S = Q K^T and O += P V on wgmma tensor cores (fp32 accumulators in
+// registers), Q/K/V tiles staged by TMA (SWIZZLE_128B), online softmax (exp2 domain) in registers, P handed to the
+// tensor core straight from registers (wgmma with A in registers).
 //
 // Replaces attention.original / split_einsum / split_einsum_v2 of the reference
 // (python_coreml_stable_diffusion/attention.py:24-168, dispatched by Einsum unet.py:45-59): the
 // three variants are one function, softmax(q^T k / sqrt(d) + mask) v per (batch, head); the
 // (B, heads, Sq, Sk) score tensor the reference materialises (671 MB at S=4096) never leaves the SM.
 //
-// CTA = 128 queries x 1 head; warp 0 TMA producer, warp 1 MMA issuer, warps 2..5 softmax (one query
-// row per thread).  The pipeline runs on 64-key halves: S is double-buffered in TMEM (2 x 64 columns) and P
-// in shared memory (2 x 16 KiB), so S_{h+1} = Q K^T and O += P_{h-1} V execute on the tensor core while the
-// softmax warps exponentiate half h.  256 TMEM columns (S 128 + O 64) so two CTAs share an SM.
+// CTA = 128 queries x 1 head; warps 0..7 are two consumer warpgroups (64 query rows each), warp 8 the TMA producer.
+// The K/V ring holds two 128-key tiles; each warpgroup walks them in 64-key halves: S_h = Q K_h^T, softmax, O += P_h V_h.
+// While one warpgroup is in its exponentials the other one keeps the tensor core busy.
 #include "common.cuh"
 #include "../../include/b200sd.h"
 
@@ -20,9 +19,10 @@ extern void count_launch(int n);
 
 static constexpr int kQ = 128;   // queries per CTA
 static constexpr int kKV = 128;  // keys per K/V tile (one TMA load)
-static constexpr int kHalf = 64;  // keys per pipeline step: S is double-buffered by halves of a tile
+static constexpr int kHalf = 64;  // keys per pipeline step
 static constexpr int kD = 64;    // head dim
-static constexpr int kAttnThreads = 192;
+static constexpr int kAttnThreads = 288;
+static constexpr int kProducerWarp = 8;
 static constexpr int kTileBytes = 128 * 64 * 2;  // 16 KiB: one [128 x 64] fp16 tile
 static constexpr int kKvStages = 2;
 
@@ -36,21 +36,20 @@ struct __align__(64) AttnParams {
     // work decomposition: query tile t -> (q tile t % q_tiles, head (t / q_tiles) % heads, image t / (q_tiles * heads)).
     // streamk == 0: grid = tiles, one CTA per query tile.  streamk == 1: the tiles x n_kv (query tile, K/V tile) units are
     // cut into gridDim.x equal contiguous ranges, so a CTA works on the tail of one query tile and the head of the next;
-    // pieces of a split tile go through `ws` and the last piece to finish merges them in slot order (see attn_finish).
+    // pieces of a split tile go through `ws` and the last piece to finish merges them in slot order.
     int q_tiles, heads, n_kv, streamk;
     long long total_units;
     float* ws;      // [gridDim.x][2] partials of kPartialFloats floats
     int* counters;  // [tiles], zero between launches
 };
 
-// one partial: O [64 d][128 rows] fp32 (column-major so a warp's rows are contiguous), then m_ref[128], l[128]
+// one partial: O [64 d][128 rows] fp32 (column-major so consecutive rows are contiguous), then m_ref[128], l[128]
 static constexpr int kPartialFloats = (kD + 2) * kQ;
 static constexpr size_t kCounterBytes = 64 * 1024;
 
-// smem layout (1024-aligned): Q | P (2 x 16K, K-chunks of 64 keys) | K[2] | V[2] | barriers
+// smem layout (1024-aligned): Q | K[2] | V[2] | barriers
 static constexpr int kSmemQ = 0;
-static constexpr int kSmemP = kTileBytes;
-static constexpr int kSmemK = kSmemP + 2 * kTileBytes;
+static constexpr int kSmemK = kSmemQ + kTileBytes;
 static constexpr int kSmemV = kSmemK + kKvStages * kTileBytes;
 static constexpr int kSmemBar = kSmemV + kKvStages * kTileBytes;
 static constexpr int kAttnSmemBytes = kSmemBar + 128;
@@ -95,65 +94,43 @@ __device__ __forceinline__ int segment_halves(const AttnParams& p, const AttnSeg
     return min(2 * sg.k1, n_half) - 2 * sg.k0;
 }
 
-__global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __grid_constant__ AttnParams p) {
+__global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid_constant__ AttnParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSmemBar);
     uint64_t* q_full = bars + 0;
     uint64_t* kv_full = bars + 1;   // [2]
     uint64_t* kv_empty = bars + 3;  // [2]
-    uint64_t* s_full = bars + 5;    // [2]  per 64-key half of S
-    uint64_t* s_empty = bars + 7;   // [2]
-    uint64_t* p_full = bars + 9;    // [2]  per 64-key chunk of P
-    uint64_t* o_full = bars + 11;   // [2]  P V of the chunk retired (P chunk reusable; O quiescent up to here)
-    uint64_t* q_empty = bars + 13;  // every S MMA of the segment retired: Q may be overwritten
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 14);
-    int* last_flag = reinterpret_cast<int*>(bars + 15);
+    uint64_t* q_empty = bars + 5;   // every S MMA of the segment retired: Q may be overwritten
+    int* last_flag = reinterpret_cast<int*>(bars + 6);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        // SWIZZLE_128B tiles need a 1024-byte aligned base; a padded buffer would cost the second CTA per SM, so a
-        // misaligned launch (never observed: the kernel has no static shared memory) fails loudly instead
+        // SWIZZLE_128B tiles need a 1024-byte aligned base; a misaligned launch (never observed: the kernel has no
+        // static shared memory) fails loudly instead
         if ((smem_u32(smem) & 1023u) != 0) __trap();
         prefetch_tmap(&p.tmQ);
         prefetch_tmap(&p.tmK);
         prefetch_tmap(&p.tmV);
         mbar_init(q_full, 1);
-        mbar_init(q_empty, 1);
+        mbar_init(q_empty, 2);
         for (int s = 0; s < kKvStages; ++s) {
             mbar_init(&kv_full[s], 1);
-            mbar_init(&kv_empty[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&s_full[b], 1);
-            mbar_init(&s_empty[b], 128);
-            mbar_init(&p_full[b], 128);
-            mbar_init(&o_full[b], 1);
+            mbar_init(&kv_empty[s], 2);  // one arrival per consumer warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr, 256);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    pdl_trigger();  // after this CTA's TMEM allocation: a dependent CTA can never take the columns this grid still needs
+    pdl_trigger();
     pdl_wait();     // PDL: the prologue above overlapped the previous kernel's tail
-    const uint32_t tmem_s = tmem_base;        // 2 x 64 columns (double-buffered S halves)
-    const uint32_t tmem_o = tmem_base + 128;  // 64 columns
 
-    // All three roles walk the same segment list.  The pipeline counters run ACROSS segments: jg counts K/V tiles (smem
-    // stage jg % 2), g counts 64-key halves (S / P buffer g & 1); a half's position inside its K/V tile is hl & 1 because
-    // segments start on tile boundaries.
+    // Both roles walk the same segment list.  The K/V tile counter jg runs ACROSS segments (smem stage jg % 2).
     SegmentWalk walk;
     walk.init(p);
     AttnSegment sg;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         if (lane == 0) {
             int seg = 0, jg = 0;
             while (walk.next(p, sg)) {
@@ -175,271 +152,115 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __grid
                 ++seg;
             }
         }
-    } else if (warp == 1) {
-        // S_h = Q K_h^T : A = Q (K-major), B = 64 rows of the K tile (K-major), M=128 N=64 K=64
-        const uint32_t idesc_s = make_idesc_f16(128, kHalf, 0, 0);
-        // O += P_h V_h : A = P chunk (K-major, 64 keys), B = 64 rows of the V tile [keys][d] = MN-major, N=64 K=64
-        const uint32_t idesc_o = make_idesc_f16(128, kD, 0, 1);
-        const uint32_t q_addr = smem_u32(smem + kSmemQ);
-        const uint32_t p_addr = smem_u32(smem + kSmemP);
-        int seg = 0, jg0 = 0, g0 = 0;
-        while (walk.next(p, sg)) {
-            const int nh = segment_halves(p, sg, (sg.tile % p.q_tiles) * kQ);
-            auto issue_s = [&](int hl) {
-                const int g = g0 + hl, b = g & 1, hi = hl & 1;
-                const int jg = jg0 + (hl >> 1), st = jg % kKvStages;
-                mbar_wait(&kv_full[st], (jg / kKvStages) & 1);
-                if (g >= 2) mbar_wait(&s_empty[b], ((g - 2) >> 1) & 1);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint64_t adesc = make_smem_desc_sw128(q_addr, 1024, 0);
-                    const uint64_t bdesc =
-                        make_smem_desc_sw128(smem_u32(smem + kSmemK + st * kTileBytes) + hi * (kHalf * 128), 1024, 0);
-#pragma unroll
-                    for (int k = 0; k < kD / 16; ++k)
-                        umma_f16_ss(tmem_s + b * kHalf, adesc + 2 * k, bdesc + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-                    umma_commit(&s_full[b]);
-                }
-                __syncwarp();
-            };
-            mbar_wait(q_full, seg & 1);
-            issue_s(0);
-            if (nh > 1) issue_s(1);
-            for (int hl = 0; hl < nh; ++hl) {
-                const int g = g0 + hl, b = g & 1, hi = hl & 1;
-                const int st = (jg0 + (hl >> 1)) % kKvStages;
-                mbar_wait(&p_full[b], (g >> 1) & 1);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t v_addr = smem_u32(smem + kSmemV + st * kTileBytes) + hi * (kHalf * 128);
-#pragma unroll
-                    for (int k = 0; k < kHalf / 16; ++k) {
-                        // A: +32 B per 16 keys inside the chunk's 128 B rows;  B: 16 keys = 16 rows of 128 B = 2048 B
-                        const uint64_t adesc = make_smem_desc_sw128(p_addr + b * kTileBytes, 1024, 0) + 2 * k;
-                        const uint64_t bdesc = make_smem_desc_sw128(v_addr + k * 2048, 1024, kKV * 128);
-                        umma_f16_ss(tmem_o, adesc, bdesc, idesc_o, (hl > 0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&o_full[b]);
-                    if (hi == 1 || hl == nh - 1) umma_commit(&kv_empty[st]);  // last half of this K/V tile
-                }
-                __syncwarp();
-                if (hl + 2 < nh) issue_s(hl + 2);
-            }
-            if (lane == 0) umma_commit(q_empty);
-            __syncwarp();
-            ++seg, jg0 += (nh + 1) / 2, g0 += nh;
-        }
-    } else {
-        // ---------------- softmax warps: one query row per thread ----------------
-        // O accumulates in TMEM across all KV steps (PV MMAs with accumulate=1).  The exp2 reference m_ref
-        // is refreshed lazily: a full, unmasked half tile is exponentiated optimistically against the current
-        // m_ref in ONE pass over S (row maximum tracked on the side); only if some row's maximum exceeds
-        // m_ref by more than kTau (log2 domain; P <= 2^kTau stays inside fp16) does the warp wait for the
-        // outstanding P V MMAs, rescale its 32 rows of O in TMEM and redo the half -- rare after the first tiles.
-        // S is double-buffered by halves, so the tensor core computes S_{h+1} / S_{h+2} and P_{h-1} V while
-        // this half is in the exponentials.
-        constexpr float kTau = 8.0f;
-        const int lane_group = warp & 3;
-        const int row = lane_group * 32 + lane;
-        const uint32_t lane_addr = static_cast<uint32_t>(lane_group * 32) << 16;
-        const uint32_t o_addr = tmem_o + lane_addr;
+    } else if (warp < kProducerWarp) {
+        // ---------------- consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) of the tile ----------------
+        // Accumulator layout (m64n64): this thread holds rows lr and lr + 8 (lr = 16 (warp % 4) + lane / 4 inside the
+        // warpgroup's 64), columns 8 j + 2 (lane % 4) + {0, 1}, j = 0..7: s[4 j + {0, 1}] row lr, s[4 j + {2, 3}] row lr + 8.
+        // A row is spread over the four lanes of a quad: row maxima / sums reduce with two shuffles.
+        const int wg = warp >> 2;
+        const int lr = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile-local row of s[.. 0, 1]; lr + 8 for s[.. 2, 3]
+        const int cq = 2 * (lane & 3);
+        const bool leader = (threadIdx.x & 127) == 0;
         const float sl2 = p.scale_log2;
-        float m_ref = -INFINITY, l_run = 0.f;
-        uint8_t* p_row = smem + kSmemP + row * 128;
-        const int sw = row & 7;
-
-        // lean row maximum of a full unmasked half (raw scores)
-        auto row_max_lean = [&](uint32_t s_addr) {
-            float m0 = -INFINITY, m1 = -INFINITY;
-            uint32_t va[32], vb[32];
-            tmem_ld32(s_addr, va);
-            tmem_ld32(s_addr + 32, vb);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                m0 = fmaxf(m0, fmaxf(__uint_as_float(va[i]), __uint_as_float(vb[i])));
-                m1 = fmaxf(m1, fmaxf(__uint_as_float(va[i + 1]), __uint_as_float(vb[i + 1])));
-            }
-            return fmaxf(m0, m1);
-        };
-        // lean probabilities of a full unmasked half against reference `ref`: writes the fp16 P chunk (one
-        // 128-byte swizzled row per query: eight 16-byte pieces), returns the row sum and (tmax) the raw maximum
-        auto probs_lean = [&](uint32_t s_addr, uint8_t* dst, float ref, float& tmax) {
-            const float neg_m = -ref;
-            float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-            float m0 = -INFINITY, m1 = -INFINITY;
-            uint32_t va[32], vb[32];
-            tmem_ld32(s_addr, va);
-            tmem_ld32(s_addr + 32, vb);
-            tmem_ld_wait();
-            uint32_t pk[32];
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                const float a0 = __uint_as_float(va[i]), a1 = __uint_as_float(va[i + 1]);
-                const float b0 = __uint_as_float(vb[i]), b1 = __uint_as_float(vb[i + 1]);
-                m0 = fmaxf(m0, fmaxf(a0, b0));
-                m1 = fmaxf(m1, fmaxf(a1, b1));
-                const float p0 = ex2_approx(fmaf(a0, sl2, neg_m));
-                const float p1 = ex2_approx(fmaf(a1, sl2, neg_m));
-                const float p2 = ex2_approx(fmaf(b0, sl2, neg_m));
-                const float p3 = ex2_approx(fmaf(b1, sl2, neg_m));
-                s0 += p0, s1 += p1, s2 += p2, s3 += p3;
-                pk[i >> 1] = pack_half2(p0, p1);
-                pk[16 + (i >> 1)] = pack_half2(p2, p3);
-            }
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                uint4 val = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-                *reinterpret_cast<uint4*>(dst + ((q ^ sw) << 4)) = val;
-            }
-            tmax = fmaxf(m0, m1);
-            return (s0 + s1) + (s2 + s3);
-        };
-        // rescale this warp's rows of O (TMEM) and the running sum from reference m_ref to m_new
-        auto rescale_o = [&](float m_new) {
-            const float factor = ex2_approx(m_ref - m_new);  // 1 for rows whose reference did not move
-#pragma unroll
-            for (int c = 0; c < kD; c += 32) {
-                uint32_t v[32];
-                tmem_ld32(o_addr + c, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * factor);
-                tmem_st32(o_addr + c, v);
-            }
-            tmem_st_wait();
-            l_run *= factor;
-        };
-
-        int g0 = 0;
+        const uint32_t q_addr = smem_u32(smem + kSmemQ) + wg * 64 * 128;
+        int seg = 0, jg0 = 0;
         while (walk.next(p, sg)) {
             const int qt = sg.tile % p.q_tiles, head = (sg.tile / p.q_tiles) % p.heads, batch = sg.tile / (p.q_tiles * p.heads);
             const int q0 = qt * kQ;
             const int nh = segment_halves(p, sg, q0);
             const float* mask_row = p.mask ? p.mask + static_cast<size_t>(batch) * p.sk : nullptr;
-            m_ref = -INFINITY, l_run = 0.f;
+            float o[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) o[i] = 0.f;
+            float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+            mbar_wait(q_full, seg & 1);
             for (int hl = 0; hl < nh; ++hl) {
-                const int g = g0 + hl, b = g & 1;
-                const int h = 2 * sg.k0 + hl;                          // this half's position among the keys
+                const int jg = jg0 + (hl >> 1), st = jg % kKvStages, hi = hl & 1;
+                if (hi == 0) mbar_wait(&kv_full[st], (jg / kKvStages) & 1);
+                // ---- S = Q K_h^T ----
+                float s[32];
+                const uint64_t qdesc = make_smem_desc_sw128(q_addr, 1024, 0);
+                const uint64_t kdesc = make_smem_desc_sw128(smem_u32(smem + kSmemK + st * kTileBytes) + hi * (kHalf * 128), 1024, 0);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kD / 16; ++k) wgmma_m64n64_ss(s, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<32>(s);
+                if (hl == nh - 1 && leader) mbar_arrive(q_empty);  // the segment's last read of Q retired
+                // ---- online softmax (log2 domain) ----
+                const int h = 2 * sg.k0 + hl;                     // this half's position among the keys
                 const int kvalid = min(kHalf, p.sk - h * kHalf);  // >= 1
                 // causal: a half whose last key is <= the tile's first query is fully visible to every row
                 const bool diag = p.causal && (h * kHalf + kHalf - 1 > q0);
-                const int qi = q0 + row;  // this thread's query index
-                const uint32_t s_addr = tmem_s + lane_addr + b * kHalf;
-                uint8_t* dst = p_row + b * kTileBytes;
-                mbar_wait(&s_full[b], (g >> 1) & 1);
-                if (g >= 2) mbar_wait(&o_full[b], ((g - 2) >> 1) & 1);  // P V of half g-2 retired: P chunk b is free
-                tc_fence_after();
-                // every P V issued so far (up to half g-1) has retired: O may be rescaled in place
-                auto wait_o_quiescent = [&]() {
-                    if (hl >= 1) {
-                        mbar_wait(&o_full[(g - 1) & 1], ((g - 1) >> 1) & 1);
-                        tc_fence_after();
-                    }
-                };
-                float l_half;
-                if (mask_row == nullptr && kvalid == kHalf && !diag) {
-                    if (hl == 0) {
-                        m_ref = row_max_lean(s_addr) * sl2;
-                        float unused;
-                        l_half = probs_lean(s_addr, dst, m_ref, unused);
-                    } else {
-                        float tmax;
-                        l_half = probs_lean(s_addr, dst, m_ref, tmax);
-                        const float m_half = tmax * sl2;
-                        if (__any_sync(0xffffffffu, m_half > m_ref + kTau)) {
-                            const float m_new = fmaxf(m_ref, m_half);
-                            wait_o_quiescent();
-                            rescale_o(m_new);
-                            m_ref = m_new;
-                            l_half = probs_lean(s_addr, dst, m_ref, tmax);
-                        }
-                    }
-                } else {
-                    // ---- general half (additive mask and/or ragged tail): two passes with per-key predicates ----
-                    float m_half = -INFINITY;
-#pragma unroll 1
-                    for (int c = 0; c < kHalf; c += 32) {
-                        uint32_t v[32];
-                        tmem_ld32(s_addr + c, v);
-                        tmem_ld_wait();
+                const bool general = mask_row != nullptr || kvalid < kHalf || diag;
 #pragma unroll
-                        for (int i = 0; i < 32; ++i) {
-                            float sc = __uint_as_float(v[i]) * sl2;
-                            const bool vis = c + i < kvalid && (!diag || h * kHalf + c + i <= qi);
-                            if (mask_row && vis) sc += mask_row[h * kHalf + c + i] * 1.4426950408889634f;
-                            if (vis) m_half = fmaxf(m_half, sc);
-                        }
+                for (int e = 0; e < 32; ++e) {
+                    float v = s[e] * sl2;
+                    if (general) {
+                        const int key = 8 * (e >> 2) + cq + (e & 1);
+                        const int qi = q0 + lr + 8 * ((e >> 1) & 1);
+                        const bool vis = key < kvalid && (!diag || h * kHalf + key <= qi);
+                        if (mask_row != nullptr && vis) v += mask_row[h * kHalf + key] * 1.4426950408889634f;
+                        if (!vis) v = -INFINITY;
                     }
-                    if (__any_sync(0xffffffffu, m_half > m_ref + kTau)) {
-                        const float m_new = fmaxf(m_ref, m_half);
-                        if (hl > 0) {
-                            wait_o_quiescent();
-                            rescale_o(m_new);
-                        }
-                        m_ref = m_new;
-                    }
-                    l_half = 0.f;
-#pragma unroll 1
-                    for (int c = 0; c < kHalf; c += 32) {
-                        uint32_t v[32];
-                        tmem_ld32(s_addr + c, v);
-                        tmem_ld_wait();
-                        uint32_t pk[16];
-#pragma unroll
-                        for (int i = 0; i < 32; i += 2) {
-                            float s0 = __uint_as_float(v[i]) * sl2, s1 = __uint_as_float(v[i + 1]) * sl2;
-                            const bool vis0 = c + i < kvalid && (!diag || h * kHalf + c + i <= qi);
-                            const bool vis1 = c + i + 1 < kvalid && (!diag || h * kHalf + c + i + 1 <= qi);
-                            if (mask_row) {
-                                if (vis0) s0 += mask_row[h * kHalf + c + i] * 1.4426950408889634f;
-                                if (vis1) s1 += mask_row[h * kHalf + c + i + 1] * 1.4426950408889634f;
-                            }
-                            const float p0 = vis0 ? ex2_approx(s0 - m_ref) : 0.f;
-                            const float p1 = vis1 ? ex2_approx(s1 - m_ref) : 0.f;
-                            l_half += p0 + p1;
-                            pk[i >> 1] = pack_half2(p0, p1);
-                        }
-                        const int piece0 = c >> 3;
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            uint4 val = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-                            *reinterpret_cast<uint4*>(dst + (((piece0 + q) ^ sw) << 4)) = val;
-                        }
-                    }
+                    s[e] = v;
                 }
-                l_run += l_half;
-                tc_fence_before();
-                mbar_arrive(&s_empty[b]);
-                fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-                mbar_arrive(&p_full[b]);
+                float m_use[2];
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    float mx = -INFINITY;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * r], s[4 * j + 2 * r + 1]));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    const float m_new = fmaxf(m_run[r], mx);
+                    m_use[r] = m_new == -INFINITY ? 0.f : m_new;  // a row with nothing visible yet
+                    const float factor = ex2_approx(m_run[r] - m_use[r]);
+                    m_run[r] = m_new;
+                    l_run[r] *= factor;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) o[4 * j + 2 * r] *= factor, o[4 * j + 2 * r + 1] *= factor;
+                }
+                uint32_t pa[4][4];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float p0 = ex2_approx(s[4 * j] - m_use[0]), p1 = ex2_approx(s[4 * j + 1] - m_use[0]);
+                    const float p2 = ex2_approx(s[4 * j + 2] - m_use[1]), p3 = ex2_approx(s[4 * j + 3] - m_use[1]);
+                    l_run[0] += p0 + p1;
+                    l_run[1] += p2 + p3;
+                    // A fragment of keys [16 kk, 16 kk + 16): {row lr, keys 0..7}, {lr + 8, 0..7}, {lr, 8..15}, {lr + 8, 8..15}
+                    pa[j >> 1][2 * (j & 1)] = pack_half2(p0, p1);
+                    pa[j >> 1][2 * (j & 1) + 1] = pack_half2(p2, p3);
+                }
+                // ---- O += P V_h: B = 64 rows of the V tile [keys][d] = MN-major, 16 keys = 2048 B per step ----
+                const uint32_t v_addr = smem_u32(smem + kSmemV + st * kTileBytes) + hi * (kHalf * 128);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < kHalf / 16; ++kk)
+                    wgmma_m64n64_rs_tb(o, pa[kk], make_smem_desc_sw128(v_addr + kk * 2048, 1024, kKV * 128), 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<32>(o);
+                if ((hi == 1 || hl == nh - 1) && leader) mbar_arrive(&kv_empty[st]);  // last half of this K/V tile
             }
-            // ---- the segment's last commit covers every earlier P V ----
-            const int gl = g0 + nh - 1;
-            mbar_wait(&o_full[gl & 1], (gl >> 1) & 1);
-            tc_fence_after();
-            g0 += nh;
-            const bool store = q0 + row < p.sq;
-            __half* dst = p.out + (static_cast<size_t>(batch) * p.sq + (store ? q0 + row : 0)) * p.ldo + head * kD;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+                l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+            }
+            ++seg, jg0 += (nh + 1) / 2;
             if (sg.k0 == 0 && sg.k1 == p.n_kv) {
                 // whole query tile in this CTA: normalise and store
-                const float inv_l = 1.0f / l_run;
 #pragma unroll
-                for (int c = 0; c < kD; c += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(o_addr + c, v);
-                    tmem_ld_wait();
-                    if (store) {
+                for (int r = 0; r < 2; ++r) {
+                    const int qi = q0 + lr + 8 * r;
+                    if (qi >= p.sq) continue;
+                    const float inv_l = 1.0f / l_run[r];
+                    __half* dst = p.out + (static_cast<size_t>(batch) * p.sq + qi) * p.ldo + head * kD;
 #pragma unroll
-                        for (int i = 0; i < 32; i += 8) {
-                            uint4 val;
-                            val.x = pack_half2(__uint_as_float(v[i]) * inv_l, __uint_as_float(v[i + 1]) * inv_l);
-                            val.y = pack_half2(__uint_as_float(v[i + 2]) * inv_l, __uint_as_float(v[i + 3]) * inv_l);
-                            val.z = pack_half2(__uint_as_float(v[i + 4]) * inv_l, __uint_as_float(v[i + 5]) * inv_l);
-                            val.w = pack_half2(__uint_as_float(v[i + 6]) * inv_l, __uint_as_float(v[i + 7]) * inv_l);
-                            *reinterpret_cast<uint4*>(dst + c + i) = val;
-                        }
-                    }
+                    for (int j = 0; j < 8; ++j)
+                        *reinterpret_cast<uint32_t*>(dst + 8 * j + cq) = pack_half2(o[4 * j + 2 * r] * inv_l, o[4 * j + 2 * r + 1] * inv_l);
                 }
             } else {
                 // ---- a piece of a split tile: park (O, m_ref, l) in the workspace; the piece that finishes last merges
@@ -448,45 +269,53 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __grid
                 const int first = slot_of(p, t0), last = slot_of(p, t0 + p.n_kv - 1);
                 float* mine = p.ws + (static_cast<size_t>(blockIdx.x) * 2 + (sg.k0 > 0 ? 1 : 0)) * kPartialFloats;
 #pragma unroll
-                for (int c = 0; c < kD; c += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(o_addr + c, v);
-                    tmem_ld_wait();
+                for (int r = 0; r < 2; ++r) {
+                    const int row = lr + 8 * r;
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) __stcg(mine + (c + i) * kQ + row, __uint_as_float(v[i]));
+                    for (int j = 0; j < 8; ++j) {
+                        __stcg(mine + (8 * j + cq) * kQ + row, o[4 * j + 2 * r]);
+                        __stcg(mine + (8 * j + cq + 1) * kQ + row, o[4 * j + 2 * r + 1]);
+                    }
+                    if ((lane & 3) == 0) {
+                        __stcg(mine + kD * kQ + row, m_run[r]);
+                        __stcg(mine + (kD + 1) * kQ + row, l_run[r]);
+                    }
                 }
-                __stcg(mine + kD * kQ + row, m_ref);
-                __stcg(mine + (kD + 1) * kQ + row, l_run);
                 __threadfence();
-                named_bar_sync(1, 128);
-                if (threadIdx.x == 64) {
+                named_bar_sync(1, 256);
+                if (threadIdx.x == 0) {
                     const int old = atomicAdd(p.counters + sg.tile, 1);
                     const int is_last = old == last - first;
                     if (is_last) p.counters[sg.tile] = 0;  // every piece has checked in: ready for the next launch
                     *last_flag = is_last;
                 }
-                named_bar_sync(1, 128);
+                named_bar_sync(1, 256);
                 if (*last_flag) {
                     __threadfence();
+                    // merge: thread t takes row t % 128, head-dim columns [32 (t / 128), + 32)
+                    const int row = threadIdx.x & 127;
+                    const int cbase = 32 * (threadIdx.x >> 7);
+                    const bool store = q0 + row < p.sq;
+                    __half* dst = p.out + (static_cast<size_t>(batch) * p.sq + (store ? q0 + row : 0)) * p.ldo + head * kD;
                     float m = -INFINITY;
-                    for (int s = first; s <= last; ++s) {
-                        const float* part = p.ws + (static_cast<size_t>(s) * 2 + (slot_begin(p, s) > t0 ? 1 : 0)) * kPartialFloats;
+                    for (int s2 = first; s2 <= last; ++s2) {
+                        const float* part = p.ws + (static_cast<size_t>(s2) * 2 + (slot_begin(p, s2) > t0 ? 1 : 0)) * kPartialFloats;
                         m = fmaxf(m, __ldcg(part + kD * kQ + row));
                     }
                     float l = 0.f;
-                    for (int s = first; s <= last; ++s) {
-                        const float* part = p.ws + (static_cast<size_t>(s) * 2 + (slot_begin(p, s) > t0 ? 1 : 0)) * kPartialFloats;
+                    for (int s2 = first; s2 <= last; ++s2) {
+                        const float* part = p.ws + (static_cast<size_t>(s2) * 2 + (slot_begin(p, s2) > t0 ? 1 : 0)) * kPartialFloats;
                         l += __ldcg(part + (kD + 1) * kQ + row) * ex2_approx(__ldcg(part + kD * kQ + row) - m);
                     }
                     const float inv_l = 1.0f / l;
 #pragma unroll 1
-                    for (int c = 0; c < kD; c += 16) {
+                    for (int c = cbase; c < cbase + 32; c += 16) {
                         float acc[16];
 #pragma unroll
                         for (int i = 0; i < 16; ++i) acc[i] = 0.f;
-                        for (int s = first; s <= last; ++s) {
+                        for (int s2 = first; s2 <= last; ++s2) {
                             const float* part =
-                                p.ws + (static_cast<size_t>(s) * 2 + (slot_begin(p, s) > t0 ? 1 : 0)) * kPartialFloats;
+                                p.ws + (static_cast<size_t>(s2) * 2 + (slot_begin(p, s2) > t0 ? 1 : 0)) * kPartialFloats;
                             const float f = ex2_approx(__ldcg(part + kD * kQ + row) - m);
 #pragma unroll
                             for (int i = 0; i < 16; ++i) acc[i] = fmaf(__ldcg(part + (c + i) * kQ + row), f, acc[i]);
@@ -504,17 +333,9 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __grid
                         }
                     }
                 }
-                named_bar_sync(1, 128);  // last_flag is rewritten by the next segment
+                named_bar_sync(1, 256);  // last_flag is rewritten by the next segment
             }
-            tc_fence_before();  // the next segment's first P V overwrites O: order it after the reads above
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 256);
     }
 }
 
@@ -522,10 +343,10 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __grid
 
 using namespace b200sd;
 
-// Stream-K pays when whole-tile scheduling leaves a badly filled last wave (320 tiles on 296 CTA slots at S = 4096) or
-// too few tiles to fill the GPU; cost model in K/V-tile units with ~2 units of fixed cost per segment.
+// Stream-K pays when whole-tile scheduling leaves a badly filled last wave (320 tiles on 132 CTA slots at S = 4096) or
+// too few tiles to fill the GPU; cost model in K/V-tile units with ~2 units of fixed cost per segment.  One CTA per SM.
 static int attention_slots(int tiles, int n_kv, int causal, bool have_ws) {
-    const int slots = 2 * num_sms();
+    const int slots = num_sms();
     if (!have_ws || causal || n_kv < 8 || static_cast<size_t>(tiles) * 4 > kCounterBytes) return 0;
     {
         const char* e = getenv("B200SD_ATTN_STREAMK");
@@ -539,7 +360,7 @@ static int attention_slots(int tiles, int n_kv, int causal, bool have_ws) {
 }
 
 extern "C" size_t b200sd_attention_workspace_bytes(void) {
-    return kCounterBytes + static_cast<size_t>(2 * num_sms()) * 2 * kPartialFloats * sizeof(float);
+    return kCounterBytes + static_cast<size_t>(num_sms()) * 2 * kPartialFloats * sizeof(float);
 }
 
 extern "C" int b200sd_attention_ws(const void* q, const void* k, const void* v, void* out, const float* mask,

@@ -1,5 +1,5 @@
-// b200sd -- shared device/host helpers for the sm_100a kernels (inline PTX wrappers for
-// mbarrier, TMA, tcgen05/TMEM; host-side tensor-map encoding; error plumbing).
+// b200sd -- shared device/host helpers for the sm_90a kernels (inline PTX wrappers for
+// mbarrier, TMA, wgmma; host-side tensor-map encoding; error plumbing).
 #pragma once
 
 #include <cuda.h>
@@ -43,7 +43,7 @@ int num_sms();
 
 // Programmatic dependent launch (PDL): when enabled every kernel is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, so the next kernel's CTAs may start (and run their
-// prologue: barrier init, TMEM allocation, tensor-map prefetch) while the previous grid drains; every kernel
+// prologue: barrier init, tensor-map prefetch) while the previous grid drains; every kernel
 // executes griddepcontrol.wait before it reads or writes global memory.
 bool pdl_enabled();
 
@@ -164,175 +164,89 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
-// ---- tcgen05 / TMEM ------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
+// ---- wgmma (sm_90a warpgroup MMA: 128 threads, fp32 accumulators in registers) ------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float* d) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16/bf16 operands, fp32 accumulate)
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
+
+#define B200SD_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x N] (+)= A[64 x 16] (smem, K-major) * B[N x 16]^T (smem, K-major unless trans_b); fp16 in, fp32 accumulate.
+// Accumulator layout (thread t of the warpgroup): d[4 j + e] = (row 16 (t / 32) + (t % 32) / 4 + 8 (e / 2),
+// column 8 j + 2 (t % 4) + e % 2).
+template <int kTransB = 0>
+__device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued tcgen05.mma of this thread arrive on `bar` when complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// ---- CTA pairs (cta_group::2): one tcgen05.mma spans the two CTAs of a cluster ---------------------
-// Leader = the even CTA of the pair; it issues the MMAs and owns the barriers the tensor core signals.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-// shared::cluster address of `local_addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
-    return ra;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void cluster_arrive_wait() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA loads of a CTA pair: the data lands in the issuing CTA's shared memory, the transaction bytes are
-// credited to `bar_cluster_addr`, which may live in the other CTA of the pair (the leader's full barrier)
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster_addr,
-                                                 int c0, int c1, uint64_t hint) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster_addr,
-                                                 int c0, int c1, int c2, int c3, uint64_t hint) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(hint)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t addr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[128 rows from each CTA's smem] * B[N/2 rows from each CTA's smem]; M = 256
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued pair MMAs arrive on the barrier at this shared-memory offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(cta_mask)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread i <-> lane base+i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24)
+        : "l"(da), "l"(db), "r"(acc), "n"(kTransB)
         : "memory");
 }
-// 32 lanes x 16 columns store (registers -> TMEM)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_m64n32_ss(float* d, uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8)
+        : "l"(da), "l"(db), "r"(acc)
         : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n16_ss(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+// A from registers (fp16 pairs in the accumulator layout of a 64 x 16 tile), B [16 x 64] from smem, MN-major
+__device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc)
+        : "memory");
+}
+#undef B200SD_F8
+
+// D[64 x bn] (+)= A[64 x 16] * B[bn x 16]^T as 64 / 32 / 16-column pieces (bn: multiple of 16, <= 2 R).  The pieces'
+// accumulators are consecutive in `d`, so d keeps the layout of one 64 x bn accumulator.  Every index is a compile-time
+// constant: d stays in registers.
+template <int R>
+__device__ __forceinline__ void wgmma_rows64(float (&d)[R], int bn, uint64_t da, uint64_t db, uint32_t acc) {
+#pragma unroll
+    for (int c = 0; c + 64 <= 2 * R; c += 64)
+        if (c + 64 <= bn) wgmma_m64n64_ss(d + c / 2, da, db + (c * 128 >> 4), acc);
+    const int c32 = bn & ~63;
+#pragma unroll
+    for (int c = 0; c + 32 <= 2 * R; c += 64)
+        if (c == c32 && (bn & 32)) wgmma_m64n32_ss(d + c / 2, da, db + (c * 128 >> 4), acc);
+    const int c16 = bn & ~31;
+#pragma unroll
+    for (int c = 0; c + 16 <= 2 * R; c += 32)
+        if (c == c16 && (bn & 16)) wgmma_m64n16_ss(d + c / 2, da, db + (c * 128 >> 4), acc);
 }
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-
-// ---- UMMA descriptors -----------------------------------------------------------------
-// Shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B.
+// ---- wgmma shared-memory matrix descriptors -------------------------------------------------------------
+// SWIZZLE_128B (layout type 1 in bits 62-63).
 //   K-major tile  : rows of 128 B (64 fp16 along K), 8-row swizzle atoms 1024 B apart (SBO=1024),
-//                   LBO unused (single atom along K).
+//                   LBO unused (single atom along K).  +32 B (desc + 2) per K=16 step.
 //   MN-major tile : rows of 128 B (64 fp16 along MN) indexed by k; 8-k atoms 1024 B apart (SBO=1024);
 //                   LBO = byte distance between successive 64-wide MN chunks.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
@@ -340,16 +254,8 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;  // descriptor version (sm_100)
-    d |= static_cast<uint64_t>(2) << 61;  // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
     return d;
-}
-// Instruction descriptor for kind::f16: fp16 A/B, fp32 D, M=128.
-//   a_major/b_major: 0 = K-major, 1 = MN-major.
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(uint32_t m, uint32_t n, uint32_t a_major, uint32_t b_major) {
-    return (1u << 4)                 // D format: F32
-           | (0u << 7) | (0u << 10)  // A, B format: F16
-           | (a_major << 15) | (b_major << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 // 2^x, single MUFU op, denormal results flushed to zero (softmax probabilities)

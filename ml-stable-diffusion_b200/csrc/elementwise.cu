@@ -17,7 +17,7 @@ static inline int grid_for(size_t n, int threads) {
 template <typename T>
 __global__ void nchw_to_nhwc_kernel(const T* __restrict__ in, __half* __restrict__ out, int n, int c, int hw,
                                     int c_pad) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t total = static_cast<size_t>(n) * hw * c_pad;
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
@@ -35,7 +35,7 @@ __global__ void nchw_to_nhwc_kernel(const T* __restrict__ in, __half* __restrict
 template <typename T>
 __global__ void nhwc_to_nchw_f32_kernel(const T* __restrict__ in, float* __restrict__ out, int n, int c, int hw,
                                         int c_pad) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t total = static_cast<size_t>(n) * c * hw;
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
@@ -51,7 +51,7 @@ __global__ void nhwc_to_nchw_f32_kernel(const T* __restrict__ in, float* __restr
 // ---- (B, D, 1, S) -> [B*S, D] fp16 (tiled transpose through shared memory) -------------------
 template <typename T>
 __global__ void ctx_to_tokens_kernel(const T* __restrict__ in, __half* __restrict__ out, int d, int s) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     __shared__ float tile[32][33];
     const int b = blockIdx.z;
@@ -72,7 +72,7 @@ __global__ void ctx_to_tokens_kernel(const T* __restrict__ in, __half* __restric
 __global__ void embed_tokens_kernel(const float* __restrict__ ids, const uint4* __restrict__ tok,
                                     const uint4* __restrict__ pos, uint4* __restrict__ out, int rows, int s, int vecs,
                                     int vocab) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t total = static_cast<size_t>(rows) * vecs;
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
@@ -92,7 +92,7 @@ __global__ void embed_tokens_kernel(const float* __restrict__ ids, const uint4* 
 // ---- nearest x2 upsample, NHWC fp16, 16-byte vectors ------------------------------------------
 __global__ void upsample2x_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, int n, int h, int w,
                                   int vecs) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t total = static_cast<size_t>(n) * (2 * h) * (2 * w) * vecs;
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
@@ -109,7 +109,7 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ in, uint4* __restric
 
 __global__ void add_kernel(const __half2* __restrict__ a, const __half2* __restrict__ b, __half2* __restrict__ out,
                            size_t n2) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n2;
          i += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(256) linear_small_kernel(const float* __restri
                                                            const float* __restrict__ add, float* __restrict__ out,
                                                            int m, int n, int k, int act_in, int act_out) {
     extern __shared__ __align__(16) float xs[];  // [kM][k]
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     for (int i = threadIdx.x; i < kM * k; i += blockDim.x) {
         const int r = i / k;
@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(256) linear_small_kernel(const float* __restri
 // ---- sinusoidal timestep embedding (unet.py:703-728) -------------------------------------------
 __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __restrict__ out, int m, int dim,
                                           int flip, float freq_shift) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int half = dim / 2;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -215,7 +215,7 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
 __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __restrict__ latents,
                                 float* __restrict__ hist, float* __restrict__ denoised, __half* __restrict__ unet_in,
                                 int c_pad, int n, int c, int hw, b200sd_step_coeffs k) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int numel = n * c * hw;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -261,7 +261,7 @@ __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __r
 template <typename T>
 __global__ void image_post_kernel(const T* __restrict__ in, int c_pad, float* __restrict__ of, uint8_t* __restrict__ ou,
                                   size_t pixels, int c) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t total = pixels * c;
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
@@ -280,7 +280,7 @@ __global__ void image_post_kernel(const T* __restrict__ in, int c_pad, float* __
 __global__ void latent_prep_kernel(const float* __restrict__ z, const float* __restrict__ w /* [c, c] */,
                                    const float* __restrict__ b, float inv_scale, __half* __restrict__ out, int n, int c,
                                    int hw, int c_pad) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n * hw) return;

@@ -1,11 +1,11 @@
-// b200sd -- tcgen05 GEMM / im2col-free implicit-GEMM 3x3 convolution for sm_100a.
+// b200sd -- wgmma GEMM / im2col-free implicit-GEMM 3x3 convolution for sm_90a.
 //
 // One persistent, warp-specialised kernel:
-//   warp 0      TMA producer  (cp.async.bulk.tensor 2D/4D boxes, SWIZZLE_128B, mbarrier tx)
-//   warp 1      MMA issuer    (one elected lane; tcgen05.mma kind::f16 M=128, N=block_n, K=16;
-//                              accumulators double-buffered in TMEM; tcgen05.commit -> mbarriers)
-//   warps 2..9  epilogue      (tcgen05.ld 32x32b; two warps per TMEM lane quarter split the columns; bias / time-embedding / GEGLU / residual; fp16|fp32
-//                              stores or fp32 split-K partials)
+//   warp 8      TMA producer  (cp.async.bulk.tensor 2D/4D boxes, SWIZZLE_128B, mbarrier tx)
+//   warps 0..7  two consumer warpgroups: wgmma m64nNk16 (fp16 operands from shared memory, fp32 accumulators in
+//               registers; warpgroup w owns tile rows [64 w, 64 w + 64)), then the epilogue: the accumulators are parked
+//               in shared memory over the drained stages and read back row-wise (bias / time-embedding / GEGLU /
+//               residual; fp16|fp32 stores or fp32 split-K partials)
 //
 // Replaces every nn.Conv2d of the reference UNet / VAE decoder (reference
 // python_coreml_stable_diffusion/unet.py:74-84, 435-464, 499-507, 533-551, 601-617, 853, 970).
@@ -23,16 +23,16 @@ namespace b200sd {
 static constexpr int kBM = 128;
 static constexpr int kBK = 64;
 static constexpr int kAStage = kBM * kBK * 2;  // 16 KiB
-static constexpr int kGemmThreads = 320;  // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
+static constexpr int kGemmThreads = 288;  // warps 0..7: two consumer warpgroups (wgmma + epilogue), warp 8: TMA producer
 static constexpr int kEpiThreads = 256;
+static constexpr int kProducerWarp = 8;
 static constexpr int kMaxStages = 8;
 static constexpr int kHaloMaxStages = 24;  // weight ring of the halo kernel (narrow tiles need many stages in flight)
 static constexpr int kSmemBudget = 220 * 1024;
 static constexpr int kEpiFixed = 2 * 256 * 4 + 256 * 4 + 64;  // bias vectors, LayerNorm fold vector, flags + image ids
 
 // Shared-memory budget of one GEMM CTA.  B200SD_SMEM_KB (read per call: tuning scripts flip it) caps the pipeline
-// depth: at <= ~110 KB (and <= 256 TMEM columns) two CTAs fit on one SM, so under programmatic dependent launch the
-// next kernel's CTAs become resident -- and prefetch their weights -- while the previous kernel still runs.
+// depth.  The register file holds one 288-thread CTA per SM, so a smaller budget only shortens the pipeline.
 static int smem_budget() {
     const char* e = getenv("B200SD_SMEM_KB");
     if (e && e[0]) {
@@ -56,14 +56,9 @@ struct __align__(64) GemmParams {
     int cluster;     // split-K on a thread-block cluster: the `splits` CTAs of a tile reduce it through DSMEM
     int pad_lo;      // conv: zero padding before the first row / column (1 = symmetric pad 1; 0 = pad only after: the
                      // VAE encoder's F.pad(x, (0, 1, 0, 1)) + stride-2 conv)
-    int two_cta;     // CTA pairs: one tcgen05.mma cta_group::2 computes two M tiles, each CTA stages half of B
-    int m_pairs;     // ceil(m_tiles / 2)
     int wgt_tiled;   // B operand pre-tiled: tile (n_tile, kb) starts at row (n_tile * kb_total + kb) * block_n
     int bias_mode;   // 0 none, 1 staged in smem (<= 2 vectors per tile), 2 read from global per chunk
     int res_smem;    // 1: residual tile prefetched into smem with cp.async
-    int acc_bufs;    // accumulator buffers in TMEM: 2 = double-buffered (persistent CTAs with several tiles), 1 otherwise
-    int acc_stride;  // TMEM columns between the buffers
-    int tmem_cols;   // columns to allocate (power of two >= 32): 256 or less lets two CTAs share an SM (PDL overlap)
     void* out;
     const float* bias;
     const __half* residual;
@@ -95,9 +90,9 @@ struct __align__(64) GemmParams {
     const float* ln_wg;        // [N] sum_k W'[j, k]
     int ln_parts, ln_k;
     float ln_eps;
-    long long* dbg;            // optional timeline of CTA 0 (clock64 at fixed points; tools/halo_timeline.py)
     int staged;                // staged epilogue (fp16 tile in shared memory, coalesced row-wise stores)
     int stage_dedicated;       // the staging tile has its own shared memory (persistent CTAs with several tiles)
+    long long* dbg;            // optional timeline of CTA 0 (clock64 at fixed points; tools/halo_timeline.py)
 };
 
 struct TileCoord {
@@ -108,13 +103,9 @@ struct TileCoord {
     int ya, xa, c0, xlo, xhi, ylo, yhi;
 };
 
-__device__ __forceinline__ TileCoord decode_work(const GemmParams& p, int work, int cta_rank = 0) {
+__device__ __forceinline__ TileCoord decode_work(const GemmParams& p, int work) {
     TileCoord t;
-    if (p.two_cta) {  // work = (pair of M tiles, N tile); the two CTAs of the pair take M tiles 2i and 2i + 1
-        t.split = 0;
-        t.m_tile = 2 * (work % p.m_pairs) + cta_rank;  // may be == m_tiles for an odd count: an all-padding tile
-        t.n_tile = work / p.m_pairs;
-    } else if (p.cluster) {  // the CTAs of a cluster (consecutive blockIdx.x) are the k-splits of one tile
+    if (p.cluster) {  // the CTAs of a cluster (consecutive blockIdx.x) are the k-splits of one tile
         t.split = work % p.splits;
         const int r = work / p.splits;
         t.m_tile = r % p.m_tiles;
@@ -396,54 +387,23 @@ __device__ __forceinline__ void staged_load_residual(const GemmParams& p, const 
 }
 
 // ---- staged epilogue (fp16 outputs) ------------------------------------------------------------------------------
-// Phase A: every epilogue thread owns one accumulator row (TMEM lane): TMEM -> registers -> (+LN fold) + bias -> fp16
-//          -> staging tile in shared memory [128][block_n + 8].
+// Phase A (stage_accumulators): each consumer thread converts its accumulator fragment ((+LN fold) + bias -> fp16) into
+//          the staging tile in shared memory [128][block_n + 8].
 // Phase B: warp w owns rows [16 w, 16 w + 16); its lanes walk a row as 16-byte vectors, so the residual read and the
 //          output store are contiguous row segments; the same pass accumulates the per-channel (column) sums that the
 //          consumer's GroupNorm needs and the per-row sums its LayerNorm needs, from the ROUNDED outputs.  Residual
-//          vectors are requested four iterations ahead (the first four before the accumulator wait).
+//          vectors are requested four iterations ahead (the first four before the main loop).
 // Phase C: column sums: lanes -> warps (shared memory, fixed order) -> one partial per (image, tile); the last CTA to
 //          arrive for an (image, n_tile) adds the partials of all tiles in slot order: deterministic, no float atomics.
 // Kept compact on purpose (runtime loops, small unroll factors): these kernels execute every instruction once per
 // CTA, so code size is instruction-fetch time.  Inlined: the parameters must come from the constant bank and the
 // shared-memory pointers must keep their address space (an out-of-line version used generic LD.E / ST.E for both).
-__device__ __forceinline__ void staged_epilogue(const GemmParams& p, const TileCoord& t, uint32_t taddr, __half* tile_s,
-                                             float* scratch, unsigned int* flag_s, const float* bias_row,
-                                             const float* wg_s, int ew, int lane, int row, int out_row, bool valid,
-                                             uint4 (&res)[4]) {
+__device__ __forceinline__ void staged_epilogue(const GemmParams& p, const TileCoord& t, __half* tile_s, float* scratch,
+                                             unsigned int* flag_s, int ew, int lane, uint4 (&res)[4]) {
     const int bn = p.block_n;
     const int ldt = bn + 8;
     const int ncol0 = t.n_tile * bn;
-    // ---------------- phase A ----------------
-    {
-        const float2 lc = ln_row_coeffs(p, out_row, valid);
-        const bool ln = p.ln_parts != 0;
-        __half* trow = tile_s + row * ldt;
-        uint32_t va[32];
-#pragma unroll 1
-        for (int c = 32 * (ew >> 2); c < bn; c += 64) {
-            tmem_ld32(taddr + c, va);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-                float x[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    float a = __uint_as_float(va[j + e]);
-                    if (ln) a = fmaf(a, lc.x, lc.y * wg_s[c + j + e]);
-                    if (bias_row != nullptr) a += bias_row[c + j + e];
-                    x[e] = a;
-                }
-                uint4 pk;
-                pk.x = pack_half2(x[0], x[1]);
-                pk.y = pack_half2(x[2], x[3]);
-                pk.z = pack_half2(x[4], x[5]);
-                pk.w = pack_half2(x[6], x[7]);
-                *reinterpret_cast<uint4*>(trow + c + j) = pk;
-            }
-        }
-    }
-    epi_bar_sync();
+    epi_bar_sync();  // phase A of every thread is in the staging tile
     // ---------------- phase B ----------------
     const StagedMap m = staged_map(p, t, lane);
     const bool want_stats = p.cs_partial != nullptr || p.rs_out != nullptr;
@@ -581,62 +541,136 @@ __device__ __forceinline__ void staged_epilogue(const GemmParams& p, const TileC
     }
 }
 
-template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kTwoCta = false, bool kStaged = false>
-__global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid_constant__ GemmParams p) {
+// Main loop of one tile on a consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile, all block_n columns, over the
+// k-blocks [kb0, kb1) of the ring.  A stage is released (one arrival per warpgroup) once the wgmma that read it retired;
+// one k-block stays in flight behind the one being issued.
+template <int R>
+__device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[R], const uint8_t* smem_a,
+                                              const uint8_t* smem_b, int b_stage, uint64_t* full_bar,
+                                              uint64_t* empty_bar, int kb0, int kb1, int& stage, uint32_t& phase,
+                                              int wg, bool leader) {
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smem_a + stage * kAStage + wg * (kAStage / 2)), 1024, 0);
+        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + stage * b_stage), 1024, 0);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k)
+            wgmma_rows64(acc, p.block_n, adesc + 2 * k, bdesc + 2 * k, (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == p.stages) {
+            stage = 0;
+            phase ^= 1;
+        }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs<R>(acc);
+    if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+}
+
+// Accumulator fragment of a consumer thread -> fp32 tile in shared memory, row-major with row stride `ld` floats
+// (the layout the row-wise epilogue and the cluster split-K reduction read).
+template <int R>
+__device__ __forceinline__ void park_accumulators(const float (&acc)[R], int bn, float* dst, int ld, int r0, int lane) {
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < R / 4; ++j) {
+        if (8 * j < bn) {
+            *reinterpret_cast<float2*>(dst + r0 * ld + 8 * j + cq) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(dst + (r0 + 8) * ld + 8 * j + cq) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+    }
+}
+
+// Phase A of the staged epilogue straight from the accumulator fragment: (+LayerNorm fold) + bias -> fp16 staging tile
+// [128][block_n + 8].  `bias0` / `bias1`: bias vectors of rows r0 and r0 + 8 (null = none).
+template <int R>
+__device__ __forceinline__ void stage_accumulators(const GemmParams& p, const TileCoord& t, const float (&acc)[R],
+                                                   __half* tile_s, const float* bias0, const float* bias1,
+                                                   const float* wg_s, int r0, int lane) {
+    const int bn = p.block_n;
+    const int ldt = bn + 8;
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        int out_row;
+        const bool valid = tile_row(p, t, r, out_row);
+        const float2 lc = ln_row_coeffs(p, out_row, valid);
+        const bool ln = p.ln_parts != 0;
+        const float* bias = h ? bias1 : bias0;
+#pragma unroll
+        for (int j = 0; j < R / 4; ++j) {
+            if (8 * j < bn) {
+                const int c = 8 * j + cq;
+                float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+                if (ln) x0 = fmaf(x0, lc.x, lc.y * wg_s[c]), x1 = fmaf(x1, lc.x, lc.y * wg_s[c + 1]);
+                if (bias != nullptr) x0 += bias[c], x1 += bias[c + 1];
+                *reinterpret_cast<uint32_t*>(tile_s + r * ldt + c) = pack_half2(x0, x1);
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+        const float4 f = *reinterpret_cast<const float4*>(src + j);
+        v[j] = __float_as_uint(f.x), v[j + 1] = __float_as_uint(f.y), v[j + 2] = __float_as_uint(f.z), v[j + 3] = __float_as_uint(f.w);
+    }
+}
+__device__ __forceinline__ void acc_ld16(const float* src, uint32_t (&v)[16]) {
+#pragma unroll
+    for (int j = 0; j < 16; j += 4) {
+        const float4 f = *reinterpret_cast<const float4*>(src + j);
+        v[j] = __float_as_uint(f.x), v[j + 1] = __float_as_uint(f.y), v[j + 2] = __float_as_uint(f.z), v[j + 3] = __float_as_uint(f.w);
+    }
+}
+
+// kR: accumulator registers per consumer thread (>= block_n / 2): 64 for tiles up to 128 columns, 128 above
+template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kR>
+__global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __grid_constant__ GemmParams p) {
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
     // integer-rounded pointer -- lets the compiler emit LDS / STS for everything derived from it; rounding through
     // uintptr_t turned every shared access of the loader and the epilogues into generic LD.E / ST.E
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw;
     if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
-    // a CTA of a pair stages only its half of the B tile (block_n / 2 rows); the MMA reads both halves
-    const int b_rows = kTwoCta ? (p.block_n >> 1) : p.block_n;
-    const int b_stage = b_rows * (kBK * 2);
-    const int cta_rank = kTwoCta ? static_cast<int>(cluster_ctarank()) : 0;
+    const int b_stage = p.block_n * (kBK * 2);
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + p.stages * kAStage;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + p.stages * b_stage);
     uint64_t* empty_bar = full_bar + kMaxStages;
-    uint64_t* tmem_full = empty_bar + kMaxStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    float* bias_s = reinterpret_cast<float*>(tmem_ptr + 4);           // [2][block_n] (16 B aligned)
+    uint64_t* acc_free = empty_bar + kMaxStages;                     // the pipeline memory is free for the next tile
+    float* bias_s = reinterpret_cast<float*>(acc_free + 4);           // [2][block_n] (16 B aligned)
     float* wg_s = bias_s + 2 * 256;                                   // [block_n] LayerNorm fold vector
     unsigned int* flag_s = reinterpret_cast<unsigned int*>(wg_s + 256);  // [8]
     __half* res_s = reinterpret_cast<__half*>(flag_s + 16);           // [128][block_n + 8] residual / staging tile
     const int ldr = p.block_n + 8;
+    // fp32 accumulator tile [128][block_n + 4] over the drained pipeline stages (the producer waits on acc_free before it
+    // loads the next tile); the row stride keeps the 32 rows a warp reads on distinct banks
+    float* acc_s = reinterpret_cast<float*>(smem);
+    const int lda = p.block_n + 4;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         prefetch_tmap(&p.tmA0);
         prefetch_tmap(&p.tmA1);
         prefetch_tmap(&p.tmB);
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
         }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tmem_full[s], 1);
-            mbar_init(&tmem_empty[s], kTwoCta ? 2 * kEpiThreads : kEpiThreads);  // pair: both CTAs' epilogues
-        }
+        mbar_init(acc_free, 1);
         fence_barrier_init();
     }
-    if (warp == 1) {
-        if (kTwoCta) {
-            tmem_alloc_pair(tmem_ptr, 512);
-            tmem_relinquish_pair();
-        } else {
-            tmem_alloc(tmem_ptr, static_cast<uint32_t>(p.tmem_cols));
-            tmem_relinquish();
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    if (kTwoCta) cluster_arrive_wait();  // the peer's barriers are initialised before anything signals them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     // PDL: everything above overlapped the previous kernel's tail.  Each role executes griddepcontrol.wait itself,
     // right before its first access to memory the previous kernels may still be producing: the TMA producer first
     // prefetches the (constant) weight tiles of its first pipeline stages, so the HBM latency of the weights hides
@@ -644,11 +678,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
     // grid is resident.
     pdl_trigger();
 
-    const int total_work = kTwoCta ? p.m_pairs * p.n_tiles : p.m_tiles * p.n_tiles * p.splits;
-    const int work0 = kTwoCta ? (blockIdx.x >> 1) : blockIdx.x;
-    const int work_step = kTwoCta ? (gridDim.x >> 1) : gridDim.x;
+    const int total_work = p.m_tiles * p.n_tiles * p.splits;
+    const int work0 = blockIdx.x;
+    const int work_step = gridDim.x;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ------------------------------- TMA producer -------------------------------
         if (lane == 0) {
             int stage = 0;
@@ -661,14 +695,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
                 const int c = (src1 ? (j - p.kc0) : j) * kBK;
                 const int wk = tap * p.Kpt + (src1 ? p.C0 : 0) + c;
                 void* dst_b = smem_b + st * b_stage;
-                const int brow = p.wgt_tiled ? (t.n_tile * p.kb_total + kb) * p.block_n + cta_rank * b_rows
-                                             : t.n_tile * p.block_n + cta_rank * b_rows;
-                if (kTwoCta)
-                    tma_load_2d_pair(dst_b, &p.tmB, mapa_u32(smem_u32(&full_bar[st]), 0), p.wgt_tiled ? 0 : wk, brow,
-                                     p.wgt_tiled ? kEvictFirst : kEvictLast);
-                else
-                    tma_load_2d(dst_b, &p.tmB, &full_bar[st], p.wgt_tiled ? 0 : wk, brow,
-                                p.wgt_tiled ? kEvictFirst : kEvictLast);
+                const int brow = p.wgt_tiled ? (t.n_tile * p.kb_total + kb) * p.block_n : t.n_tile * p.block_n;
+                tma_load_2d(dst_b, &p.tmB, &full_bar[st], p.wgt_tiled ? 0 : wk, brow, p.wgt_tiled ? kEvictFirst : kEvictLast);
             };
             auto load_a = [&](const TileCoord& t, int kb, int st) {
                 int tap = kb / p.kc;
@@ -688,44 +716,34 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
                 }
                 void* dst_a = smem_a + st * kAStage;
                 const int r = tap / 3, s3 = tap - 3 * r;
-                if (kTwoCta) {
-                    const uint32_t fb = mapa_u32(smem_u32(&full_bar[st]), 0);
-                    if (p.mode == 0) tma_load_2d_pair(dst_a, tmA, fb, c, t.m_tile * kBM, kEvictNormal);
-                    else tma_load_4d_pair(dst_a, tmA, fb, c, t.w0 * p.stride + s3 - p.pad_lo, t.h0 * p.stride + r - p.pad_lo, t.n0,
-                                          kEvictNormal);
-                } else {
-                    if (p.mode == 0) tma_load_2d(dst_a, tmA, &full_bar[st], c, t.m_tile * kBM, kEvictNormal);
-                    else tma_load_4d(dst_a, tmA, &full_bar[st], c, t.w0 * p.stride + s3 - p.pad_lo,
-                                     t.h0 * p.stride + r - p.pad_lo, t.n0, kEvictNormal);
-                }
-            };
-            // both CTAs' loads of a pair are credited to the leader's full barrier: it sees 2 x tx_bytes per stage
-            auto arm = [&](int st) {
-                if (!kTwoCta) mbar_expect_tx(&full_bar[st], tx_bytes);
-                else if (cta_rank == 0) mbar_expect_tx(&full_bar[st], 2 * tx_bytes);
+                if (p.mode == 0) tma_load_2d(dst_a, tmA, &full_bar[st], c, t.m_tile * kBM, kEvictNormal);
+                else tma_load_4d(dst_a, tmA, &full_bar[st], c, t.w0 * p.stride + s3 - p.pad_lo,
+                                 t.h0 * p.stride + r - p.pad_lo, t.n0, kEvictNormal);
             };
             // ---- weight prefetch ahead of the grid dependency (constant weights only: pre-tiled B operands) ----
             int npre = 0;
             if (p.wgt_tiled && work0 < total_work) {
-                const TileCoord t = decode_work(p, work0, cta_rank);
+                const TileCoord t = decode_work(p, work0);
                 int kb0, kb1;
                 split_range(p, t.split, kb0, kb1);
                 npre = min(p.stages, kb1 - kb0);
                 for (int i = 0; i < npre; ++i) {
-                    arm(i);
+                    mbar_expect_tx(&full_bar[i], tx_bytes);
                     load_b(t, kb0 + i, i);
                 }
             }
             pdl_wait();
             int it = 0;  // k-blocks issued so far by this CTA
-            for (int work = work0; work < total_work; work += work_step) {
-                const TileCoord t = decode_work(p, work, cta_rank);
+            int iter = 0;
+            for (int work = work0; work < total_work; work += work_step, ++iter) {
+                const TileCoord t = decode_work(p, work);
                 int kb0, kb1;
                 split_range(p, t.split, kb0, kb1);
+                if (iter > 0) mbar_wait(acc_free, (iter - 1) & 1);  // the previous tile's epilogue left the stages
                 for (int kb = kb0; kb < kb1; ++kb, ++it) {
                     if (it >= npre) {
                         mbar_wait(&empty_bar[stage], phase ^ 1);
-                        arm(stage);
+                        mbar_expect_tx(&full_bar[stage], tx_bytes);
                         load_a(t, kb, stage);
                         load_b(t, kb, stage);
                     } else {
@@ -738,75 +756,31 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------- MMA issuer ---------------------------------
-        // a pair issues M = 256 (128 rows from each CTA) from the leader only; the peer's MMA warp idles
-        const uint32_t idesc = make_idesc_f16(kTwoCta ? 2 * kBM : kBM, p.block_n, 0, 0);
+    } else if (warp < kProducerWarp) {
+        // ------------------------- consumers: wgmma main loop, then the epilogue -------------------------
+        const int wg = warp >> 2;          // rows [64 wg, 64 wg + 64) of the tile in the main loop
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // accumulator rows r0, r0 + 8 of this thread
+        const int half = warp >> 2;        // epilogue: which of the two warps of a 32-row group; it takes every other chunk
+        const int row = (warp & 3) * 32 + lane;  // epilogue: the tile row this thread owns
+        const int tid_e = threadIdx.x;     // 0..255
+        const bool leader = (threadIdx.x & 127) == 0;
+        float acc[kR];
         int stage = 0;
         uint32_t phase = 0;
-        int iter = 0;
-        if (!kTwoCta || cta_rank == 0) {
-            for (int work = work0; work < total_work; work += work_step, ++iter) {
-                const TileCoord t = decode_work(p, work, cta_rank);
-                int kb0, kb1;
-                split_range(p, t.split, kb0, kb1);
-                const int as = p.acc_bufs == 2 ? (iter & 1) : 0;
-                const uint32_t aphase = (p.acc_bufs == 2 ? (iter >> 1) : iter) & 1;
-                mbar_wait(&tmem_empty[as], aphase ^ 1);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + as * p.acc_stride;
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smem_a + stage * kAStage), 1024, 0);
-                        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + stage * b_stage), 1024, 0);
-#pragma unroll
-                        for (int k = 0; k < kBK / 16; ++k) {
-                            // +32 B per K=16 step inside the 128 B swizzle row (start address is in 16 B units)
-                            if (kTwoCta)
-                                umma_f16_ss_pair(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                            else
-                                umma_f16_ss(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                        }
-                        if (kTwoCta) {  // release the stage / publish the accumulator in both CTAs
-                            umma_commit_pair(&empty_bar[stage], 3);
-                            if (kb == kb1 - 1) umma_commit_pair(&tmem_full[as], 3);
-                        } else {
-                            umma_commit(&empty_bar[stage]);
-                            if (kb == kb1 - 1) umma_commit(&tmem_full[as]);
-                        }
-                    }
-                    __syncwarp();
-                    if (++stage == p.stages) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-            }
-        }
-    } else {
-        // ------------------------------- epilogue -----------------------------------
-        const int lane_group = warp & 3;  // TMEM lanes [32*lane_group, +32) are accessible to this warp
-        const int half = (warp - 2) >> 2;  // which of the two warps of this lane quarter: it takes every other chunk
-        const int row = lane_group * 32 + lane;
-        const int tid_e = threadIdx.x - 64;  // 0..255 among the epilogue warps
-        int iter = 0;
         pdl_wait();  // bias / residual / output buffers belong to the stream order
-        for (int work = work0; work < total_work; work += work_step, ++iter) {
-            const TileCoord t = decode_work(p, work, cta_rank);
-            const int as = p.acc_bufs == 2 ? (iter & 1) : 0;
-            const uint32_t aphase = (p.acc_bufs == 2 ? (iter >> 1) : iter) & 1;
+        for (int work = work0; work < total_work; work += work_step) {
+            const TileCoord t = decode_work(p, work);
             const int ncol0 = t.n_tile * p.block_n;
             int out_row;
             const bool valid = tile_row(p, t, row, out_row);
-            // ---- operand prefetch, overlapped with this tile's main loop: bias -> smem, residual -> smem ----
-            epi_bar_sync();  // everyone is done reading the staging buffers of the previous tile
-            int bias_sel = 0;
+            int kb0, kb1;
+            split_range(p, t.split, kb0, kb1);
+            // ---- operand prefetch ahead of the main loop: bias -> smem, residual -> smem (cp.async) ----
+            int bias_sel = 0, img0 = 0;
             if (p.bias_mode == 1) {
                 int row0;
                 tile_row(p, t, 0, row0);
-                const int img0 = p.bias_rows > 0 ? row0 / p.bias_rows : 0;
+                img0 = p.bias_rows > 0 ? row0 / p.bias_rows : 0;
                 const int nvec = p.bias_rows > 0 ? (p.M + p.bias_rows - 1) / p.bias_rows : 1;
                 for (int c = tid_e; c < 2 * p.block_n; c += kEpiThreads) {
                     const int which = c >= p.block_n ? 1 : 0;
@@ -822,7 +796,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
             if (p.ln_parts != 0)
                 for (int c = tid_e; c < p.block_n; c += kEpiThreads) wg_s[c] = (ncol0 + c < p.N) ? p.ln_wg[ncol0 + c] : 0.f;
             uint4 res_pre[4];
-            if (kStaged) staged_load_residual(p, t, staged_map(p, t, lane), warp - 2, 0, res_pre);
+            if (kStaged) staged_load_residual(p, t, staged_map(p, t, lane), warp, 0, res_pre);
             if (p.res_smem) {
                 const int vpr = p.block_n >> 3;  // 16-byte vectors per tile row
                 for (int i = tid_e; i < kBM * vpr; i += kEpiThreads) {
@@ -833,96 +807,86 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
                 }
             }
             const int bias_base = (p.bias_mode == 2 && p.bias_rows > 0 && valid) ? (out_row / p.bias_rows) * p.bias_stride : 0;
-            mbar_wait(&tmem_full[as], aphase);
-            tc_fence_after();
+
+            gemm_mainloop(p, acc, smem_a, smem_b, b_stage, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
+
             if (p.res_smem) cp_async_wait_all();
-            epi_bar_sync();  // staged bias / residual visible to all epilogue threads
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_group * 32) << 16) + as * p.acc_stride;
+            epi_bar_sync();  // every wgmma of the tile retired: the stages may be overwritten; staged operands visible
             if (kStaged) {
                 // staging tile: over the drained pipeline stages when this CTA has no further tile, else dedicated
                 __half* tile_s = p.stage_dedicated ? res_s : reinterpret_cast<__half*>(smem);
                 float* scratch = reinterpret_cast<float*>(tile_s + kBM * (p.block_n + 8));
-                staged_epilogue(p, t, taddr, tile_s, scratch, flag_s,
-                                p.bias_mode == 1 ? bias_s + bias_sel * p.block_n : nullptr, wg_s, warp - 2, lane, row,
-                                out_row, valid, res_pre);
-                tc_fence_before();
-                mbar_arrive(&tmem_empty[as]);
-                continue;
-            }
-            const float2 lnc = ln_row_coeffs(p, out_row, valid);
-            float2 rowacc = make_float2(0.f, 0.f);
-            auto process16 = [&](float (&acc)[16], int c) {  // c: column offset inside the tile
-                if (p.ln_parts != 0) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) acc[j] = fmaf(acc[j], lnc.x, lnc.y * wg_s[c + j]);
+                const float* b0 = nullptr;
+                const float* b1 = nullptr;
+                if (p.bias_mode == 1) {
+                    int o0, o1;
+                    const bool v0 = tile_row(p, t, r0, o0), v1 = tile_row(p, t, r0 + 8, o1);
+                    const int s0 = (p.bias_rows > 0 && v0) ? min(1, max(0, o0 / p.bias_rows - img0)) : 0;
+                    const int s1 = (p.bias_rows > 0 && v1) ? min(1, max(0, o1 / p.bias_rows - img0)) : 0;
+                    b0 = bias_s + s0 * p.block_n, b1 = bias_s + s1 * p.block_n;
                 }
-                const float* bptr = nullptr;
-                if (p.bias_mode == 1) bptr = bias_s + bias_sel * p.block_n + c;
-                else if (kGeneric && p.bias_mode == 2) bptr = p.bias + bias_base + ncol0 + c;
-                const __half* rptr = nullptr;
-                if (p.res_smem) rptr = res_s + row * ldr + c;
-                else if (kGeneric && p.residual != nullptr)
-                    rptr = p.residual + static_cast<size_t>(out_row) * p.n_store + ((ncol0 + c) >> (p.geglu ? 1 : 0));
-                epilogue_store16<kGeneric, kGeglu, kOutF32, kPartial>(p, acc, out_row, ncol0 + c, t.split, bptr, rptr, rowacc);
-            };
-            auto process32 = [&](const uint32_t (&v)[32], int c) {
-                if (kPartial && p.cluster) {
-                    // fp32 accumulators -> this CTA's shared memory (over the drained pipeline stages); row stride
-                    // block_n + 4 floats keeps the 32 rows of a warp on distinct banks
-                    float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(smem) + row * (p.block_n + 4) + c);
+                stage_accumulators(p, t, acc, tile_s, b0, b1, wg_s, r0, lane);
+                staged_epilogue(p, t, tile_s, scratch, flag_s, warp, lane, res_pre);
+            } else {
+                park_accumulators(acc, p.block_n, acc_s, lda, r0, lane);
+                epi_bar_sync();
+                if (!(kPartial && p.cluster)) {  // cluster split-K: the parked tile is what the peers reduce
+                    const float* arow = acc_s + row * lda;
+                    const float2 lnc = ln_row_coeffs(p, out_row, valid);
+                    float2 rowacc = make_float2(0.f, 0.f);
+                    auto process16 = [&](float (&a16)[16], int c) {  // c: column offset inside the tile
+                        if (p.ln_parts != 0) {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        dst[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                             __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                    return;
-                }
-                if (!valid) return;
+                            for (int j = 0; j < 16; ++j) a16[j] = fmaf(a16[j], lnc.x, lnc.y * wg_s[c + j]);
+                        }
+                        const float* bptr = nullptr;
+                        if (p.bias_mode == 1) bptr = bias_s + bias_sel * p.block_n + c;
+                        else if (kGeneric && p.bias_mode == 2) bptr = p.bias + bias_base + ncol0 + c;
+                        const __half* rptr = nullptr;
+                        if (p.res_smem) rptr = res_s + row * ldr + c;
+                        else if (kGeneric && p.residual != nullptr)
+                            rptr = p.residual + static_cast<size_t>(out_row) * p.n_store + ((ncol0 + c) >> (p.geglu ? 1 : 0));
+                        epilogue_store16<kGeneric, kGeglu, kOutF32, kPartial>(p, a16, out_row, ncol0 + c, t.split, bptr, rptr, rowacc);
+                    };
+                    auto process32 = [&](const uint32_t (&v)[32], int c) {
+                        if (!valid) return;
 #pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    if (ncol0 + c + 16 * hh < p.N) {
-                        float acc[16];
+                        for (int hh = 0; hh < 2; ++hh) {
+                            if (ncol0 + c + 16 * hh < p.N) {
+                                float a16[16];
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) acc[j] = __uint_as_float(v[16 * hh + j]);
-                        process16(acc, c + 16 * hh);
+                                for (int j = 0; j < 16; ++j) a16[j] = __uint_as_float(v[16 * hh + j]);
+                                process16(a16, c + 16 * hh);
+                            }
+                        }
+                    };
+                    if (!kGeneric || (p.block_n & 31) == 0) {
+                        // this warp's 32-column chunks: half, half+2, ...
+                        for (int c = 32 * half; c < p.block_n; c += 64) {
+                            uint32_t va[32];
+                            acc_ld32(arow + c, va);
+                            process32(va, c);
+                        }
+                    } else if (kGeneric) {
+                        for (int c = 16 * half; c < p.block_n; c += 32) {
+                            uint32_t v[16];
+                            acc_ld16(arow + c, v);
+                            if (valid && ncol0 + c < p.N) {
+                                float a16[16];
+#pragma unroll
+                                for (int j = 0; j < 16; ++j) a16[j] = __uint_as_float(v[j]);
+                                process16(a16, c);
+                            }
+                        }
                     }
-                }
-            };
-            if (!kGeneric || (p.block_n & 31) == 0) {
-                // this warp's 32-column chunks: half, half+2, ...; software-pipelined (the TMEM load of the next
-                // chunk is in flight while the current one is converted and stored)
-                uint32_t va[32], vb[32];
-                int c = 32 * half;
-                if (c < p.block_n) tmem_ld32(taddr + c, va);
-                while (c < p.block_n) {
-                    tmem_ld_wait();
-                    const int c2 = c + 64;
-                    if (c2 < p.block_n) tmem_ld32(taddr + c2, vb);
-                    process32(va, c);
-                    if (c2 >= p.block_n) break;
-                    tmem_ld_wait();
-                    const int c3 = c2 + 64;
-                    if (c3 < p.block_n) tmem_ld32(taddr + c3, va);
-                    process32(vb, c2);
-                    c = c3;
-                }
-            } else if (kGeneric) {
-                for (int c = 16 * half; c < p.block_n; c += 32) {
-                    uint32_t v[16];
-                    tmem_ld16(taddr + c, v);
-                    tmem_ld_wait();
-                    if (valid && ncol0 + c < p.N) {
-                        float acc[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) acc[j] = __uint_as_float(v[j]);
-                        process16(acc, c);
-                    }
+                    if (!kPartial && p.rs_out != nullptr && valid)  // one partial per (n_tile, column half): 2 * n_tiles parts
+                        *reinterpret_cast<float2*>(p.rs_out + (static_cast<size_t>(t.n_tile * 2 + half) * p.M + out_row) * 2) = rowacc;
                 }
             }
-            if (!kPartial && p.rs_out != nullptr && valid)  // one partial per (n_tile, column half): 2 * n_tiles parts
-                *reinterpret_cast<float2*>(p.rs_out + (static_cast<size_t>(t.n_tile * 2 + half) * p.M + out_row) * 2) = rowacc;
-            tc_fence_before();
-            if (kTwoCta) mbar_arrive_cluster(mapa_u32(smem_u32(&tmem_empty[as]), 0));  // the leader's MMA warp waits
-            else mbar_arrive(&tmem_empty[as]);
+            // generic-proxy accesses of the staging / accumulator tiles are ordered before the producer's next TMA writes
+            fence_proxy_async_smem();
+            epi_bar_sync();  // everyone is done with the accumulator / staging tiles and the staged bias / residual
+            if (threadIdx.x == 0) mbar_arrive(acc_free);
         }
     }
 
@@ -931,7 +895,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
         // sums its 1/splits slice of the tile over all peers through DSMEM in rank order (deterministic), applies
         // bias / residual / conversion and stores it.  No workspace round trip, no second launch. ----
         __syncwarp();
-        pdl_wait();  // (warps 0 / 1: the reduction below reads bias / residual and writes the output)
+        pdl_wait();  // (the producer warp: the reduction below reads bias / residual and writes the output)
         cluster_sync_all();
         const TileCoord t = decode_work(p, blockIdx.x);
         const int ncol0 = t.n_tile * p.block_n;
@@ -947,42 +911,33 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
             int orow;
             if (!tile_row(p, t, r, orow) || col >= p.N) continue;
             const uint32_t la = red_base + static_cast<uint32_t>(r * ldred + c4 * 4) * 4u;
-            float4 acc = ld_dsmem_f4(la, 0);
+            float4 a4 = ld_dsmem_f4(la, 0);
             for (int sp = 1; sp < p.splits; ++sp) {
                 const float4 v = ld_dsmem_f4(la, sp);
-                acc.x += v.x, acc.y += v.y, acc.z += v.z, acc.w += v.w;
+                a4.x += v.x, a4.y += v.y, a4.z += v.z, a4.w += v.w;
             }
             if (p.bias != nullptr) {
                 const float4 b = *reinterpret_cast<const float4*>(
                     p.bias + (p.bias_rows > 0 ? (orow / p.bias_rows) * p.bias_stride : 0) + col);
-                acc.x += b.x, acc.y += b.y, acc.z += b.z, acc.w += b.w;
+                a4.x += b.x, a4.y += b.y, a4.z += b.z, a4.w += b.w;
             }
             const size_t off = static_cast<size_t>(orow) * p.N + col;
             if (p.residual != nullptr) {
                 const uint2 rr = *reinterpret_cast<const uint2*>(p.residual + off);
-                const float2 r0 = __half22float2(*reinterpret_cast<const __half2*>(&rr.x));
-                const float2 r1 = __half22float2(*reinterpret_cast<const __half2*>(&rr.y));
-                acc.x += r0.x, acc.y += r0.y, acc.z += r1.x, acc.w += r1.y;
+                const float2 q0 = __half22float2(*reinterpret_cast<const __half2*>(&rr.x));
+                const float2 q1 = __half22float2(*reinterpret_cast<const __half2*>(&rr.y));
+                a4.x += q0.x, a4.y += q0.y, a4.z += q1.x, a4.w += q1.y;
             }
             if (p.out_f32) {
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + off) = acc;
+                *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + off) = a4;
             } else {
                 uint2 pk;
-                pk.x = pack_half2(acc.x, acc.y);
-                pk.y = pack_half2(acc.z, acc.w);
+                pk.x = pack_half2(a4.x, a4.y);
+                pk.y = pack_half2(a4.z, a4.w);
                 *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + off) = pk;
             }
         }
         cluster_sync_all();  // nobody leaves (or frees its shared memory) while a peer may still read it
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (kTwoCta) cluster_arrive_wait();  // the pair retires together: remote barrier arrivals, peer smem / TMEM reads
-    if (warp == 1) {
-        tc_fence_after();
-        if (kTwoCta) tmem_dealloc_pair(tmem_base, 512);
-        else tmem_dealloc(tmem_base, static_cast<uint32_t>(p.tmem_cols));
     }
 }
 
@@ -994,13 +949,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
 // The image is walked in padded-linear order q = y * (W + 1) + x (one shared zero column between image rows), so the
 // input of output position q for tap (dy, dx) is position q + dy * (W + 1) + dx: every tap of a 128-position tile is
 // the SAME shared-memory patch read from a row-shifted start address.  Per 64-channel chunk:
-//   warps 2..9  load the (rows + 2) x (W + 1) pixel patch ONCE with plain 16-byte loads, apply x * sc[n, c] + sh[n, c]
-//               (GroupNorm with the statistics its producer left behind) and SiLU in registers, and store it in the
-//               128-byte-swizzled K-major layout the tensor core reads (zero rows for the padding / pad column);
-//   warp 0      streams the nine [block_n x 64] weight tiles of the chunk with TMA;
-//   warp 1      issues 9 x 4 tcgen05.mma whose A descriptors start at patch + s_tap * 128 bytes.
+//   warps 0..7  (two consumer warpgroups) issue 9 x 4 wgmma per warpgroup whose A descriptors start at
+//               patch + (s_tap + 64 wg) * 128 bytes, and between the taps load the NEXT chunk's (rows + 2) x (W + 1)
+//               pixel patch with plain 16-byte loads, apply x * sc[n, c] + sh[n, c] (GroupNorm with the statistics its
+//               producer left behind) and SiLU in registers, and store it in the 128-byte-swizzled K-major layout the
+//               tensor core reads (zero rows for the padding / pad column) into the other patch buffer;
+//   warp 8      streams the nine [block_n x 64] weight tiles of the chunk with TMA.
 // One activation byte enters shared memory once per chunk instead of nine times, is normalised once, and the
-// standalone GroupNorm launch (and its round trip through L2) disappears.  Warps 2..9 then run the staged epilogue.
+// standalone GroupNorm launch (and its round trip through L2) disappears.  Warps 0..7 then run the epilogue.
 // =====================================================================================================================
 __device__ __forceinline__ float silu_fast(float y) {
     // y * sigmoid(y) with sigmoid(y) = 0.5 * tanh(0.5 y) + 0.5: one MUFU op per element (the patch transform is MUFU
@@ -1019,8 +975,9 @@ __device__ __forceinline__ void ldr_bar_sync() { asm volatile("bar.sync 1, 256;"
 
 // kKind 0: loader warps + staged epilogue (GroupNorm / upsample on the patch, column statistics);  1: loader warps + tiny
 // fp32 epilogue (conv_out);  2: plain convolution -- the producer warp fetches each patch with one TMA box (hardware zero
-// fill for the padding ring and the pad column) and the eight epilogue warps use the register epilogue of the GEMM kernel.
-template <int kKind>
+// fill for the padding ring and the pad column) and the consumer warps use the register epilogue of the GEMM kernel.
+// kR: accumulator registers per consumer thread (block_n / 2): the loader kinds hold the patch vectors in registers too.
+template <int kKind, int kR>
 __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid_constant__ GemmParams p) {
     constexpr bool kFp32Direct = kKind == 1;
     constexpr bool kTmaPatch = kKind == 2;
@@ -1037,19 +994,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid
     uint64_t* empty_b = full_b + kHaloMaxStages;
     uint64_t* full_a = empty_b + kHaloMaxStages;            // [2]
     uint64_t* empty_a = full_a + 2;                         // [2]
-    uint64_t* tmem_full = empty_a + 2;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    float* bias_s = reinterpret_cast<float*>(tmem_ptr + 4);               // [256]
+    uint64_t* acc_free = empty_a + 2;                       // the patch / weight memory is free for the next tile
+    float* bias_s = reinterpret_cast<float*>(acc_free + 4);               // [256]
     unsigned int* flag_s = reinterpret_cast<unsigned int*>(bias_s + 256);   // [8]
     float2* stat_s = reinterpret_cast<float2*>(flag_s + 16);              // [64] (mean, rstd) per group
     float2* scsh = stat_s + 64;                                           // [C0 + C1] (scale, shift) per channel
     const int Cin = p.C0 + p.C1;
     __half* stage_tile = reinterpret_cast<__half*>(scsh + ((Cin + 7) & ~7));  // dedicated staging tile (if any)
+    float* acc_s = reinterpret_cast<float*>(smem);          // fp32 accumulator tile over the drained patches / stages
+    const int lda = p.block_n + 4;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         prefetch_tmap(&p.tmB);
         if (kTmaPatch) {
             prefetch_tmap(&p.tmA0);
@@ -1057,43 +1014,29 @@ __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid
         }
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(&full_b[s], 1);
-            mbar_init(&empty_b[s], 1);
+            mbar_init(&empty_b[s], 2);
         }
         for (int s = 0; s < 2; ++s) {
-            mbar_init(&full_a[s], kTmaPatch ? 1 : kEpiThreads);
-            mbar_init(&empty_a[s], 1);
-            mbar_init(&tmem_full[s], 1);
-            mbar_init(&tmem_empty[s], kEpiThreads);
+            mbar_init(&full_a[s], 1);
+            mbar_init(&empty_a[s], 2);
         }
+        mbar_init(acc_free, 1);
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr, static_cast<uint32_t>(p.tmem_cols));
-        tmem_relinquish();
-    }
-    if (threadIdx.x >= 64 && threadIdx.x < 80) {  // "pixel -1" of both patches: the zero pad column that precedes the patch
-        const int which = (threadIdx.x - 64) >> 3;
-        *reinterpret_cast<uint4*>(patch + which * p.patch_bytes + 7 * 128 + (threadIdx.x & 7) * 16) = make_uint4(0, 0, 0, 0);
-        fence_proxy_async_smem();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     pdl_trigger();
-    if (threadIdx.x == 64) dbg_mark(p, 0);
 
     const int total_work = p.m_tiles * p.n_tiles;
     const int work0 = blockIdx.x, work_step = gridDim.x;
     const int kc = p.kc;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ------------------------------- weight producer (TMA; constant data: no grid dependency) -------------------
         if (lane == 0) {
-            int it = 0;
+            int it = 0, iter = 0;
             // kTmaPatch: this thread also fetches the activation patches, one chunk ahead of the weight tiles that use
-            // them (two patch buffers): the next patch is requested as soon as its buffer is free, checked without
-            // blocking between weight tiles so the weight ring never drains behind a patch wait
+            // them (two patch buffers): the next patch of the tile is requested as soon as its buffer is free, checked
+            // without blocking between weight tiles so the weight ring never drains behind a patch wait
             int ci = 0, pai = 0, pwork = work0, pj = 0;
             auto issue_patch = [&](bool blocking) -> bool {
                 const int pa = pai & 1;
@@ -1110,12 +1053,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid
                 return true;
             };
             if (kTmaPatch) pdl_wait();  // the activations are the previous kernel's output
-            for (int work = work0; work < total_work; work += work_step) {
+            for (int work = work0; work < total_work; work += work_step, ++iter) {
                 const TileCoord t = decode_work(p, work);
+                if (iter > 0) mbar_wait(acc_free, (iter - 1) & 1);  // the previous tile's epilogue left the buffers
                 for (int j = 0; j < kc; ++j, ++ci) {
                     if (kTmaPatch && pai == ci) issue_patch(true);
                     for (int tap = 0; tap < p.taps; ++tap, ++it) {
-                        if (kTmaPatch && pai == ci + 1 && pwork < total_work) issue_patch(false);
+                        if (kTmaPatch && pai == ci + 1 && pwork == work) issue_patch(false);
                         const int st = it % p.stages;
                         const uint32_t ph = (it / p.stages) & 1;
                         mbar_wait(&empty_b[st], ph ^ 1);
@@ -1126,90 +1070,46 @@ __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------- MMA issuer -------------------------------------------------------------------
-        const uint32_t idesc = make_idesc_f16(kBM, p.block_n, 0, 0);
-        int it = 0, ait = 0, iter = 0;
-        for (int work = work0; work < total_work; work += work_step, ++iter) {
-            const TileCoord t = decode_work(p, work);
-            const int as = p.acc_bufs == 2 ? (iter & 1) : 0;
-            const uint32_t aphase = (p.acc_bufs == 2 ? (iter >> 1) : iter) & 1;
-            mbar_wait(&tmem_empty[as], aphase ^ 1);
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * p.acc_stride;
-            for (int j = 0; j < kc; ++j, ++ait) {
-                const int pa = ait & 1;
-                mbar_wait(&full_a[pa], (ait >> 1) & 1);
-                tc_fence_after();
-                if (lane == 0 && j < 24) dbg_mark(p, 64 + 2 * j);
-                const uint32_t pbase = smem_u32(patch + pa * p.patch_bytes) + 1024;
-                for (int tap = 0; tap < p.taps; ++tap, ++it) {
-                    const int st = it % p.stages;
-                    mbar_wait(&full_b[st], (it / p.stages) & 1);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const int dy = p.taps == 9 ? tap / 3 - 1 : 0, dx = p.taps == 9 ? tap - (tap / 3) * 3 - 1 : 0;
-                        // patch pixel of the tile's first output position for this tap (>= -1)
-                        const int srow = t.c0 + dy * p.Wp + dx;
-                        const uint32_t a_addr = pbase + srow * 128;
-                        // start address shifted by whole 128-byte rows inside the 1024-byte swizzle atom (the patch was
-                        // written in the absolute-address swizzle pattern of a 1024-byte aligned buffer)
-                        const uint64_t adesc = make_smem_desc_sw128(a_addr, 1024, 0) |
-                                               (static_cast<uint64_t>(p.desc_bo ? ((a_addr >> 7) & 7) : 0) << 49);
-                        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + st * b_stage), 1024, 0);
-#pragma unroll
-                        for (int k = 0; k < kBK / 16; ++k)
-                            umma_f16_ss(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (j > 0 || tap > 0 || k > 0) ? 1u : 0u);
-                        umma_commit(&empty_b[st]);
-                        if (tap == p.taps - 1) {
-                            umma_commit(&empty_a[pa]);
-                            if (j == kc - 1) umma_commit(&tmem_full[as]);
-                            if (j < 24) dbg_mark(p, 65 + 2 * j);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else {
-        // ------------------------------- loader / transform warps, then epilogue ---------------------------------------
-        const int ltid = threadIdx.x - 64;
-        const int ew = warp - 2;
-        const int lane_group = warp & 3;
-        const int row = lane_group * 32 + lane;
+    } else if (warp < kProducerWarp) {
+        // --------------------- consumers: patch loader / transform, wgmma, epilogue ---------------------
+        const int ltid = threadIdx.x;
+        const int ew = warp;
+        const int wg = warp >> 2;
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // accumulator rows r0, r0 + 8 of this thread
+        const int row = (warp & 3) * 32 + lane;                   // epilogue: the tile row this thread owns
+        const bool leader = (threadIdx.x & 127) == 0;
         const bool gn = p.gn_gamma != nullptr;
         const bool ups = p.upsample != 0;
         const int Hs = ups ? (p.H >> 1) : p.H, Ws = ups ? (p.W >> 1) : p.W;
+        float acc[kR];
+        if (ltid == 0) dbg_mark(p, 0);
         pdl_wait();
         if (ltid == 0) dbg_mark(p, 1);
-        int cur_img = -1, ait = 0, iter = 0;
-        for (int work = work0; work < total_work; work += work_step, ++iter) {
+        int cur_img = -1, ait = 0, it = 0;
+        for (int work = work0; work < total_work; work += work_step) {
             const TileCoord t = decode_work(p, work);
             const int img = t.n0;
             const int ya = t.ya, xa = t.xa;
-            if (!kTmaPatch) {
-            // ---- operand patches: one per 64-channel chunk ----
+            const int ncol0 = t.n_tile * p.block_n;
+            if (p.bias != nullptr) {
+                const float* bsrc = p.bias + (p.bias_rows > 0 ? static_cast<size_t>(img) * p.bias_stride : 0);
+                for (int c = ltid; c < p.block_n; c += kEpiThreads) bias_s[c] = (ncol0 + c < p.N) ? bsrc[ncol0 + c] : 0.f;
+            }
+            if (ltid < 16) {  // "pixel -1" of both patches: the zero pad column that precedes the patch
+                const int which = ltid >> 3;
+                *reinterpret_cast<uint4*>(patch + which * p.patch_bytes + 7 * 128 + (ltid & 7) * 16) = make_uint4(0, 0, 0, 0);
+            }
+            // ---- operand patches (loader kinds): one per 64-channel chunk ----
             // Thread t always handles vector (t & 7) of the patch pixels t / 8, t / 8 + 32, ...: pixel offsets and
             // shared-memory destinations are computed once per tile, the eight (scale, shift) pairs once per chunk, and
             // the raw vectors of chunk j + 1 are requested while chunk j is being normalised (one register set: a slot is
             // refilled as soon as its vector has been consumed), so the L2 latency hides behind the transform.
-            constexpr int NBMAX = 12;
+            constexpr int NBMAX = kTmaPatch ? 1 : 12;
             const int nvec = p.patch_rows * p.Wp * 8;
             const int nb = (nvec + kEpiThreads - 1) / kEpiThreads;
             const int jj = ltid & 7;
             int soff[NBMAX], doff[NBMAX];
-#pragma unroll
-            for (int i = 0; i < NBMAX; ++i) {
-                const int v = ltid + kEpiThreads * i;
-                const int pi = v >> 3;
-                const int prow = (pi * p.inv_wp) >> 20;
-                const int yy = ya + prow, xx = xa + (pi - prow * p.Wp);
-                const bool in_patch = i < nb && v < nvec;
-                const bool ok = in_patch && yy >= 0 && yy < p.H && xx >= 0 && xx < p.W;
-                const int ys = ups ? (yy >> 1) : yy, xs = ups ? (xx >> 1) : xx;
-                soff[i] = ok ? (ys * Ws + xs) : -1;
-                doff[i] = in_patch ? pi * 128 + ((jj ^ (pi & 7)) << 4) : -1;
-            }
+            uint4 regs[NBMAX];
             auto chunk_src = [&](int j, int& csrc) -> const __half* {
                 const bool src1 = j >= p.kc0;
                 const int cbase = (src1 ? j - p.kc0 : j) * kBK + jj * 8;
@@ -1217,72 +1117,28 @@ __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid
                 if (cbase >= csrc) return nullptr;  // ragged last chunk: channels beyond the source are zeros
                 return (src1 ? p.a1 : p.a0) + static_cast<size_t>(img) * Hs * Ws * csrc + cbase;
             };
-            uint4 regs[NBMAX];
-            {
-                int csrc;
-                const __half* src = chunk_src(0, csrc);
-#pragma unroll
-                for (int i = 0; i < NBMAX; ++i) {
-                    regs[i] = make_uint4(0, 0, 0, 0);
-                    if (src != nullptr && soff[i] >= 0)
-                        regs[i] = __ldg(reinterpret_cast<const uint4*>(src + static_cast<size_t>(soff[i]) * csrc));
-                }
-            }
-            if (ltid == 0) dbg_mark(p, 2);
-            // (the first chunk's vectors are already in flight while the coefficient table is built)
-            if (gn && img != cur_img) {
-                // ---- GroupNorm coefficients of this image: group statistics from the producers' per-channel sums ----
-                const int cpg = Cin / p.gn_groups;
-                const float inv_cnt = 1.0f / (static_cast<float>(cpg) * static_cast<float>(p.gn_hw));
-                ldr_bar_sync();  // previous tile's readers of the table are done
-                // eight lanes per group, all groups of a round in flight at once (one L2 round trip for <= 32 groups)
-                for (int g = ltid >> 3; g < p.gn_groups; g += kEpiThreads >> 3) {
-                    float s = 0.f, q = 0.f;
-                    for (int c = g * cpg + (ltid & 7); c < (g + 1) * cpg; c += 8) {
-                        const float2 v = (c < p.C0)
-                            ? __ldg(reinterpret_cast<const float2*>(p.gn_chan0 + (static_cast<size_t>(img) * p.C0 + c) * 2))
-                            : __ldg(reinterpret_cast<const float2*>(p.gn_chan1 + (static_cast<size_t>(img) * p.C1 + c - p.C0) * 2));
-                        s += v.x, q += v.y;
-                    }
-#pragma unroll
-                    for (int o = 4; o > 0; o >>= 1) {
-                        s += __shfl_xor_sync(0xffffffffu, s, o);
-                        q += __shfl_xor_sync(0xffffffffu, q, o);
-                    }
-                    if ((ltid & 7) == 0) {
-                        const float mean = s * inv_cnt;
-                        stat_s[g] = make_float2(mean, rsqrtf(fmaxf(q * inv_cnt - mean * mean, 0.f) + p.gn_eps));
-                    }
-                }
-                ldr_bar_sync();
-                for (int c = ltid; c < Cin; c += kEpiThreads) {
-                    const float2 st = stat_s[c / cpg];
-                    const float sc = p.gn_gamma[c] * st.y;
-                    scsh[c] = make_float2(sc, fmaf(-st.x, sc, p.gn_beta[c]));
-                }
-                ldr_bar_sync();
-                cur_img = img;
-            }
-            for (int j = 0; j < kc; ++j, ++ait) {
-                const int pa = ait & 1;
-                const bool src1 = j >= p.kc0;
+            // per-chunk state of the transform of chunk `tj`
+            float4 cf[4];
+            bool chan_ok = false;
+            int csrc_nxt = 0;
+            const __half* nsrc = nullptr;
+            auto transform_begin = [&](int tj) {
+                const bool src1 = tj >= p.kc0;
                 int csrc_cur;
-                const bool chan_ok = chunk_src(j, csrc_cur) != nullptr;
-                int csrc_nxt = 0;
-                const __half* nsrc = (j + 1 < kc) ? chunk_src(j + 1, csrc_nxt) : nullptr;
-                float4 cf[4];  // (scale, shift) of this thread's eight channels
+                chan_ok = chunk_src(tj, csrc_cur) != nullptr;
+                nsrc = (tj + 1 < kc) ? chunk_src(tj + 1, csrc_nxt) : nullptr;
                 if (gn) {
-                    const float2* tab = scsh + (src1 ? p.C0 : 0) + (src1 ? j - p.kc0 : j) * kBK + jj * 8;
+                    const float2* tab = scsh + (src1 ? p.C0 : 0) + (src1 ? tj - p.kc0 : tj) * kBK + jj * 8;
 #pragma unroll
                     for (int q = 0; q < 4; ++q) cf[q] = chan_ok ? *reinterpret_cast<const float4*>(tab + 2 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
                 }
-                if (ltid == 0 && j == 0) dbg_mark(p, 3);
-                mbar_wait(&empty_a[pa], ((ait >> 1) & 1) ^ 1);
-                if (ltid == 0 && j < 24) dbg_mark(p, 8 + 2 * j);
+            };
+            // the vectors i with i % nslices == slice of chunk `tj` into patch buffer `pa`
+            auto transform_slice = [&](int pa, int slice, int nslices) {
                 uint8_t* pbase = patch + pa * p.patch_bytes + 1024;
 #pragma unroll
                 for (int i = 0; i < NBMAX; ++i) {
-                    if (doff[i] < 0) continue;
+                    if (doff[i] < 0 || i % nslices != slice) continue;
                     uint4 val = regs[i];
                     const bool live = soff[i] >= 0;
                     regs[i] = make_uint4(0, 0, 0, 0);
@@ -1300,96 +1156,183 @@ __global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid
                     }
                     *reinterpret_cast<uint4*>(pbase + doff[i]) = val;
                 }
-                fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
-                mbar_arrive(&full_a[pa]);
-                if (ltid == 0 && j < 24) dbg_mark(p, 9 + 2 * j);
+            };
+            if (!kTmaPatch) {
+#pragma unroll
+                for (int i = 0; i < NBMAX; ++i) {
+                    const int v = ltid + kEpiThreads * i;
+                    const int pi = v >> 3;
+                    const int prow = (pi * p.inv_wp) >> 20;
+                    const int yy = ya + prow, xx = xa + (pi - prow * p.Wp);
+                    const bool in_patch = i < nb && v < nvec;
+                    const bool ok = in_patch && yy >= 0 && yy < p.H && xx >= 0 && xx < p.W;
+                    const int ys = ups ? (yy >> 1) : yy, xs = ups ? (xx >> 1) : xx;
+                    soff[i] = ok ? (ys * Ws + xs) : -1;
+                    doff[i] = in_patch ? pi * 128 + ((jj ^ (pi & 7)) << 4) : -1;
+                }
+                {
+                    int csrc;
+                    const __half* src = chunk_src(0, csrc);
+#pragma unroll
+                    for (int i = 0; i < NBMAX; ++i) {
+                        regs[i] = make_uint4(0, 0, 0, 0);
+                        if (src != nullptr && soff[i] >= 0)
+                            regs[i] = __ldg(reinterpret_cast<const uint4*>(src + static_cast<size_t>(soff[i]) * csrc));
+                    }
+                }
+                if (ltid == 0) dbg_mark(p, 2);
+                // (the first chunk's vectors are already in flight while the coefficient table is built)
+                if (gn && img != cur_img) {
+                    // ---- GroupNorm coefficients of this image: group statistics from the producers' per-channel sums ----
+                    const int cpg = Cin / p.gn_groups;
+                    const float inv_cnt = 1.0f / (static_cast<float>(cpg) * static_cast<float>(p.gn_hw));
+                    ldr_bar_sync();  // previous tile's readers of the table are done
+                    // eight lanes per group, all groups of a round in flight at once (one L2 round trip for <= 32 groups)
+                    for (int g = ltid >> 3; g < p.gn_groups; g += kEpiThreads >> 3) {
+                        float s = 0.f, q = 0.f;
+                        for (int c = g * cpg + (ltid & 7); c < (g + 1) * cpg; c += 8) {
+                            const float2 v = (c < p.C0)
+                                ? __ldg(reinterpret_cast<const float2*>(p.gn_chan0 + (static_cast<size_t>(img) * p.C0 + c) * 2))
+                                : __ldg(reinterpret_cast<const float2*>(p.gn_chan1 + (static_cast<size_t>(img) * p.C1 + c - p.C0) * 2));
+                            s += v.x, q += v.y;
+                        }
+#pragma unroll
+                        for (int o = 4; o > 0; o >>= 1) {
+                            s += __shfl_xor_sync(0xffffffffu, s, o);
+                            q += __shfl_xor_sync(0xffffffffu, q, o);
+                        }
+                        if ((ltid & 7) == 0) {
+                            const float mean = s * inv_cnt;
+                            stat_s[g] = make_float2(mean, rsqrtf(fmaxf(q * inv_cnt - mean * mean, 0.f) + p.gn_eps));
+                        }
+                    }
+                    ldr_bar_sync();
+                    for (int c = ltid; c < Cin; c += kEpiThreads) {
+                        const float2 st = stat_s[c / cpg];
+                        const float sc = p.gn_gamma[c] * st.y;
+                        scsh[c] = make_float2(sc, fmaf(-st.x, sc, p.gn_beta[c]));
+                    }
+                    ldr_bar_sync();
+                    cur_img = img;
+                }
+                if (ltid == 0) dbg_mark(p, 8);
+                transform_begin(0);
+                transform_slice(ait & 1, 0, 1);
             }
-            }  // !kTmaPatch
+            fence_proxy_async_smem();  // generic-proxy writes (patch, pad column) -> visible to the tensor core
+            epi_bar_sync();
+            if (ltid == 0) {
+                if (!kTmaPatch) dbg_mark(p, 9);  // loader: chunk 0 stored
+                dbg_mark(p, 3);
+            }
+            // ---- main loop: chunks x taps; the loader kinds transform chunk j + 1 between the taps of chunk j ----
+            for (int j = 0; j < kc; ++j, ++ait) {
+                const int pa = ait & 1;
+                if (kTmaPatch) mbar_wait(&full_a[pa], (ait >> 1) & 1);
+                const bool more = !kTmaPatch && j + 1 < kc;
+                if (ltid == 0 && j < 24) dbg_mark(p, 64 + 2 * j);
+                if (more) {
+                    if (ltid == 0 && j < 23) dbg_mark(p, 10 + 2 * j);  // loader: chunk j + 1 begins
+                    transform_begin(j + 1);
+                }
+                const uint32_t pbase = smem_u32(patch + pa * p.patch_bytes) + 1024;
+                int prev = -1;
+                for (int tap = 0; tap < p.taps; ++tap, ++it) {
+                    const int st = it % p.stages;
+                    mbar_wait(&full_b[st], (it / p.stages) & 1);
+                    const int dy = p.taps == 9 ? tap / 3 - 1 : 0, dx = p.taps == 9 ? tap - (tap / 3) * 3 - 1 : 0;
+                    // patch pixel of this warpgroup's first output position for this tap (>= -1)
+                    const int srow = t.c0 + dy * p.Wp + dx + 64 * wg;
+                    const uint32_t a_addr = pbase + srow * 128;
+                    // start address shifted by whole 128-byte rows inside the 1024-byte swizzle atom (the patch was
+                    // written in the absolute-address swizzle pattern of a 1024-byte aligned buffer)
+                    const uint64_t adesc = make_smem_desc_sw128(a_addr, 1024, 0) |
+                                           (static_cast<uint64_t>(p.desc_bo ? ((a_addr >> 7) & 7) : 0) << 49);
+                    const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + st * b_stage), 1024, 0);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < kBK / 16; ++k)
+                        wgmma_rows64(acc, p.block_n, adesc + 2 * k, bdesc + 2 * k, (j > 0 || tap > 0 || k > 0) ? 1u : 0u);
+                    wgmma_commit();
+                    if (more) transform_slice(pa ^ 1, tap, p.taps);
+                    wgmma_wait<1>();
+                    if (prev >= 0 && leader) mbar_arrive(&empty_b[prev]);
+                    prev = st;
+                }
+                wgmma_wait<0>();
+                wgmma_fence_regs<kR>(acc);
+                if (ltid == 0 && j < 24) dbg_mark(p, 65 + 2 * j);
+                if (leader) {
+                    mbar_arrive(&empty_b[prev]);
+                    if (kTmaPatch) mbar_arrive(&empty_a[pa]);
+                }
+                if (more) {
+                    fence_proxy_async_smem();
+                    epi_bar_sync();  // chunk j + 1 is in its buffer; both warpgroups are done reading chunk j's
+                    if (ltid == 0 && j < 23) dbg_mark(p, 11 + 2 * j);  // loader: chunk j + 1 stored
+                }
+            }
             // ---- epilogue ----
-            const int as = p.acc_bufs == 2 ? (iter & 1) : 0;
-            const uint32_t aphase = (p.acc_bufs == 2 ? (iter >> 1) : iter) & 1;
-            const int ncol0 = t.n_tile * p.block_n;
-            if (p.bias != nullptr) {
-                const float* bsrc = p.bias + (p.bias_rows > 0 ? static_cast<size_t>(img) * p.bias_stride : 0);
-                for (int c = ltid; c < p.block_n; c += kEpiThreads) bias_s[c] = (ncol0 + c < p.N) ? bsrc[ncol0 + c] : 0.f;
-            }
             int out_row;
             const bool valid = tile_row(p, t, row, out_row);
             uint4 res_pre[4];
-            if (kKind == 0) staged_load_residual(p, t, staged_map(p, t, lane), ew, 0, res_pre);  // hides behind the last chunk's MMAs
-            mbar_wait(&tmem_full[as], aphase);
-            tc_fence_after();
+            if (kKind == 0) staged_load_residual(p, t, staged_map(p, t, lane), ew, 0, res_pre);
+            epi_bar_sync();  // every wgmma of the tile retired: patches and stages may be overwritten
             if (ltid == 0) dbg_mark(p, 4);
-            epi_bar_sync();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_group * 32) << 16) + as * p.acc_stride;
-            if (kFp32Direct) {
-                // tiny output width (conv_out: 4 channels, fp32): one thread per output pixel
-                if (ew < 4) {
-                    uint32_t v[16];
-                    tmem_ld16(taddr, v);
-                    tmem_ld_wait();
-                    if (valid) {
-                        for (int c = 0; c < 16 && ncol0 + c < p.N; ++c) {
-                            const float x = __uint_as_float(v[c]) + (p.bias != nullptr ? bias_s[c] : 0.f);
-                            if (p.out_f32) reinterpret_cast<float*>(p.out)[static_cast<size_t>(out_row) * p.N + ncol0 + c] = x;
-                            else reinterpret_cast<__half*>(p.out)[static_cast<size_t>(out_row) * p.N + ncol0 + c] = __float2half_rn(x);
-                        }
-                    }
-                }
-            } else if (kTmaPatch) {
-                // register epilogue: this warp's 32-column chunks (two warps per TMEM lane quarter), TMEM load of the next
-                // chunk in flight while the current one is converted and stored
-                const int half = ew >> 2;
-                float2 rowacc = make_float2(0.f, 0.f);
-                auto process32 = [&](const uint32_t (&v)[32], int c) {
-                    if (!valid) return;
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        const int cc = c + 16 * hh;
-                        if (ncol0 + cc < p.N) {
-                            float acc[16];
-#pragma unroll
-                            for (int q = 0; q < 16; ++q) acc[q] = __uint_as_float(v[16 * hh + q]);
-                            const float* bptr = p.bias != nullptr ? bias_s + cc : nullptr;
-                            const __half* rptr = p.residual != nullptr
-                                ? p.residual + static_cast<size_t>(out_row) * p.n_store + ncol0 + cc : nullptr;
-                            epilogue_store16<true, false, false, false>(p, acc, out_row, ncol0 + cc, 0, bptr, rptr, rowacc);
-                        }
-                    }
-                };
-                uint32_t va[32], vb[32];
-                int c = 32 * half;
-                if (c < p.block_n) tmem_ld32(taddr + c, va);
-                while (c < p.block_n) {
-                    tmem_ld_wait();
-                    const int c2 = c + 64;
-                    if (c2 < p.block_n) tmem_ld32(taddr + c2, vb);
-                    process32(va, c);
-                    if (c2 >= p.block_n) break;
-                    tmem_ld_wait();
-                    const int c3 = c2 + 64;
-                    if (c3 < p.block_n) tmem_ld32(taddr + c3, va);
-                    process32(vb, c2);
-                    c = c3;
-                }
-            } else {
+            if (kKind == 0) {
                 __half* tile_s = p.stage_dedicated ? stage_tile : reinterpret_cast<__half*>(smem);
                 float* scratch = reinterpret_cast<float*>(tile_s + kBM * (p.block_n + 8));
-                staged_epilogue(p, t, taddr, tile_s, scratch, flag_s, p.bias != nullptr ? bias_s : nullptr, bias_s, ew, lane,
-                                row, out_row, valid, res_pre);
+                const float* bias = p.bias != nullptr ? bias_s : nullptr;
+                stage_accumulators(p, t, acc, tile_s, bias, bias, bias_s, r0, lane);
+                staged_epilogue(p, t, tile_s, scratch, flag_s, ew, lane, res_pre);
+            } else {
+                park_accumulators(acc, p.block_n, acc_s, lda, r0, lane);
+                epi_bar_sync();
+                const float* arow = acc_s + row * lda;
+                if (kFp32Direct) {
+                    // tiny output width (conv_out: 4 channels, fp32): one thread per output pixel
+                    if (ew < 4) {
+                        uint32_t v[16];
+                        acc_ld16(arow, v);
+                        if (valid) {
+                            for (int c = 0; c < 16 && ncol0 + c < p.N; ++c) {
+                                const float x = __uint_as_float(v[c]) + (p.bias != nullptr ? bias_s[c] : 0.f);
+                                if (p.out_f32) reinterpret_cast<float*>(p.out)[static_cast<size_t>(out_row) * p.N + ncol0 + c] = x;
+                                else reinterpret_cast<__half*>(p.out)[static_cast<size_t>(out_row) * p.N + ncol0 + c] = __float2half_rn(x);
+                            }
+                        }
+                    }
+                } else {
+                    // register epilogue: this warp's 32-column chunks (two warps per 32-row group)
+                    const int half = ew >> 2;
+                    float2 rowacc = make_float2(0.f, 0.f);
+                    for (int c = 32 * half; c < p.block_n && valid; c += 64) {
+                        uint32_t v[32];
+                        acc_ld32(arow + c, v);
+#pragma unroll
+                        for (int hh = 0; hh < 2; ++hh) {
+                            const int cc = c + 16 * hh;
+                            if (ncol0 + cc < p.N) {
+                                float a16[16];
+#pragma unroll
+                                for (int q = 0; q < 16; ++q) a16[q] = __uint_as_float(v[16 * hh + q]);
+                                const float* bptr = p.bias != nullptr ? bias_s + cc : nullptr;
+                                const __half* rptr = p.residual != nullptr
+                                    ? p.residual + static_cast<size_t>(out_row) * p.n_store + ncol0 + cc : nullptr;
+                                epilogue_store16<true, false, false, false>(p, a16, out_row, ncol0 + cc, 0, bptr, rptr, rowacc);
+                            }
+                        }
+                    }
+                }
             }
-            tc_fence_before();
-            mbar_arrive(&tmem_empty[as]);
-            if (ltid == 0) dbg_mark(p, 5);
-            epi_bar_sync();  // staging buffers (and, when aliased, the pipeline memory) are free again
+            // generic-proxy accesses of the staging / accumulator tiles are ordered before the producer's next TMA writes
+            fence_proxy_async_smem();
+            epi_bar_sync();  // staging buffers (and the patch / weight memory under them) are free again
+            if (ltid == 0) {
+                dbg_mark(p, 5);
+                mbar_arrive(acc_free);
+            }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, static_cast<uint32_t>(p.tmem_cols));
     }
 }
 
@@ -1439,11 +1382,10 @@ struct GemmPlan {
     int Hout, Wout, bw, bh, bn_img, tiles_w, tiles_h, tiles_n;
     int bias_mode, res_smem, epi_smem;
     int cluster;  // split-K reduced inside a thread-block cluster of `splits` CTAs (DSMEM) instead of a second kernel
-    int two_cta;  // CTA pairs (tcgen05.mma cta_group::2, M = 256): each CTA stages half of the B tile
     int halo;     // mode 2: halo-reuse convolution
     int Wp, tiles_per_img, patch_rows, patch_bytes;
     int win, tw, th, tiles_x;
-    int staged, stage_dedicated, acc_bufs;
+    int staged, stage_dedicated;
     int tma_patch;
     int cs_slots;  // statistics slots per image this tiling produces (0: column statistics not available)
     int smem_bytes;
@@ -1453,13 +1395,6 @@ static bool cluster_splitk_enabled() {
     // B200SD_CLUSTER_SPLITK=0: always take the workspace + reduce-kernel path (read per call: tuning scripts flip it)
     const char* e = getenv("B200SD_CLUSTER_SPLITK");
     return !(e && e[0] == '0');
-}
-
-static bool two_cta_enabled() {
-    // opt-in (B200SD_2CTA=1, read per call: tuning scripts flip it).  Correct on every parity test, but measured
-    // 2 % slower end to end than single-CTA tiles on the SD-2.1 UNet (199.2 vs 203.5 iter/s): see profiles/README.md
-    const char* e = getenv("B200SD_2CTA");
-    return e && e[0] == '1';
 }
 
 static int ilog2(int v) {
@@ -1476,7 +1411,9 @@ static bool staged_enabled() {
 }
 
 static bool desc_base_offset_enabled() {
-    // how row-shifted SWIZZLE_128B descriptors are formed (tools/desc_probe.cu decides; read per call)
+    // how row-shifted SWIZZLE_128B descriptors are formed: 0 (default) = the start address alone (the hardware applies
+    // the swizzle to absolute address bits; the halo tests pass on H100 only this way), 1 = also the matrix-base-offset
+    // field; read per call
     const char* e = getenv("B200SD_DESC_BO");
     return e && e[0] == '1';
 }
@@ -1527,16 +1464,17 @@ static int plan_halo(const b200sd_gemm_args& a, GemmPlan& pl) {
     pl.block_n = a.block_n;
     B200SD_REQUIRE(pl.block_n == 16 || (pl.block_n % 32 == 0 && pl.block_n <= 256), "b200sd_gemm: halo block_n %d", pl.block_n);
     pl.n_tiles = (a.n + pl.block_n - 1) / pl.block_n;
-    pl.splits = 1, pl.kb_per_split = pl.kb_total, pl.cluster = 0, pl.two_cta = 0;
+    pl.splits = 1, pl.kb_per_split = pl.kb_total, pl.cluster = 0;
     pl.bias_mode = a.bias != nullptr ? 1 : 0;
     pl.res_smem = 0;
-    const long units = static_cast<long>(pl.m_tiles) * pl.n_tiles;
-    pl.acc_bufs = units > num_sms() ? 2 : 1;
     const bool fp32_direct = a.out_f32 || pl.block_n == 16;
     B200SD_REQUIRE(!fp32_direct || (pl.block_n == 16 && a.residual == nullptr && a.cs_partial == nullptr),
                    "b200sd_gemm: halo fp32 / narrow output needs block_n 16, no residual, no statistics");
     pl.staged = (fp32_direct || pl.tma_patch) ? 0 : 1;
-    pl.stage_dedicated = (pl.staged && pl.acc_bufs == 2) ? 1 : 0;
+    // the loader kinds keep twelve patch vectors per thread in registers beside the accumulators
+    B200SD_REQUIRE(pl.tma_patch || pl.block_n <= 128, "b200sd_gemm: halo block_n %d > 128 needs halo = 2", pl.block_n);
+    // the epilogue tiles live over the drained patches / weight stages (the producer waits for them between tiles)
+    pl.stage_dedicated = 0;
     const int cin = a.c0 + a.c1;
     const int fixed = 2 * pl.patch_bytes + (2 * kHaloMaxStages + 8) * 8 + 16 + 256 * 4 + 64 + 64 * 8 + ((cin + 7) & ~7) * 8 +
                       (pl.stage_dedicated ? kBM * (pl.block_n + 8) * 2 + 8 * pl.block_n * 8 : 0) + 1024;
@@ -1544,6 +1482,9 @@ static int plan_halo(const b200sd_gemm_args& a, GemmPlan& pl) {
     pl.stages = std::min(kHaloMaxStages, (227 * 1024 - fixed) / b_stage);
     B200SD_REQUIRE(pl.stages >= 3, "b200sd_gemm: halo kernel does not fit shared memory (w=%d c=%d block_n=%d)", a.w, cin, pl.block_n);
     pl.smem_bytes = fixed + pl.stages * b_stage;
+    const int over = 2 * pl.patch_bytes + pl.stages * b_stage;
+    B200SD_REQUIRE(over >= (pl.staged ? kBM * (pl.block_n + 8) * 2 + 8 * pl.block_n * 8 : kBM * (pl.block_n + 4) * 4),
+                   "b200sd_gemm: halo epilogue tile does not fit over the pipeline memory (block_n=%d)", pl.block_n);
     pl.epi_smem = 0;
     pl.cs_slots = pl.tiles_per_img;
     return 0;
@@ -1558,7 +1499,7 @@ static int halo_pick_block_n(const b200sd_gemm_args& a) {
     if (wp > 80) m_tiles = static_cast<long>(a.n_img) * ((static_cast<long>(a.h) * a.w + 101) / 102);  // windows: ~80 % useful rows
     double best = 1e30;
     int best_bn = 128;
-    for (int bn = 256; bn >= 32; bn -= 32) {
+    for (int bn = a.halo == 2 ? 256 : 128; bn >= 32; bn -= 32) {
         const int nt = (a.n + bn - 1) / bn;
         if (nt * bn > a.n + a.n / 4 + 31) continue;
         const double waves = std::ceil(static_cast<double>(m_tiles * nt) / num_sms());
@@ -1583,7 +1524,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
     B200SD_REQUIRE((a.c2 == 0 && a.c3 == 0) || (a.mode == 1 && a.stride == 1 && !a.halo && a.c2 > 0 && a.c2 % 8 == 0 && a.c3 % 8 == 0),
                    "b200sd_gemm: shortcut sources (a2 / a3) need a stride-1 3x3 convolution and channel counts that are multiples of 8");
     pl.halo = 0, pl.Wp = 0, pl.tiles_per_img = 0, pl.patch_rows = 0, pl.patch_bytes = 0;
-    pl.staged = 0, pl.stage_dedicated = 0, pl.acc_bufs = 1, pl.cs_slots = 0, pl.smem_bytes = 0;
+    pl.staged = 0, pl.stage_dedicated = 0, pl.cs_slots = 0, pl.smem_bytes = 0;
     const bool want_stats = a.cs_partial != nullptr || a.rs_out != nullptr;
     B200SD_REQUIRE(!want_stats || (!a.geglu && !a.out_f32 && a.act == 0 && a.n % 8 == 0 && a.split_k <= 1),
                    "b200sd_gemm: statistics outputs need a plain fp16 epilogue without split-K");
@@ -1622,7 +1563,8 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
         pl.m_tiles = pl.tiles_w * pl.tiles_h * pl.tiles_n;
     }
     if (a.geglu) B200SD_REQUIRE(a.n % 16 == 0, "b200sd_gemm: GEGLU needs n %% 16 == 0");
-    // ---- tile shape / split-K selection by a small cost model (cycles; constants fitted to B200 runs) ----
+    // ---- tile shape / split-K selection by a small cost model (cycles per SM; constants fitted to B200 runs, not
+    // refitted for H100 -- tools/bench_gemm_shapes.py measures the shapes they are fitted to) ----
     const int sms = num_sms();
     const bool can_split = !a.geglu && a.n % 4 == 0 && a.act == 0 && !want_stats && a.ln_parts == 0;
     auto epi_cycles = [&](int bn) { return 400.0 + (bn / 32.0) * (a.geglu ? 520.0 : 230.0); };
@@ -1653,7 +1595,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
                     const long units = static_cast<long>(pl.m_tiles) * nt * sp;
                     // clusters need sp free SMs of one GPC: count ~10 % of the SMs as stranded
                     const double waves = std::ceil(static_cast<double>(units) / (sms - sms / 10));
-                    const double epi = 1500.0 + (bn / 32.0) * 120.0 + 128.0 * bn * 4.0 / 17.0;  // TMEM->smem, 2 syncs, DSMEM
+                    const double epi = 1500.0 + (bn / 32.0) * 120.0 + 128.0 * bn * 4.0 / 17.0;  // registers->smem, 2 syncs, DSMEM
                     t = 5000.0 + waves * (main + epi);
                 } else {
                     const long units = static_cast<long>(pl.m_tiles) * nt * se;
@@ -1700,27 +1642,22 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
         }
         if (a.residual != nullptr && !a.geglu && a.n % 8 == 0) pl.res_smem = 1;
     }
-    // ---- CTA pairs: two M tiles share one B tile (each CTA loads half of it), which halves the L2 -> SM operand
-    // traffic per flop of B -- the limiter of these GEMMs (~42 B/clk/SM of L2 bandwidth vs 48 KiB per k-block) ----
     const bool regular = (a.act == 0) && (a.n % 16 == 0) && ((a.geglu ? a.n / 2 : a.n) % 8 == 0) && (pl.block_n % 32 == 0) &&
                          pl.bias_mode != 2 && (a.residual == nullptr || pl.res_smem);
-    pl.two_cta = (two_cta_enabled() && pl.splits == 1 && regular && pl.m_tiles >= 2 &&
-                  static_cast<long>((pl.m_tiles + 1) / 2) * pl.n_tiles * 2 >= num_sms() / 2) ? 1 : 0;
-    const int per_stage = kAStage + (pl.two_cta ? pl.block_n / 2 : pl.block_n) * kBK * 2;
+    const int per_stage = kAStage + pl.block_n * kBK * 2;
     {
-        const long units = static_cast<long>(pl.m_tiles) * pl.n_tiles * pl.splits;
-        pl.acc_bufs = ((!pl.cluster && units > num_sms()) || pl.two_cta) ? 2 : 1;
         // staged epilogue: fp16 tile in shared memory, row-contiguous residual reads / stores, statistics outputs
-        const bool eligible = regular && pl.splits == 1 && !pl.two_cta && !a.geglu && !a.out_f32 && a.n % 8 == 0;
+        const bool eligible = regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
         // column statistics need the staged epilogue; row statistics alone ride on the register epilogue (every thread
         // owns a row there), which keeps the residual tile prefetched in shared memory during the main loop
         pl.staged = (eligible && (a.cs_partial != nullptr || (a.residual != nullptr && staged_enabled()))) ? 1 : 0;
         B200SD_REQUIRE(a.cs_partial == nullptr || pl.staged, "b200sd_gemm: this shape cannot emit column statistics (n=%d block_n=%d)", a.n,
                        pl.block_n);
-        B200SD_REQUIRE(a.rs_out == nullptr || pl.staged || (regular && !a.geglu && !a.out_f32 && pl.splits == 1 && !pl.two_cta),
+        B200SD_REQUIRE(a.rs_out == nullptr || pl.staged || (regular && !a.geglu && !a.out_f32 && pl.splits == 1),
                        "b200sd_gemm: this shape cannot emit row statistics (n=%d block_n=%d)", a.n, pl.block_n);
         if (pl.staged) pl.res_smem = 0;
-        pl.stage_dedicated = (pl.staged && pl.acc_bufs == 2) ? 1 : 0;
+        // the staging tile lives over the drained pipeline stages (the producer waits for it between tiles)
+        pl.stage_dedicated = 0;
         if (a.cs_partial != nullptr) {
             // every 16-row group of a tile must lie inside one image, and the tiles of an image must be countable
             int slots = 0;
@@ -1738,6 +1675,10 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
     pl.epi_smem = kEpiFixed + (pl.res_smem ? kBM * (pl.block_n + 8) * 2 : 0) +
                   (pl.stage_dedicated ? kBM * (pl.block_n + 8) * 2 + 8 * pl.block_n * 8 : 0);
     pl.stages = std::max(2, std::min(kMaxStages, (smem_budget() - pl.epi_smem) / per_stage));
+    // the fp32 accumulator tile (or the fp16 staging tile) is parked over the drained stages
+    const int park = pl.staged ? kBM * (pl.block_n + 8) * 2 + 8 * pl.block_n * 8 : kBM * (pl.block_n + 4) * 4;
+    while (pl.stages * per_stage < park && pl.stages < kMaxStages) ++pl.stages;
+    B200SD_REQUIRE(pl.stages * per_stage >= park, "b200sd_gemm: epilogue tile does not fit over the stages (block_n=%d)", pl.block_n);
     pl.smem_bytes = pl.stages * per_stage + (2 * kMaxStages + 4) * 8 + 16 + pl.epi_smem + 1024;
     return 0;
 }
@@ -1822,13 +1763,13 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
         const uint64_t rows = static_cast<uint64_t>(pl.n_tiles) * pl.kb_total * pl.block_n;
         const uint64_t dims[2] = {kBK, rows};
         const uint64_t str[1] = {kBK * 2};
-        const uint32_t box[2] = {kBK, static_cast<uint32_t>(pl.two_cta ? pl.block_n / 2 : pl.block_n)};
+        const uint32_t box[2] = {kBK, static_cast<uint32_t>(pl.block_n)};
         if (int rc = encode_tmap_f16(&p.tmB, a.wgt, 2, dims, str, box, es1)) return rc;
     } else {
         const uint64_t ktot = static_cast<uint64_t>(pl.taps) * pl.Kpt;
         const uint64_t dims[2] = {ktot, static_cast<uint64_t>(a.n)};
         const uint64_t str[1] = {ktot * 2};
-        const uint32_t box[2] = {kBK, static_cast<uint32_t>(pl.two_cta ? pl.block_n / 2 : pl.block_n)};
+        const uint32_t box[2] = {kBK, static_cast<uint32_t>(pl.block_n)};
         if (int rc = encode_tmap_f16(&p.tmB, a.wgt, 2, dims, str, box, es1)) return rc;
     }
     p.mode = pl.halo ? 2 : a.mode;
@@ -1870,8 +1811,6 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
     p.residual = reinterpret_cast<const __half*>(a.residual);
     p.partial = (pl.splits > 1 && !pl.cluster) ? a.workspace : nullptr;
     p.cluster = pl.cluster;
-    p.two_cta = pl.two_cta;
-    p.m_pairs = (pl.m_tiles + 1) / 2;
     p.H = a.h, p.W = a.w, p.Wp = pl.Wp, p.tiles_per_img = pl.tiles_per_img;
     p.win = pl.win, p.tw = pl.tw, p.th = pl.th, p.tiles_x = pl.tiles_x;
     p.inv_wp = pl.Wp > 0 ? (1 << 20) / pl.Wp + 1 : 0;
@@ -1898,24 +1837,17 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
         const char* e = getenv("B200SD_DBG_PTR");  // tools/halo_timeline.py: device address of a 128-slot int64 buffer
         p.dbg = (e && e[0]) ? reinterpret_cast<long long*>(strtoull(e, nullptr, 0)) : nullptr;
     }
-    {
-        // one accumulator buffer when no CTA sees a second tile (nothing to overlap the epilogue with); the allocation
-        // is the smallest power of two that holds the buffers, so small tiles leave TMEM for a co-resident CTA
-        p.acc_bufs = pl.acc_bufs;
-        int stride = 32;
-        while (stride < pl.block_n) stride <<= 1;
-        if (pl.two_cta) stride = 256;
-        p.acc_stride = stride;
-        p.tmem_cols = pl.two_cta ? 512 : stride * p.acc_bufs;
-    }
     if (pl.halo) {
         using HaloFn = void (*)(GemmParams);
         const int kind = pl.tma_patch ? 2 : (pl.staged == 0 ? 1 : 0);
-        HaloFn hfn = kind == 2 ? halo_conv_kernel<2> : (kind == 1 ? halo_conv_kernel<1> : halo_conv_kernel<0>);
-        static bool hattr[3] = {false, false, false};
-        if (!hattr[kind]) {
+        const bool wide = pl.block_n > 128;  // (only the TMA-patch kind takes tiles wider than 128 columns)
+        HaloFn hfn = kind == 2 ? (wide ? halo_conv_kernel<2, 128> : halo_conv_kernel<2, 64>)
+                               : (kind == 1 ? halo_conv_kernel<1, 8> : halo_conv_kernel<0, 64>);
+        const int hslot = kind == 2 && wide ? 3 : kind;
+        static bool hattr[4] = {false, false, false, false};
+        if (!hattr[hslot]) {
             B200SD_CHECK_CUDA(cudaFuncSetAttribute(hfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            hattr[kind] = true;
+            hattr[hslot] = true;
         }
         const int units = pl.m_tiles * pl.n_tiles;
         B200SD_CHECK_CUDA(launch_kernel(hfn, dim3(std::min(units, num_sms())), dim3(kGemmThreads), pl.smem_bytes, stream, p));
@@ -1934,46 +1866,45 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
     using KernelFn = void (*)(GemmParams);
     KernelFn fn;
     int variant;
+    const bool wide = pl.block_n > 128;
+#define B200SD_GEMM_FN(g, gl, f32, part, st) (wide ? wgmma_gemm_kernel<g, gl, f32, part, st, 128> : wgmma_gemm_kernel<g, gl, f32, part, st, 64>)
     if (!regular) {
-        fn = umma_gemm_kernel<true, false, false, false>, variant = 0;
+        fn = B200SD_GEMM_FN(true, false, false, false, false), variant = 0;
     } else if (pl.staged) {
-        fn = umma_gemm_kernel<false, false, false, false, false, true>, variant = 8;
+        fn = B200SD_GEMM_FN(false, false, false, false, true), variant = 5;
     } else if (pl.splits > 1) {
-        fn = umma_gemm_kernel<false, false, false, true>, variant = 1;
+        fn = B200SD_GEMM_FN(false, false, false, true, false), variant = 1;
     } else if (a.geglu) {
-        fn = pl.two_cta ? umma_gemm_kernel<false, true, false, false, true> : umma_gemm_kernel<false, true, false, false>;
-        variant = pl.two_cta ? 5 : 2;
+        fn = B200SD_GEMM_FN(false, true, false, false, false), variant = 2;
     } else if (a.out_f32) {
-        fn = pl.two_cta ? umma_gemm_kernel<false, false, true, false, true> : umma_gemm_kernel<false, false, true, false>;
-        variant = pl.two_cta ? 6 : 3;
+        fn = B200SD_GEMM_FN(false, false, true, false, false), variant = 3;
     } else {
-        fn = pl.two_cta ? umma_gemm_kernel<false, false, false, false, true> : umma_gemm_kernel<false, false, false, false>;
-        variant = pl.two_cta ? 7 : 4;
+        fn = B200SD_GEMM_FN(false, false, false, false, false), variant = 4;
     }
-    B200SD_REQUIRE(!pl.two_cta || variant >= 5, "b200sd_gemm: CTA pairs need a regular single-split epilogue variant");
+#undef B200SD_GEMM_FN
+    if (wide) variant += 6;
     if (pl.splits > 1 && !pl.cluster) {
         // the separate reduce kernel applies bias / residual; the partial writer must not
         p.bias = nullptr;
         p.residual = nullptr;
     }
-    static bool attr_set[9] = {false, false, false, false, false, false, false, false, false};
+    static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
     if (!attr_set[variant]) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set[variant] = true;
     }
-    if (pl.cluster || pl.two_cta) {
-        B200SD_REQUIRE(pl.two_cta || variant == 1, "b200sd_gemm: cluster split-K needs the regular epilogue variant");
+    if (pl.cluster) {
+        B200SD_REQUIRE(variant % 6 == 1, "b200sd_gemm: cluster split-K needs the regular epilogue variant");
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
-        // split-K: one (tile, split) per CTA, the splits of a tile are one cluster;  pairs: persistent clusters of 2
-        const int pair_units = ((pl.m_tiles + 1) / 2) * pl.n_tiles;
-        cfg.gridDim = pl.two_cta ? dim3(2 * std::min(pair_units, num_sms() / 2)) : dim3(total);
+        // split-K: one (tile, split) per CTA, the splits of a tile are one cluster
+        cfg.gridDim = dim3(total);
         cfg.blockDim = dim3(kGemmThreads);
         cfg.dynamicSmemBytes = smem_bytes;
         cfg.stream = stream;
         cudaLaunchAttribute at[2];
         at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = pl.two_cta ? 2 : pl.splits;
+        at[0].val.clusterDim.x = pl.splits;
         at[0].val.clusterDim.y = 1;
         at[0].val.clusterDim.z = 1;
         cfg.attrs = at;
@@ -2042,9 +1973,9 @@ extern "C" int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf
     if (int rc = b200sd::plan_gemm(*args, pl)) return rc;
     snprintf(buf, buf_size,
              "M=%d N=%d kb_total=%d m_tiles=%d n_tiles=%d block_n=%d splits=%d kb_per_split=%d stages=%d "
-             "box=%dx%dx%d bias_mode=%d res_smem=%d epi_smem=%d cluster=%d two_cta=%d",
+             "box=%dx%dx%d bias_mode=%d res_smem=%d epi_smem=%d cluster=%d",
              pl.M, pl.N, pl.kb_total, pl.m_tiles, pl.n_tiles, pl.block_n, pl.splits, pl.kb_per_split, pl.stages,
-             pl.bn_img, pl.bh, pl.bw, pl.bias_mode, pl.res_smem, pl.epi_smem, pl.cluster, pl.two_cta);
+             pl.bn_img, pl.bh, pl.bw, pl.bias_mode, pl.res_smem, pl.epi_smem, pl.cluster);
     return 0;
 }
 

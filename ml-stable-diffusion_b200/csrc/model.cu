@@ -26,7 +26,7 @@ namespace {
     } while (0)
 
 __global__ void add_f32_kernel(float* __restrict__ a, const float* __restrict__ b, int n) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) a[i] += b[i];
@@ -97,9 +97,8 @@ public:
     bool kv_ready = false;
     int attn_impl = 1;
     // GroupNorm fusion (B200SD_FUSED=1 at create time): GroupNorm + SiLU inside the halo convolution's operand path with
-    // statistics from the producers' epilogues.  Default off, like the Python host: on a B200 at batch 2 the one-launch
-    // cluster GroupNorm in front of the 9-tap TMA convolution measured faster (profiles/README.md); LayerNorm is always
-    // folded into its consumer GEMM.
+    // statistics from the producers' epilogues.  Default off, like the Python host (the one-launch cluster GroupNorm in
+    // front of the 9-tap TMA convolution is the default path); LayerNorm is always folded into its consumer GEMM.
     bool fuse_gn = false;
 
     ~UNet() {

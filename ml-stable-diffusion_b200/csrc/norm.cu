@@ -1,4 +1,4 @@
-// b200sd -- GroupNorm (+SiLU, + channel concat of two sources) and LayerNorm for sm_100a.
+// b200sd -- GroupNorm (+SiLU, + channel concat of two sources) and LayerNorm for sm_90a.
 // HBM/L2-bound elementwise + reduction kernels: 16-byte vectorised, coalesced along channels.
 //
 // GroupNorm replaces torch.nn.GroupNorm in the reference (unet.py:430,448,528,966; eps 1e-5 in
@@ -41,7 +41,7 @@ __global__ void __launch_bounds__(416) gn_stats_kernel(const __half* __restrict_
                                                        float eps, float* __restrict__ partial /* [n][chunks][g][2] */,
                                                        float* __restrict__ final_stats /* [n][g][2] */,
                                                        unsigned int* __restrict__ tickets /* [n] */) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int C = c0 + c1;
     const int cpg = C / groups;
@@ -177,7 +177,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __half* __restrict_
                                                        const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, int silu,
                                                        __half* __restrict__ out, int px_per_block) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int C = c0 + c1;
     const int cpg = C / groups;
@@ -229,7 +229,7 @@ __global__ void __launch_bounds__(256) gn_apply_chan_kernel(const __half* __rest
                                                             const float* __restrict__ chan0, const float* __restrict__ chan1,
                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
                                                             int silu, __half* __restrict__ out, int px_per_block) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int C = c0 + c1;
     const int cpg = C / groups;
@@ -327,7 +327,7 @@ __global__ void gn_cluster_kernel(const __half* __restrict__ x0, const __half* _
     float* chsum = red + 2 * TY * chunk_ch;                                        // [2][chunk_ch]
     float* xchg = chsum + 2 * chunk_ch;                                            // [2][ng]  (read by the peers)
     float* stat = xchg + 2 * ng;                                                   // [2][ng]  mean, rstd
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
 
     // ---- one pass: global -> shared slab, per-channel (sum, sum of squares) in registers; ONE exchange through
@@ -463,7 +463,7 @@ template <int kVecsPerLane>
 __global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restrict__ x, const float* __restrict__ gamma,
                                                          const float* __restrict__ beta, __half* __restrict__ out,
                                                          int rows, int c, float eps) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -536,7 +536,7 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restric
 // ---- row softmax: fp32 scores [rows, cols] -> fp16 probabilities (VAE mid-block attention, d=512) ----
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ in, __half* __restrict__ out,
                                                            int cols, float scale_log2) {
-    pdl_trigger();  // no TMEM / large shared memory here: dependents may start their prologue at once
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t row = blockIdx.x;
     const float* src = in + row * cols;

@@ -31,8 +31,7 @@ bool pdl_enabled() {
     if (g_pdl < 0) {
         const char* e = getenv("B200SD_PDL");
         // on by default (B200SD_PDL=0 disables): every kernel executes griddepcontrol.wait before it touches global
-        // memory and releases its dependents early (kernels that allocate TMEM only after their own allocation, so a
-        // dependent CTA can never hold columns the running grid still needs); measured +2.7 % on the whole step
+        // memory and releases its dependents early, so the next kernel's prologue overlaps this one's tail
         g_pdl = (e != nullptr && e[0] == '0') ? 0 : 1;
     }
     return g_pdl == 1;
@@ -42,8 +41,8 @@ int num_sms() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     }
     return sms;
 }

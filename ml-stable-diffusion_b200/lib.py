@@ -124,7 +124,7 @@ def load():
     if not os.path.exists(_LIB_PATH):
         raise B200SDError(
             f"{_LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). b200sd has no CPU or PyTorch fallback path.")
+            "(nvcc, sm_90a). b200sd has no CPU or PyTorch fallback path.")
     lib = C.CDLL(_LIB_PATH)
     for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported

@@ -1,4 +1,4 @@
-"""Text-to-image pipeline with the reference's call surface, running on the B200 kernels.
+"""Text-to-image pipeline with the reference's call surface, running on the sm_90a kernels.
 
 Mirrors ``CoreMLStableDiffusionPipeline.__call__`` (``python_coreml_stable_diffusion/pipeline.py:403-589``):
 same keyword arguments, same order of operations (encode -> latents -> [CFG-duplicated UNet ->
@@ -66,7 +66,7 @@ class SyntheticTextEncoder:
 
 
 class B200StableDiffusionPipeline:
-    """Drop-in for ``CoreMLStableDiffusionPipeline`` on one B200."""
+    """Drop-in for ``CoreMLStableDiffusionPipeline`` on one H100."""
 
     def __init__(self, unet: UNetModel, vae_decoder: VAEDecoderModel, scheduler="DDIM", text_encoder=None,
                  tokenizer=None, force_zeros_for_empty_prompt=True, xl=False, controlnet=None, loop_graph=True,

@@ -1,4 +1,4 @@
-"""CLIP text encoder on the sm_100a kernels (SURVEY 8f N2, device half).
+"""CLIP text encoder on the sm_90a kernels (SURVEY 8f N2, device half).
 
 Replaces the ``text_encoder`` Core ML model of the reference -- ``transformers.CLIPTextModel`` as converted by
 ``torch2coreml.py:408-441`` and called by ``pipeline.py:151-175`` with *float* ``input_ids`` (1, 77), returning

@@ -1,4 +1,4 @@
-"""UNet denoiser on the sm_100a kernels: weight pre-packing + the launch graph.
+"""UNet denoiser on the sm_90a kernels: weight pre-packing + the launch graph.
 
 This is the device-side replacement for the traced graph of the reference
 ``UNet2DConditionModel.forward`` / ``UNet2DConditionModelXL.forward``
@@ -98,10 +98,10 @@ class UNetEngine:
         self.in_pad = max(8, (self.in_ch + 7) // 8 * 8)
         self.xl = cfg.get("addition_embed_type") == "text_time"
         self.support_controlnet = bool(cfg.get("support_controlnet", False))
-        # Normalisation fusion level (B200SD_FUSED; measurements in profiles/README.md):
+        # Normalisation fusion level (B200SD_FUSED):
         #   "ln" (default)  LayerNorm folded into its consumer GEMM, row statistics from the producer's epilogue;
-        #                   GroupNorm stays the one-launch cluster kernel in front of the 9-tap TMA convolution -- on
-        #                   a B200 at batch 2 every fused-GroupNorm variant below measured SLOWER than this
+        #                   GroupNorm stays the one-launch cluster kernel in front of the 9-tap TMA convolution (the
+        #                   fused-GroupNorm variants below are opt-in; they have not been timed against it on H100)
         #   "1"  GroupNorm + SiLU applied in the halo convolution's operand path (no GroupNorm launch at all),
         #        statistics from the producers' staged epilogues
         #   "2"  statistics from the producers, one elementwise GroupNorm-apply launch + 9-tap convolution

@@ -1,4 +1,4 @@
-"""VAE decoder on the sm_100a kernels (same conv / GroupNorm / GEMM kernels as the UNet).
+"""VAE decoder on the sm_90a kernels (same conv / GroupNorm / GEMM kernels as the UNet).
 
 Replaces the ``vae_decoder`` Core ML model the reference calls once per image
 (``pipeline.py:313-320``), whose graph is ``decoder(post_quant_conv(z))`` of diffusers'

@@ -1,15 +1,14 @@
-"""BPE tokenizer: algorithm on a tiny hand-made vocabulary (runs anywhere) and the reference's known-answer ids
-(StableDiffusionTests.swift:43-48) with the CLIP vocabulary / merges that ship inside the reference tree (build
-container only: the files are data of the reference and are not copied into this repository)."""
+"""BPE tokenizer: algorithm on a tiny hand-made vocabulary and the reference's known-answer ids
+(StableDiffusionTests.swift:43-48) with the part of the CLIP vocabulary / merges those prompts touch
+(tests/golden/clip_bpe, cut from the reference's files by tests/golden/make_golden_tokenizer.py)."""
 import json
 import os
 
 import numpy as np
-import pytest
 
 from b200sd.tokenizer import BPETokenizer
 
-RES = "/root/reference/swift/StableDiffusionTests/Resources"
+RES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "clip_bpe")
 
 
 def test_bpe_merges_by_rank_and_pads(tmp_path):
@@ -33,7 +32,6 @@ def test_bpe_merges_by_rank_and_pads(tmp_path):
     assert padded.input_ids("low") == [0, 2, 1, 7, 7, 7]
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(RES, "vocab.json")), reason="reference resources not present")
 def test_reference_known_answer_ids():
     tok = BPETokenizer.from_files(os.path.join(RES, "merges.txt"), os.path.join(RES, "vocab.json"))
     cases = {

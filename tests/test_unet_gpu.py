@@ -480,8 +480,7 @@ def test_pipeline_tiny_image_to_image_vs_oracle(cuda_lib):
 
 def test_controlnet_sd21_vs_reference_golden(cuda_lib):
     """BASELINE configs[4] network at full size (SD-2.1 ControlNet, 361 M parameters, 512x512 condition image):
-    the 13 residuals against the unmodified reference module run on the CPU (make_golden_controlnet.py; measured
-    on a B200: worst max-abs 4.4e-3 on a residual of magnitude 2.2)."""
+    the 13 residuals against the unmodified reference module run on the CPU (make_golden_controlnet.py)."""
     from b200sd.controlnet import ControlNetModel
 
     gold = np.load(os.path.join(GOLD, "controlnet_sd21.npz"))

@@ -77,4 +77,4 @@ for name, mode, nimg, h, c0, c1, co in SHAPES:
     L._tiled_cache.clear()
     del ws
     torch.cuda.empty_cache()
-json.dump(out, open("gpurun_out/gemm_shapes.json", "w"), indent=1)
+json.dump(out, open(sys.argv[1] if len(sys.argv) > 1 else "gemm_shapes.json", "w"), indent=1)

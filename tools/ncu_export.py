@@ -1,4 +1,4 @@
-"""Exports the key metrics of an .ncu-rep (ncu -i ... --page raw --csv) to a compact CSV under profiles/."""
+"""Exports the key metrics of an .ncu-rep (ncu -i ... --page raw --csv) to a compact CSV."""
 import csv
 import subprocess
 import sys

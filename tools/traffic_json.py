@@ -1,5 +1,5 @@
 """ncu launch list with dram__bytes_read.sum / dram__bytes_write.sum / gpu__time_duration.sum (cold caches: ncu flushes
-L2 before every kernel) -> profiles/traffic_rN.json: DRAM bytes per launch of the GEMM / convolution kernels and per kernel."""
+L2 before every kernel) -> a JSON file: DRAM bytes per launch of the GEMM / convolution kernels and per kernel."""
 import collections
 import csv
 import io
@@ -29,13 +29,13 @@ def main(path, out):
             e["us"] += v
     for e in per.values():
         e["launches"] = len(e["launches"])
-    gemm = [e for k, e in per.items() if k.startswith(("umma_gemm", "halo_conv", "splitk_reduce"))]
-    n = sum(e["launches"] for k, e in per.items() if k.startswith(("umma_gemm", "halo_conv")))
+    gemm = [e for k, e in per.items() if k.startswith(("wgmma_gemm", "halo_conv", "splitk_reduce"))]
+    n = sum(e["launches"] for k, e in per.items() if k.startswith(("wgmma_gemm", "halo_conv")))
     tot = sum(e["read_bytes"] + e["write_bytes"] for e in gemm)
     doc = {"source": f"{path} (ncu dram__bytes_read.sum + dram__bytes_write.sum of ONE bench.py iteration, "
                      "`bench.py --profile-step`; L2 flushed before every kernel by ncu, so activations that stay in L2 "
                      "during a real step are counted as DRAM reads here: an upper bound)",
-           "kernel": "umma_gemm_kernel (all variants) + splitk_reduce_kernel", "launches": n,
+           "kernel": "wgmma_gemm_kernel (all variants) + splitk_reduce_kernel", "launches": n,
            "dram_bytes_per_forward": tot, "dram_bytes_per_launch": tot / max(n, 1),
            "algorithmic_weight_bytes_per_forward": 1.73e9, "per_kernel": dict(sorted(per.items()))}
     json.dump(doc, open(out, "w"), indent=1)
