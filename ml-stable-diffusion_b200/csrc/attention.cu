@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
                 const uint64_t kdesc = make_smem_desc_sw128(smem_u32(smem + kSmemK + st * kTileBytes) + hi * (kHalf * 128), 1024, 0);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < kD / 16; ++k) wgmma_m64n64_ss(s, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
+                for (int k = 0; k < kD / 16; ++k) wgmma_ss<64>(s, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
                 wgmma_commit();
                 wgmma_wait<0>();
                 wgmma_fence_regs<32>(s);

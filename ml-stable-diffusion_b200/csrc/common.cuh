@@ -171,6 +171,16 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Register reallocation between warpgroups: a warpgroup returns registers to the CTA's pool (dec) or waits for them
+// (inc).  Every warp of the warpgroup executes the same instruction; N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 // keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float* d) {
@@ -179,38 +189,125 @@ __device__ __forceinline__ void wgmma_fence_regs(float* d) {
 }
 
 #define B200SD_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-// D[64 x N] (+)= A[64 x 16] (smem, K-major) * B[N x 16]^T (smem, K-major unless trans_b); fp16 in, fp32 accumulate.
-// Accumulator layout (thread t of the warpgroup): d[4 j + e] = (row 16 (t / 32) + (t % 32) / 4 + 8 (e / 2),
-// column 8 j + 2 (t % 4) + e % 2).
-template <int kTransB = 0>
-__device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24)
-        : "l"(da), "l"(db), "r"(acc), "n"(kTransB)
-        : "memory");
-}
-__device__ __forceinline__ void wgmma_m64n32_ss(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void wgmma_m64n16_ss(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+// D[64 x N] (+)= A[64 x 16] (smem, K-major) * B[N x 16]^T (smem, K-major) as ONE wgmma; fp16 in, fp32 accumulate.
+// N / 2 accumulators per thread (thread t of the warpgroup): d[4 j + e] = (row 16 (t / 32) + (t % 32) / 4 + 8 (e / 2),
+// column 8 j + 2 (t % 4) + e % 2).  Specialised for the widths the kernels issue.
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t acc);
+template <>
+__device__ __forceinline__ void wgmma_ss<16>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
         : B200SD_F8(0)
         : "l"(da), "l"(db), "r"(acc)
         : "memory");
 }
+template <>
+__device__ __forceinline__ void wgmma_ss<32>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<96>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+        "}, %48, %49, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<128>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<160>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+        "}, %80, %81, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
+          B200SD_F8(64), B200SD_F8(72)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<192>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+        "}, %96, %97, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
+          B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<256>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, 0, 0;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
+          B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88), B200SD_F8(96), B200SD_F8(104), B200SD_F8(112), B200SD_F8(120)
+        : "l"(da), "l"(db), "r"(acc)
+        : "memory");
+}
+
 // A from registers (fp16 pairs in the accumulator layout of a 64 x 16 tile), B [16 x 64] from smem, MN-major
 __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
     asm volatile(
@@ -225,22 +322,23 @@ __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t (&a)
 }
 #undef B200SD_F8
 
-// D[64 x bn] (+)= A[64 x 16] * B[bn x 16]^T as 64 / 32 / 16-column pieces (bn: multiple of 16, <= 2 R).  The pieces'
-// accumulators are consecutive in `d`, so d keeps the layout of one 64 x bn accumulator.  Every index is a compile-time
-// constant: d stays in registers.
+// D[64 x bn] (+)= A[64 x 16] * B[bn x 16]^T as 64 / 32 / 16-column pieces for a RUNTIME width (bn: multiple of 16,
+// <= 2 R; the halo kernels).  The pieces' accumulators are consecutive in `d`, so d keeps the layout of one 64 x bn
+// accumulator.  The accumulators are written by predicated asm, so ptxas serialises the wgmma pipeline (each wgmma
+// waits for the previous one); the GEMM kernel issues one wgmma_ss<kBN> per k16 step instead.
 template <int R>
 __device__ __forceinline__ void wgmma_rows64(float (&d)[R], int bn, uint64_t da, uint64_t db, uint32_t acc) {
 #pragma unroll
     for (int c = 0; c + 64 <= 2 * R; c += 64)
-        if (c + 64 <= bn) wgmma_m64n64_ss(d + c / 2, da, db + (c * 128 >> 4), acc);
+        if (c + 64 <= bn) wgmma_ss<64>(d + c / 2, da, db + (c * 128 >> 4), acc);
     const int c32 = bn & ~63;
 #pragma unroll
     for (int c = 0; c + 32 <= 2 * R; c += 64)
-        if (c == c32 && (bn & 32)) wgmma_m64n32_ss(d + c / 2, da, db + (c * 128 >> 4), acc);
+        if (c == c32 && (bn & 32)) wgmma_ss<32>(d + c / 2, da, db + (c * 128 >> 4), acc);
     const int c16 = bn & ~31;
 #pragma unroll
     for (int c = 0; c + 16 <= 2 * R; c += 32)
-        if (c == c16 && (bn & 16)) wgmma_m64n16_ss(d + c / 2, da, db + (c * 128 >> 4), acc);
+        if (c == c16 && (bn & 16)) wgmma_ss<16>(d + c / 2, da, db + (c * 128 >> 4), acc);
 }
 
 // ---- wgmma shared-memory matrix descriptors -------------------------------------------------------------

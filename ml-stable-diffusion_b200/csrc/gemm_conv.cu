@@ -1,7 +1,8 @@
 // b200sd -- wgmma GEMM / im2col-free implicit-GEMM 3x3 convolution for sm_90a.
 //
-// One persistent, warp-specialised kernel:
-//   warp 8      TMA producer  (cp.async.bulk.tensor 2D/4D boxes, SWIZZLE_128B, mbarrier tx)
+// One persistent, warp-specialised kernel, compiled per tile width kBN:
+//   warps 8..11 producer warpgroup: warp 8 issues TMA (cp.async.bulk.tensor 2D/4D boxes, SWIZZLE_128B, mbarrier tx);
+//               the warpgroup gives its registers to the consumers (setmaxnreg)
 //   warps 0..7  two consumer warpgroups: wgmma m64nNk16 (fp16 operands from shared memory, fp32 accumulators in
 //               registers; warpgroup w owns tile rows [64 w, 64 w + 64)), then the epilogue: the accumulators are parked
 //               in shared memory over the drained stages and read back row-wise (bias / time-embedding / GEGLU /
@@ -23,7 +24,13 @@ namespace b200sd {
 static constexpr int kBM = 128;
 static constexpr int kBK = 64;
 static constexpr int kAStage = kBM * kBK * 2;  // 16 KiB
-static constexpr int kGemmThreads = 288;  // warps 0..7: two consumer warpgroups (wgmma + epilogue), warp 8: TMA producer
+// GEMM kernel: warps 0..7 are two consumer warpgroups (wgmma + epilogue), warps 8..11 the producer warpgroup (warp 8,
+// lane 0 issues TMA).  The producer warpgroup hands most of its registers to the consumers (setmaxnreg), so a 64 x 256
+// fp32 accumulator tile (128 registers per thread) fits: 128 x kProducerRegs + 256 x kConsumerRegs <= 65536.
+static constexpr int kGemmThreads = 384;
+static constexpr int kProducerRegs = 40;
+static constexpr int kConsumerRegs = 232;
+static constexpr int kHaloThreads = 288;  // halo kernels: warps 0..7 consumers, warp 8 producer
 static constexpr int kEpiThreads = 256;
 static constexpr int kProducerWarp = 8;
 static constexpr int kMaxStages = 8;
@@ -32,7 +39,7 @@ static constexpr int kSmemBudget = 220 * 1024;
 static constexpr int kEpiFixed = 2 * 256 * 4 + 256 * 4 + 64;  // bias vectors, LayerNorm fold vector, flags + image ids
 
 // Shared-memory budget of one GEMM CTA.  B200SD_SMEM_KB (read per call: tuning scripts flip it) caps the pipeline
-// depth.  The register file holds one 288-thread CTA per SM, so a smaller budget only shortens the pipeline.
+// depth.  The register file holds one GEMM CTA per SM, so a smaller budget only shortens the pipeline.
 static int smem_budget() {
     const char* e = getenv("B200SD_SMEM_KB");
     if (e && e[0]) {
@@ -541,14 +548,16 @@ __device__ __forceinline__ void staged_epilogue(const GemmParams& p, const TileC
     }
 }
 
-// Main loop of one tile on a consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile, all block_n columns, over the
+// Main loop of one tile on a consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile, all kBN columns, over the
 // k-blocks [kb0, kb1) of the ring.  A stage is released (one arrival per warpgroup) once the wgmma that read it retired;
-// one k-block stays in flight behind the one being issued.
-template <int R>
-__device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[R], const uint8_t* smem_a,
-                                              const uint8_t* smem_b, int b_stage, uint64_t* full_bar,
+// one k-block stays in flight behind the one being issued.  One unconditional m64nkBNk16 per k16 step: ptxas only
+// pipelines wgmma whose accumulator registers no predicated instruction writes.
+template <int kBN>
+__device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[kBN / 2], const uint8_t* smem_a,
+                                              const uint8_t* smem_b, uint64_t* full_bar,
                                               uint64_t* empty_bar, int kb0, int kb1, int& stage, uint32_t& phase,
                                               int wg, bool leader) {
+    constexpr int b_stage = kBN * kBK * 2;
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -557,7 +566,7 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k)
-            wgmma_rows64(acc, p.block_n, adesc + 2 * k, bdesc + 2 * k, (kb > kb0 || k > 0) ? 1u : 0u);
+            wgmma_ss<kBN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb > kb0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();
         if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
@@ -568,7 +577,7 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[
         }
     }
     wgmma_wait<0>();
-    wgmma_fence_regs<R>(acc);
+    wgmma_fence_regs<kBN / 2>(acc);
     if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
 }
 
@@ -631,8 +640,54 @@ __device__ __forceinline__ void acc_ld16(const float* src, uint32_t (&v)[16]) {
     }
 }
 
-// kR: accumulator registers per consumer thread (>= block_n / 2): 64 for tiles up to 128 columns, 128 above
-template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kR>
+// Split-K reduction inside a thread-block cluster, run by the 256 consumer threads of every CTA: each CTA has parked its
+// fp32 tile in shared memory; CTA `rank` sums its 1/splits slice of the tile over all peers through DSMEM in rank order
+// (deterministic), applies bias / residual / conversion and stores it.  No workspace round trip, no second launch.
+__device__ __forceinline__ void cluster_splitk_reduce(const GemmParams& p, const uint8_t* smem, int tid) {
+    const TileCoord t = decode_work(p, blockIdx.x);
+    const int ncol0 = t.n_tile * p.block_n;
+    const int ldred = p.block_n + 4;
+    const int q4 = p.block_n >> 2;
+    const int total4 = kBM * q4;
+    const int lo = static_cast<int>(static_cast<long long>(total4) * t.split / p.splits);
+    const int hi = static_cast<int>(static_cast<long long>(total4) * (t.split + 1) / p.splits);
+    const uint32_t red_base = smem_u32(smem);
+    for (int idx = lo + tid; idx < hi; idx += kEpiThreads) {
+        const int r = idx / q4, c4 = idx - r * q4;
+        const int col = ncol0 + c4 * 4;
+        int orow;
+        if (!tile_row(p, t, r, orow) || col >= p.N) continue;
+        const uint32_t la = red_base + static_cast<uint32_t>(r * ldred + c4 * 4) * 4u;
+        float4 a4 = ld_dsmem_f4(la, 0);
+        for (int sp = 1; sp < p.splits; ++sp) {
+            const float4 v = ld_dsmem_f4(la, sp);
+            a4.x += v.x, a4.y += v.y, a4.z += v.z, a4.w += v.w;
+        }
+        if (p.bias != nullptr) {
+            const float4 b = *reinterpret_cast<const float4*>(
+                p.bias + (p.bias_rows > 0 ? (orow / p.bias_rows) * p.bias_stride : 0) + col);
+            a4.x += b.x, a4.y += b.y, a4.z += b.z, a4.w += b.w;
+        }
+        const size_t off = static_cast<size_t>(orow) * p.N + col;
+        if (p.residual != nullptr) {
+            const uint2 rr = *reinterpret_cast<const uint2*>(p.residual + off);
+            const float2 q0 = __half22float2(*reinterpret_cast<const __half2*>(&rr.x));
+            const float2 q1 = __half22float2(*reinterpret_cast<const __half2*>(&rr.y));
+            a4.x += q0.x, a4.y += q0.y, a4.z += q1.x, a4.w += q1.y;
+        }
+        if (p.out_f32) {
+            *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + off) = a4;
+        } else {
+            uint2 pk;
+            pk.x = pack_half2(a4.x, a4.y);
+            pk.y = pack_half2(a4.z, a4.w);
+            *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + off) = pk;
+        }
+    }
+}
+
+// kBN: tile width (columns); p.block_n == kBN.  Each consumer thread holds kBN / 2 fp32 accumulators.
+template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN>
 __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __grid_constant__ GemmParams p) {
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
     // integer-rounded pointer -- lets the compiler emit LDS / STS for everything derived from it; rounding through
@@ -640,7 +695,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw;
     if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
-    const int b_stage = p.block_n * (kBK * 2);
+    constexpr int b_stage = kBN * kBK * 2;
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + p.stages * kAStage;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + p.stages * b_stage);
@@ -682,9 +737,10 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
     const int work0 = blockIdx.x;
     const int work_step = gridDim.x;
 
-    if (warp == kProducerWarp) {
-        // ------------------------------- TMA producer -------------------------------
-        if (lane == 0) {
+    if (warp >= kProducerWarp) {
+        // ------------------------- producer warpgroup: warp 8, lane 0 issues TMA -------------------------
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == kProducerWarp && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             const uint32_t tx_bytes = kAStage + b_stage;
@@ -756,15 +812,21 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
                 }
             }
         }
-    } else if (warp < kProducerWarp) {
+        if (kPartial && p.cluster) {  // the consumers' two cluster barriers around the split-K reduction
+            __syncwarp();
+            cluster_sync_all();
+            cluster_sync_all();
+        }
+    } else {
         // ------------------------- consumers: wgmma main loop, then the epilogue -------------------------
+        setmaxnreg_inc<kConsumerRegs>();
         const int wg = warp >> 2;          // rows [64 wg, 64 wg + 64) of the tile in the main loop
         const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // accumulator rows r0, r0 + 8 of this thread
         const int half = warp >> 2;        // epilogue: which of the two warps of a 32-row group; it takes every other chunk
         const int row = (warp & 3) * 32 + lane;  // epilogue: the tile row this thread owns
         const int tid_e = threadIdx.x;     // 0..255
         const bool leader = (threadIdx.x & 127) == 0;
-        float acc[kR];
+        float acc[kBN / 2];
         int stage = 0;
         uint32_t phase = 0;
         pdl_wait();  // bias / residual / output buffers belong to the stream order
@@ -808,7 +870,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
             }
             const int bias_base = (p.bias_mode == 2 && p.bias_rows > 0 && valid) ? (out_row / p.bias_rows) * p.bias_stride : 0;
 
-            gemm_mainloop(p, acc, smem_a, smem_b, b_stage, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
+            gemm_mainloop<kBN>(p, acc, smem_a, smem_b, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
 
             if (p.res_smem) cp_async_wait_all();
             epi_bar_sync();  // every wgmma of the tile retired: the stages may be overwritten; staged operands visible
@@ -828,7 +890,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
                 stage_accumulators(p, t, acc, tile_s, b0, b1, wg_s, r0, lane);
                 staged_epilogue(p, t, tile_s, scratch, flag_s, warp, lane, res_pre);
             } else {
-                park_accumulators(acc, p.block_n, acc_s, lda, r0, lane);
+                park_accumulators(acc, kBN, acc_s, lda, r0, lane);
                 epi_bar_sync();
                 if (!(kPartial && p.cluster)) {  // cluster split-K: the parked tile is what the peers reduce
                     const float* arow = acc_s + row * lda;
@@ -888,59 +950,33 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
             epi_bar_sync();  // everyone is done with the accumulator / staging tiles and the staged bias / residual
             if (threadIdx.x == 0) mbar_arrive(acc_free);
         }
-    }
-
-    if (kPartial && p.cluster) {
-        // ---- split-K reduction inside the cluster: every CTA has parked its fp32 tile in shared memory; CTA `rank`
-        // sums its 1/splits slice of the tile over all peers through DSMEM in rank order (deterministic), applies
-        // bias / residual / conversion and stores it.  No workspace round trip, no second launch. ----
-        __syncwarp();
-        pdl_wait();  // (the producer warp: the reduction below reads bias / residual and writes the output)
-        cluster_sync_all();
-        const TileCoord t = decode_work(p, blockIdx.x);
-        const int ncol0 = t.n_tile * p.block_n;
-        const int ldred = p.block_n + 4;
-        const int q4 = p.block_n >> 2;
-        const int total4 = kBM * q4;
-        const int lo = static_cast<int>(static_cast<long long>(total4) * t.split / p.splits);
-        const int hi = static_cast<int>(static_cast<long long>(total4) * (t.split + 1) / p.splits);
-        const uint32_t red_base = smem_u32(smem);
-        for (int idx = lo + static_cast<int>(threadIdx.x); idx < hi; idx += kGemmThreads) {
-            const int r = idx / q4, c4 = idx - r * q4;
-            const int col = ncol0 + c4 * 4;
-            int orow;
-            if (!tile_row(p, t, r, orow) || col >= p.N) continue;
-            const uint32_t la = red_base + static_cast<uint32_t>(r * ldred + c4 * 4) * 4u;
-            float4 a4 = ld_dsmem_f4(la, 0);
-            for (int sp = 1; sp < p.splits; ++sp) {
-                const float4 v = ld_dsmem_f4(la, sp);
-                a4.x += v.x, a4.y += v.y, a4.z += v.z, a4.w += v.w;
-            }
-            if (p.bias != nullptr) {
-                const float4 b = *reinterpret_cast<const float4*>(
-                    p.bias + (p.bias_rows > 0 ? (orow / p.bias_rows) * p.bias_stride : 0) + col);
-                a4.x += b.x, a4.y += b.y, a4.z += b.z, a4.w += b.w;
-            }
-            const size_t off = static_cast<size_t>(orow) * p.N + col;
-            if (p.residual != nullptr) {
-                const uint2 rr = *reinterpret_cast<const uint2*>(p.residual + off);
-                const float2 q0 = __half22float2(*reinterpret_cast<const __half2*>(&rr.x));
-                const float2 q1 = __half22float2(*reinterpret_cast<const __half2*>(&rr.y));
-                a4.x += q0.x, a4.y += q0.y, a4.z += q1.x, a4.w += q1.y;
-            }
-            if (p.out_f32) {
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + off) = a4;
-            } else {
-                uint2 pk;
-                pk.x = pack_half2(a4.x, a4.y);
-                pk.y = pack_half2(a4.z, a4.w);
-                *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + off) = pk;
-            }
+        if (kPartial && p.cluster) {  // every CTA of the cluster has parked its tile (one tile per CTA)
+            cluster_sync_all();
+            cluster_splitk_reduce(p, smem, threadIdx.x);
+            cluster_sync_all();  // nobody leaves (or frees its shared memory) while a peer may still read it
         }
-        cluster_sync_all();  // nobody leaves (or frees its shared memory) while a peer may still read it
     }
 }
 
+
+// Tile widths the GEMM kernel is compiled for; plan_gemm chooses among exactly these (widest first).
+static constexpr int kGemmWidths[] = {256, 192, 160, 128, 96, 64, 32, 16};
+static constexpr int kNumGemmWidths = sizeof(kGemmWidths) / sizeof(kGemmWidths[0]);
+static int gemm_width_index(int bn) {
+    for (int i = 0; i < kNumGemmWidths; ++i)
+        if (kGemmWidths[i] == bn) return i;
+    return -1;
+}
+using KernelFn = void (*)(GemmParams);
+template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged>
+static KernelFn gemm_kernel(int width_index) {
+#define B200SD_GEMM_FN(bn) wgmma_gemm_kernel<kGeneric, kGeglu, kOutF32, kPartial, kStaged, bn>
+    static const KernelFn fns[kNumGemmWidths] = {B200SD_GEMM_FN(256), B200SD_GEMM_FN(192), B200SD_GEMM_FN(160),
+                                                 B200SD_GEMM_FN(128), B200SD_GEMM_FN(96),  B200SD_GEMM_FN(64),
+                                                 B200SD_GEMM_FN(32),  B200SD_GEMM_FN(16)};
+#undef B200SD_GEMM_FN
+    return fns[width_index];
+}
 
 // =====================================================================================================================
 // Halo-reuse 3x3 convolution (mode 2) with GroupNorm-apply + SiLU fused into the operand path
@@ -978,7 +1014,7 @@ __device__ __forceinline__ void ldr_bar_sync() { asm volatile("bar.sync 1, 256;"
 // fill for the padding ring and the pad column) and the consumer warps use the register epilogue of the GEMM kernel.
 // kR: accumulator registers per consumer thread (block_n / 2): the loader kinds hold the patch vectors in registers too.
 template <int kKind, int kR>
-__global__ void __launch_bounds__(kGemmThreads, 1) halo_conv_kernel(const __grid_constant__ GemmParams p) {
+__global__ void __launch_bounds__(kHaloThreads, 1) halo_conv_kernel(const __grid_constant__ GemmParams p) {
     constexpr bool kFp32Direct = kKind == 1;
     constexpr bool kTmaPatch = kKind == 2;
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
@@ -1563,18 +1599,20 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
         pl.m_tiles = pl.tiles_w * pl.tiles_h * pl.tiles_n;
     }
     if (a.geglu) B200SD_REQUIRE(a.n % 16 == 0, "b200sd_gemm: GEGLU needs n %% 16 == 0");
-    // ---- tile shape / split-K selection by a small cost model (cycles per SM; constants fitted to B200 runs, not
-    // refitted for H100 -- tools/bench_gemm_shapes.py measures the shapes they are fitted to) ----
+    // ---- tile shape / split-K selection by a small cost model (cycles per SM).  The constants were fitted to B200 runs;
+    // checked on an H100 (400 W) with tools/bench_gemm_shapes.py over the 28 SD-2.1 shapes it times: the plans this model
+    // picks take 1080 us in total against 1058 us for the fastest candidate of every shape (2 %, about the run-to-run
+    // spread of a single shape), so they were kept.  The largest misses: conv 2560->1280 at 8x8 (1.3x) and linear
+    // 1280->1280 at M = 512 (1.25x). ----
     const int sms = num_sms();
     const bool can_split = !a.geglu && a.n % 4 == 0 && a.act == 0 && !want_stats && a.ln_parts == 0;
     auto epi_cycles = [&](int bn) { return 400.0 + (bn / 32.0) * (a.geglu ? 520.0 : 230.0); };
     auto kb_cycles = [&](int bn) { return std::max(2.0 * bn, (kAStage + 128.0 * bn) / 38.0); };
     double best_t = 1e30;
     int best_bn = 0, best_s = 1, best_cluster = 0;
-    static const int kBns[] = {256, 224, 192, 160, 128, 96, 64, 32, 16};
     static const int kSplits[] = {1, 2, 3, 4, 6, 8, 12, 16, 24, 32};
     const bool can_cluster = can_split && cluster_splitk_enabled() && a.n % 16 == 0;
-    for (int bn : kBns) {
+    for (int bn : kGemmWidths) {
         if (a.block_n > 0 && bn != a.block_n) continue;
         const int nt = (a.n + bn - 1) / bn;
         if (a.block_n == 0 && bn > 16 && nt * bn > a.n + a.n / 4 + 15) continue;  // > 25 % padding
@@ -1616,7 +1654,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
         best_bn = a.block_n > 0 ? a.block_n : 128;
         best_s = a.split_k > 0 ? a.split_k : 1;
     }
-    B200SD_REQUIRE(best_bn % 16 == 0 && best_bn >= 16 && best_bn <= 256, "b200sd_gemm: block_n %d", best_bn);
+    B200SD_REQUIRE(gemm_width_index(best_bn) >= 0, "b200sd_gemm: block_n %d is not a compiled tile width", best_bn);
     pl.block_n = best_bn;
     pl.n_tiles = (a.n + pl.block_n - 1) / pl.block_n;
     int splits = std::max(1, std::min(best_s, pl.kb_total));
@@ -1850,7 +1888,7 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
             hattr[hslot] = true;
         }
         const int units = pl.m_tiles * pl.n_tiles;
-        B200SD_CHECK_CUDA(launch_kernel(hfn, dim3(std::min(units, num_sms())), dim3(kGemmThreads), pl.smem_bytes, stream, p));
+        B200SD_CHECK_CUDA(launch_kernel(hfn, dim3(std::min(units, num_sms())), dim3(kHaloThreads), pl.smem_bytes, stream, p));
         B200SD_CHECK_CUDA(cudaGetLastError());
         count_launch(1);
         return 0;
@@ -1863,38 +1901,34 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
     B200SD_REQUIRE(a.act == 0 || (a.act >= 1 && a.act <= 3 && pl.splits == 1 && !a.geglu), "b200sd_gemm: act=%d unsupported here", a.act);
     const bool regular = (a.act == 0) && (a.n % 16 == 0) && (p.n_store % 8 == 0) && (pl.block_n % 32 == 0) && pl.bias_mode != 2 &&
                          (a.residual == nullptr || pl.res_smem || pl.splits > 1 || pl.staged);
-    using KernelFn = void (*)(GemmParams);
+    const int wi = gemm_width_index(pl.block_n);
     KernelFn fn;
     int variant;
-    const bool wide = pl.block_n > 128;
-#define B200SD_GEMM_FN(g, gl, f32, part, st) (wide ? wgmma_gemm_kernel<g, gl, f32, part, st, 128> : wgmma_gemm_kernel<g, gl, f32, part, st, 64>)
     if (!regular) {
-        fn = B200SD_GEMM_FN(true, false, false, false, false), variant = 0;
+        fn = gemm_kernel<true, false, false, false, false>(wi), variant = 0;
     } else if (pl.staged) {
-        fn = B200SD_GEMM_FN(false, false, false, false, true), variant = 5;
+        fn = gemm_kernel<false, false, false, false, true>(wi), variant = 5;
     } else if (pl.splits > 1) {
-        fn = B200SD_GEMM_FN(false, false, false, true, false), variant = 1;
+        fn = gemm_kernel<false, false, false, true, false>(wi), variant = 1;
     } else if (a.geglu) {
-        fn = B200SD_GEMM_FN(false, true, false, false, false), variant = 2;
+        fn = gemm_kernel<false, true, false, false, false>(wi), variant = 2;
     } else if (a.out_f32) {
-        fn = B200SD_GEMM_FN(false, false, true, false, false), variant = 3;
+        fn = gemm_kernel<false, false, true, false, false>(wi), variant = 3;
     } else {
-        fn = B200SD_GEMM_FN(false, false, false, false, false), variant = 4;
+        fn = gemm_kernel<false, false, false, false, false>(wi), variant = 4;
     }
-#undef B200SD_GEMM_FN
-    if (wide) variant += 6;
     if (pl.splits > 1 && !pl.cluster) {
         // the separate reduce kernel applies bias / residual; the partial writer must not
         p.bias = nullptr;
         p.residual = nullptr;
     }
-    static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
-    if (!attr_set[variant]) {
+    static bool attr_set[6][kNumGemmWidths] = {};
+    if (!attr_set[variant][wi]) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set[variant] = true;
+        attr_set[variant][wi] = true;
     }
     if (pl.cluster) {
-        B200SD_REQUIRE(variant % 6 == 1, "b200sd_gemm: cluster split-K needs the regular epilogue variant");
+        B200SD_REQUIRE(variant == 1, "b200sd_gemm: cluster split-K needs the regular epilogue variant");
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
         // split-K: one (tile, split) per CTA, the splits of a tile are one cluster
