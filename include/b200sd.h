@@ -192,6 +192,7 @@ int b200sd_softmax_rows(const float* in, void* out, int32_t rows, int32_t cols, 
  * q [batch, sq, ldq] / k,v [batch, sk, ldk] fp16 token-major with head h in columns
  * [h*d, (h+1)*d) of the given base pointers; out [batch, sq, ldo].  d must be 64.
  * mask: optional fp32 additive [batch, sk] (unet.py:99-114) or NULL.
+ * scale: multiplies q k^T before the softmax; must be > 0 (the kernel takes row maxima of the unscaled scores).
  * impl: 0 ORIGINAL, 1 SPLIT_EINSUM, 2 SPLIT_EINSUM_V2 (tile policy only; same result);
  *       | 0x100 adds the causal mask of the CLIP text encoder (key j visible to query i iff j <= i). */
 int b200sd_attention(const void* q, const void* k, const void* v, void* out, const float* mask,
@@ -200,7 +201,7 @@ int b200sd_attention(const void* q, const void* k, const void* v, void* out, con
                      void* stream);
 /* The same with a caller-provided device workspace of b200sd_attention_workspace_bytes() bytes, which lets the launch
  * cut the (query tile x K/V tile) work into equal per-CTA ranges ("stream-K") when whole query tiles would fill the GPU
- * badly (S = 4096: 320 tiles on 296 CTA slots).  Pieces of a split tile meet in the workspace and are merged in a fixed
+ * badly (S = 4096: 320 tiles on 132 CTA slots).  Pieces of a split tile meet in the workspace and are merged in a fixed
  * order, so results are reproducible.  The workspace must be zero-filled once before its first use (the kernel leaves its
  * counters at zero) and must not be shared with a concurrently running attention launch. */
 size_t b200sd_attention_workspace_bytes(void);

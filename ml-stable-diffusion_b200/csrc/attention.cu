@@ -7,9 +7,12 @@
 // three variants are one function, softmax(q^T k / sqrt(d) + mask) v per (batch, head); the
 // (B, heads, Sq, Sk) score tensor the reference materialises (671 MB at S=4096) never leaves the SM.
 //
-// CTA = 128 queries x 1 head; warps 0..7 are two consumer warpgroups (64 query rows each), warp 8 the TMA producer.
-// The K/V ring holds two 128-key tiles; each warpgroup walks them in 64-key halves: S_h = Q K_h^T, softmax, O += P_h V_h.
-// While one warpgroup is in its exponentials the other one keeps the tensor core busy.
+// CTA = 128 queries x 1 head; warps 0..7 are two consumer warpgroups (64 query rows each), warps 8..11 the producer
+// warpgroup (warp 8, lane 0 issues TMA; the warpgroup hands most of its registers to the consumers).  K and V tiles of
+// 128 keys sit in a kKvStages-deep ring with separate full / empty barriers.  Each consumer step j issues S_j = Q K_j^T
+// and, behind it, O += P_{j-1} V_{j-1}; the exponentials of S_j run while that PV product is still on the tensor core.
+// The two warpgroups issue independently: with the softmax already under the PV product, making them take turns
+// (named-barrier ping-pong) measured 2-3 % slower at S = 4096.
 #include "common.cuh"
 #include "../../include/b200sd.h"
 
@@ -18,13 +21,16 @@ namespace b200sd {
 extern void count_launch(int n);
 
 static constexpr int kQ = 128;   // queries per CTA
-static constexpr int kKV = 128;  // keys per K/V tile (one TMA load)
-static constexpr int kHalf = 64;  // keys per pipeline step
+static constexpr int kKV = 128;  // keys per K/V tile (one TMA load) = keys per pipeline step
 static constexpr int kD = 64;    // head dim
-static constexpr int kAttnThreads = 288;
+static constexpr int kAttnThreads = 384;
 static constexpr int kProducerWarp = 8;
+// 128 x kAttnProducerRegs + 256 x kAttnConsumerRegs <= 65536
+static constexpr int kAttnProducerRegs = 24;
+static constexpr int kAttnConsumerRegs = 240;
 static constexpr int kTileBytes = 128 * 64 * 2;  // 16 KiB: one [128 x 64] fp16 tile
-static constexpr int kKvStages = 2;
+static constexpr int kKvStages = 3;
+static constexpr int kMergeBar = 1;  // named barrier of the consumers' stream-K merge
 
 struct __align__(64) AttnParams {
     CUtensorMap tmQ, tmK, tmV;
@@ -47,7 +53,7 @@ struct __align__(64) AttnParams {
 static constexpr int kPartialFloats = (kD + 2) * kQ;
 static constexpr size_t kCounterBytes = 64 * 1024;
 
-// smem layout (1024-aligned): Q | K[2] | V[2] | barriers
+// smem layout (1024-aligned): Q | K[kKvStages] | V[kKvStages] | barriers
 static constexpr int kSmemQ = 0;
 static constexpr int kSmemK = kSmemQ + kTileBytes;
 static constexpr int kSmemV = kSmemK + kKvStages * kTileBytes;
@@ -87,21 +93,22 @@ struct SegmentWalk {
     }
 };
 
-// number of 64-key halves a segment visits (the last K/V tile may be ragged; causal tiles stop at the diagonal)
-__device__ __forceinline__ int segment_halves(const AttnParams& p, const AttnSegment& sg, int q0) {
+// number of K/V tiles a segment visits (>= 1; causal tiles stop at the diagonal)
+__device__ __forceinline__ int segment_steps(const AttnParams& p, const AttnSegment& sg, int q0) {
     const int sk_eff = p.causal ? min(p.sk, q0 + kQ) : p.sk;
-    const int n_half = (sk_eff + kHalf - 1) / kHalf;
-    return min(2 * sg.k1, n_half) - 2 * sg.k0;
+    return min(sg.k1, (sk_eff + kKV - 1) / kKV) - sg.k0;
 }
 
 __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid_constant__ AttnParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSmemBar);
     uint64_t* q_full = bars + 0;
-    uint64_t* kv_full = bars + 1;   // [2]
-    uint64_t* kv_empty = bars + 3;  // [2]
-    uint64_t* q_empty = bars + 5;   // every S MMA of the segment retired: Q may be overwritten
-    int* last_flag = reinterpret_cast<int*>(bars + 6);
+    uint64_t* q_empty = bars + 1;  // every S MMA of the segment retired: Q may be overwritten
+    uint64_t* k_full = bars + 2;                   // [kKvStages]
+    uint64_t* k_empty = k_full + kKvStages;        // [kKvStages] released once S_j retired
+    uint64_t* v_full = k_empty + kKvStages;        // [kKvStages]
+    uint64_t* v_empty = v_full + kKvStages;        // [kKvStages] released once P_j V_j retired
+    int* last_flag = reinterpret_cast<int*>(v_empty + kKvStages);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -116,8 +123,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
         mbar_init(q_full, 1);
         mbar_init(q_empty, 2);
         for (int s = 0; s < kKvStages; ++s) {
-            mbar_init(&kv_full[s], 1);
-            mbar_init(&kv_empty[s], 2);  // one arrival per consumer warpgroup
+            mbar_init(&k_full[s], 1);
+            mbar_init(&v_full[s], 1);
+            mbar_init(&k_empty[s], 2);  // one arrival per consumer warpgroup
+            mbar_init(&v_empty[s], 2);
         }
         fence_barrier_init();
     }
@@ -125,131 +134,208 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
     pdl_trigger();
     pdl_wait();     // PDL: the prologue above overlapped the previous kernel's tail
 
-    // Both roles walk the same segment list.  The K/V tile counter jg runs ACROSS segments (smem stage jg % 2).
+    // Both roles walk the same segment list.  The K/V tile counter jg runs ACROSS segments (smem stage jg % kKvStages).
     SegmentWalk walk;
     walk.init(p);
     AttnSegment sg;
 
-    if (warp == kProducerWarp) {
-        if (lane == 0) {
+    if (warp >= kProducerWarp) {
+        setmaxnreg_dec<kAttnProducerRegs>();
+        if (warp == kProducerWarp && lane == 0) {
             int seg = 0, jg = 0;
             while (walk.next(p, sg)) {
                 const int qt = sg.tile % p.q_tiles, head = (sg.tile / p.q_tiles) % p.heads, batch = sg.tile / (p.q_tiles * p.heads);
-                const int nh = segment_halves(p, sg, qt * kQ);
+                const int ns = segment_steps(p, sg, qt * kQ);
                 if (seg > 0) mbar_wait(q_empty, (seg - 1) & 1);
                 mbar_expect_tx(q_full, kTileBytes);
                 tma_load_3d(smem + kSmemQ, &p.tmQ, q_full, head * kD, qt * kQ, batch, kEvictFirst);
-                for (int jl = 0; jl < (nh + 1) / 2; ++jl, ++jg) {
+                for (int jl = 0; jl < ns; ++jl, ++jg) {
                     const int st = jg % kKvStages;
                     const uint32_t ph = (jg / kKvStages) & 1;
-                    mbar_wait(&kv_empty[st], ph ^ 1);
-                    mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
-                    tma_load_3d(smem + kSmemK + st * kTileBytes, &p.tmK, &kv_full[st], head * kD, (sg.k0 + jl) * kKV, batch,
+                    mbar_wait(&k_empty[st], ph ^ 1);
+                    mbar_expect_tx(&k_full[st], kTileBytes);
+                    tma_load_3d(smem + kSmemK + st * kTileBytes, &p.tmK, &k_full[st], head * kD, (sg.k0 + jl) * kKV, batch,
                                 kEvictLast);
-                    tma_load_3d(smem + kSmemV + st * kTileBytes, &p.tmV, &kv_full[st], head * kD, (sg.k0 + jl) * kKV, batch,
+                    mbar_wait(&v_empty[st], ph ^ 1);
+                    mbar_expect_tx(&v_full[st], kTileBytes);
+                    tma_load_3d(smem + kSmemV + st * kTileBytes, &p.tmV, &v_full[st], head * kD, (sg.k0 + jl) * kKV, batch,
                                 kEvictLast);
                 }
                 ++seg;
             }
         }
-    } else if (warp < kProducerWarp) {
+    } else {
         // ---------------- consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) of the tile ----------------
-        // Accumulator layout (m64n64): this thread holds rows lr and lr + 8 (lr = 16 (warp % 4) + lane / 4 inside the
-        // warpgroup's 64), columns 8 j + 2 (lane % 4) + {0, 1}, j = 0..7: s[4 j + {0, 1}] row lr, s[4 j + {2, 3}] row lr + 8.
+        setmaxnreg_inc<kAttnConsumerRegs>();
+        // Accumulator layout (m64nN): this thread holds rows lr and lr + 8 (lr = 16 (warp % 4) + lane / 4 inside the
+        // warpgroup's 64), columns 8 j + 2 (lane % 4) + {0, 1}: x[4 j + {0, 1}] row lr, x[4 j + {2, 3}] row lr + 8.
         // A row is spread over the four lanes of a quad: row maxima / sums reduce with two shuffles.
         const int wg = warp >> 2;
-        const int lr = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile-local row of s[.. 0, 1]; lr + 8 for s[.. 2, 3]
+        const int lr = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile-local row of x[.. 0, 1]; lr + 8 for x[.. 2, 3]
         const int cq = 2 * (lane & 3);
         const bool leader = (threadIdx.x & 127) == 0;
         const float sl2 = p.scale_log2;
         const uint32_t q_addr = smem_u32(smem + kSmemQ) + wg * 64 * 128;
+        const uint64_t qdesc = make_smem_desc_sw128(q_addr, 1024, 0);
+
         int seg = 0, jg0 = 0;
         while (walk.next(p, sg)) {
             const int qt = sg.tile % p.q_tiles, head = (sg.tile / p.q_tiles) % p.heads, batch = sg.tile / (p.q_tiles * p.heads);
             const int q0 = qt * kQ;
-            const int nh = segment_halves(p, sg, q0);
+            const int ns = segment_steps(p, sg, q0);
             const float* mask_row = p.mask ? p.mask + static_cast<size_t>(batch) * p.sk : nullptr;
             float o[32];
 #pragma unroll
             for (int i = 0; i < 32; ++i) o[i] = 0.f;
             float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-            mbar_wait(q_full, seg & 1);
-            for (int hl = 0; hl < nh; ++hl) {
-                const int jg = jg0 + (hl >> 1), st = jg % kKvStages, hi = hl & 1;
-                if (hi == 0) mbar_wait(&kv_full[st], (jg / kKvStages) & 1);
-                // ---- S = Q K_h^T ----
-                float s[32];
-                const uint64_t qdesc = make_smem_desc_sw128(q_addr, 1024, 0);
-                const uint64_t kdesc = make_smem_desc_sw128(smem_u32(smem + kSmemK + st * kTileBytes) + hi * (kHalf * 128), 1024, 0);
-                wgmma_fence();
+            float s[64];         // S_j, then its probabilities (fp32)
+            uint32_t pa[8][4];   // P_{j-1} as fp16 A fragments: pa[kk] covers keys [16 kk, 16 kk + 16)
+            float factor[2];     // rescale of O for S_j's new row maxima, applied once P_{j-1} V_{j-1} retired
+
+            auto issue_s = [&](int st) {
+                const uint64_t kdesc = make_smem_desc_sw128(smem_u32(smem + kSmemK + st * kTileBytes), 1024, 0);
 #pragma unroll
-                for (int k = 0; k < kD / 16; ++k) wgmma_ss<64>(s, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
+                for (int k = 0; k < kD / 16; ++k) wgmma_ss<128>(s, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
                 wgmma_commit();
-                wgmma_wait<0>();
-                wgmma_fence_regs<32>(s);
-                if (hl == nh - 1 && leader) mbar_arrive(q_empty);  // the segment's last read of Q retired
-                // ---- online softmax (log2 domain) ----
-                const int h = 2 * sg.k0 + hl;                     // this half's position among the keys
-                const int kvalid = min(kHalf, p.sk - h * kHalf);  // >= 1
-                // causal: a half whose last key is <= the tile's first query is fully visible to every row
-                const bool diag = p.causal && (h * kHalf + kHalf - 1 > q0);
-                const bool general = mask_row != nullptr || kvalid < kHalf || diag;
+            };
+            // B = the V tile [keys][d] = MN-major, 16 keys = 2048 B per k16 step
+            auto issue_pv = [&](int st) {
+                const uint32_t v_addr = smem_u32(smem + kSmemV + st * kTileBytes);
 #pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    float v = s[e] * sl2;
-                    if (general) {
-                        const int key = 8 * (e >> 2) + cq + (e & 1);
-                        const int qi = q0 + lr + 8 * ((e >> 1) & 1);
-                        const bool vis = key < kvalid && (!diag || h * kHalf + key <= qi);
-                        if (mask_row != nullptr && vis) v += mask_row[h * kHalf + key] * 1.4426950408889634f;
-                        if (!vis) v = -INFINITY;
-                    }
-                    s[e] = v;
-                }
-                float m_use[2];
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    float mx = -INFINITY;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * r], s[4 * j + 2 * r + 1]));
-                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                    const float m_new = fmaxf(m_run[r], mx);
-                    m_use[r] = m_new == -INFINITY ? 0.f : m_new;  // a row with nothing visible yet
-                    const float factor = ex2_approx(m_run[r] - m_use[r]);
-                    m_run[r] = m_new;
-                    l_run[r] *= factor;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) o[4 * j + 2 * r] *= factor, o[4 * j + 2 * r + 1] *= factor;
-                }
-                uint32_t pa[4][4];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float p0 = ex2_approx(s[4 * j] - m_use[0]), p1 = ex2_approx(s[4 * j + 1] - m_use[0]);
-                    const float p2 = ex2_approx(s[4 * j + 2] - m_use[1]), p3 = ex2_approx(s[4 * j + 3] - m_use[1]);
-                    l_run[0] += p0 + p1;
-                    l_run[1] += p2 + p3;
-                    // A fragment of keys [16 kk, 16 kk + 16): {row lr, keys 0..7}, {lr + 8, 0..7}, {lr, 8..15}, {lr + 8, 8..15}
-                    pa[j >> 1][2 * (j & 1)] = pack_half2(p0, p1);
-                    pa[j >> 1][2 * (j & 1) + 1] = pack_half2(p2, p3);
-                }
-                // ---- O += P V_h: B = 64 rows of the V tile [keys][d] = MN-major, 16 keys = 2048 B per step ----
-                const uint32_t v_addr = smem_u32(smem + kSmemV + st * kTileBytes) + hi * (kHalf * 128);
-                wgmma_fence();
-#pragma unroll
-                for (int kk = 0; kk < kHalf / 16; ++kk)
+                for (int kk = 0; kk < kKV / 16; ++kk)
                     wgmma_m64n64_rs_tb(o, pa[kk], make_smem_desc_sw128(v_addr + kk * 2048, 1024, kKV * 128), 1u);
                 wgmma_commit();
+            };
+            // online softmax (log2 domain) of S_j in place; touches neither o nor pa (P_{j-1} V_{j-1} may be in flight).
+            // The fast path leaves raw scores in s and folds the scale into the exponent's FFMA; the general path stores
+            // scaled scores (mask added, invisible keys at -inf).  Called as `if (general) softmax(j, true); else
+            // softmax(j, false);` so that each variant is a block of its own: ptxas hoists a wgmma wait to the top of
+            // the basic block it sits in, and a wait<0> in the same block as the exponentials would run them after the
+            // PV product instead of under it.
+            auto softmax = [&](int j, bool general) {
+                const int h = sg.k0 + j;                      // this K/V tile's position among the keys
+                const int kvalid = min(kKV, p.sk - h * kKV);  // >= 1
+                // causal: a tile whose last key is <= the tile's first query is fully visible to every row
+                const bool diag = p.causal && (h * kKV + kKV - 1 > q0);
+                const float sc = general ? 1.f : sl2;
+                if (general) {
+#pragma unroll
+                    for (int e = 0; e < 64; ++e) {
+                        const int key = 8 * (e >> 2) + cq + (e & 1);
+                        const int qi = q0 + lr + 8 * ((e >> 1) & 1);
+                        const bool vis = key < kvalid && (!diag || h * kKV + key <= qi);
+                        float v = s[e] * sl2;
+                        if (mask_row != nullptr && vis) v += mask_row[h * kKV + key] * 1.4426950408889634f;
+                        s[e] = vis ? v : -INFINITY;
+                    }
+                }
+                // row maxima and sums as trees of 8 partials: with two consumer warps per scheduler there is little to
+                // hide a 32-long dependency chain behind
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    float t[8];
+#pragma unroll
+                    for (int c = 0; c < 8; ++c)
+                        t[c] = fmaxf(fmaxf(s[8 * c + 2 * r], s[8 * c + 2 * r + 1]), fmaxf(s[8 * c + 4 + 2 * r], s[8 * c + 5 + 2 * r]));
+#pragma unroll
+                    for (int w = 4; w >= 1; w >>= 1)
+#pragma unroll
+                        for (int c = 0; c < w; ++c) t[c] = fmaxf(t[c], t[c + w]);
+                    float mx = t[0];
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    const float m_new = fmaxf(m_run[r], mx * sc);
+                    const float m_use = m_new == -INFINITY ? 0.f : m_new;  // a row with nothing visible yet
+                    factor[r] = ex2_approx(m_run[r] - m_use);
+                    m_run[r] = m_new;
+#pragma unroll
+                    for (int c = 0; c < 16; ++c) {
+                        s[4 * c + 2 * r] = ex2_approx(fmaf(s[4 * c + 2 * r], sc, -m_use));
+                        s[4 * c + 2 * r + 1] = ex2_approx(fmaf(s[4 * c + 2 * r + 1], sc, -m_use));
+                    }
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) t[c] = (s[8 * c + 2 * r] + s[8 * c + 2 * r + 1]) + (s[8 * c + 4 + 2 * r] + s[8 * c + 5 + 2 * r]);
+#pragma unroll
+                    for (int w = 4; w >= 1; w >>= 1)
+#pragma unroll
+                        for (int c = 0; c < w; ++c) t[c] += t[c + w];
+                    l_run[r] = fmaf(l_run[r], factor[r], t[0]);
+                }
+            };
+            auto is_general = [&](int j) {
+                const int h = sg.k0 + j;
+                return mask_row != nullptr || p.sk - h * kKV < kKV || (p.causal && h * kKV + kKV - 1 > q0);
+            };
+            // once P_{j-1} V_{j-1} retired: rescale O, and S_j's probabilities become the next A operand
+            auto rescale_and_pack = [&]() {
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    o[4 * c] *= factor[0], o[4 * c + 1] *= factor[0];
+                    o[4 * c + 2] *= factor[1], o[4 * c + 3] *= factor[1];
+                }
+                // A fragment of keys [16 kk, 16 kk + 16): {row lr, keys 0..7}, {lr + 8, 0..7}, {lr, 8..15}, {lr + 8, 8..15}
+#pragma unroll
+                for (int c = 0; c < 16; ++c) {
+                    pa[c >> 1][2 * (c & 1)] = pack_half2(s[4 * c], s[4 * c + 1]);
+                    pa[c >> 1][2 * (c & 1) + 1] = pack_half2(s[4 * c + 2], s[4 * c + 3]);
+                }
+            };
+
+            mbar_wait(q_full, seg & 1);
+            // ---- step 0: S_0 alone ----
+            {
+                const int st = jg0 % kKvStages;
+                mbar_wait(&k_full[st], (jg0 / kKvStages) & 1);
+                wgmma_fence();
+                issue_s(st);
+                wgmma_wait<0>();
+                wgmma_fence_regs<64>(s);
+                if (leader) {
+                    mbar_arrive(&k_empty[st]);
+                    if (ns == 1) mbar_arrive(q_empty);  // the segment's last read of Q retired
+                }
+                if (is_general(0)) softmax(0, true);
+                else softmax(0, false);
+                rescale_and_pack();
+            }
+            // ---- steps 1..ns-1: S_j and P_{j-1} V_{j-1} in one burst; softmax(S_j) overlaps the PV product ----
+            for (int j = 1; j < ns; ++j) {
+                const int jg = jg0 + j, st = jg % kKvStages, sp = (jg - 1) % kKvStages;
+                mbar_wait(&k_full[st], (jg / kKvStages) & 1);
+                mbar_wait(&v_full[sp], ((jg - 1) / kKvStages) & 1);
+                wgmma_fence();
+                issue_s(st);
+                issue_pv(sp);
+                wgmma_wait<1>();  // S_j retired; P_{j-1} V_{j-1} may still run
+                wgmma_fence_regs<64>(s);
+                if (leader) {
+                    mbar_arrive(&k_empty[st]);
+                    if (j == ns - 1) mbar_arrive(q_empty);
+                }
+                if (is_general(j)) softmax(j, true);
+                else softmax(j, false);
                 wgmma_wait<0>();
                 wgmma_fence_regs<32>(o);
-                if ((hi == 1 || hl == nh - 1) && leader) mbar_arrive(&kv_empty[st]);  // last half of this K/V tile
+                wgmma_fence_regs<64>(s);  // keeps the repacking of P behind the wait: P_{j-1} V_{j-1} reads pa
+                if (leader) mbar_arrive(&v_empty[sp]);
+                rescale_and_pack();
+            }
+            // ---- last PV ----
+            {
+                const int jg = jg0 + ns - 1, st = jg % kKvStages;
+                mbar_wait(&v_full[st], (jg / kKvStages) & 1);
+                wgmma_fence();
+                issue_pv(st);
+                wgmma_wait<0>();
+                wgmma_fence_regs<32>(o);
+                if (leader) mbar_arrive(&v_empty[st]);
             }
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
                 l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
                 l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
             }
-            ++seg, jg0 += (nh + 1) / 2;
+            ++seg, jg0 += ns;
             if (sg.k0 == 0 && sg.k1 == p.n_kv) {
                 // whole query tile in this CTA: normalise and store
 #pragma unroll
@@ -282,14 +368,14 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
                     }
                 }
                 __threadfence();
-                named_bar_sync(1, 256);
+                named_bar_sync(kMergeBar, 256);
                 if (threadIdx.x == 0) {
                     const int old = atomicAdd(p.counters + sg.tile, 1);
                     const int is_last = old == last - first;
                     if (is_last) p.counters[sg.tile] = 0;  // every piece has checked in: ready for the next launch
                     *last_flag = is_last;
                 }
-                named_bar_sync(1, 256);
+                named_bar_sync(kMergeBar, 256);
                 if (*last_flag) {
                     __threadfence();
                     // merge: thread t takes row t % 128, head-dim columns [32 (t / 128), + 32)
@@ -333,7 +419,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
                         }
                     }
                 }
-                named_bar_sync(1, 256);  // last_flag is rewritten by the next segment
+                named_bar_sync(kMergeBar, 256);  // last_flag is rewritten by the next segment
             }
         }
     }
@@ -373,6 +459,8 @@ extern "C" int b200sd_attention_ws(const void* q, const void* k, const void* v, 
     B200SD_REQUIRE(d == kD, "b200sd_attention: head dim %d not supported by this kernel (needs 64)", d);
     B200SD_REQUIRE(impl >= 0 && (impl & 0xff) <= 2 && (impl & ~0x1ff) == 0, "b200sd_attention: unknown attention implementation %d", impl);
     B200SD_REQUIRE(batch > 0 && heads > 0 && sq > 0 && sk > 0, "b200sd_attention: bad sizes");
+    // the softmax takes row maxima of the unscaled scores and scales them afterwards: only valid for a positive scale
+    B200SD_REQUIRE(scale > 0.f, "b200sd_attention: scale must be > 0 (got %g)", static_cast<double>(scale));
     B200SD_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0,
                    "b200sd_attention: leading dimensions must be multiples of 8");
     AttnParams p;
