@@ -190,7 +190,8 @@ int b200sd_softmax_rows(const float* in, void* out, int32_t rows, int32_t cols, 
  * softmax(q k^T / sqrt(d) [+ mask]) v per (batch, head): attention.py:24-168 (all three
  * AttentionImplementations compute this function) via Einsum (unet.py:45-59).
  * q [batch, sq, ldq] / k,v [batch, sk, ldk] fp16 token-major with head h in columns
- * [h*d, (h+1)*d) of the given base pointers; out [batch, sq, ldo].  d must be 64.
+ * [h*d, (h+1)*d) of the given base pointers; out [batch, sq, ldo].  d must be 40, 64, 80 or 160 (64: SD 2.x, SDXL
+ * and CLIP; 40 / 80 / 160: the 8-head blocks of SD 1.x); any other d is rejected with an error.
  * mask: optional fp32 additive [batch, sk] (unet.py:99-114) or NULL.
  * scale: multiplies q k^T before the softmax; must be > 0 (the kernel takes row maxima of the unscaled scores).
  * impl: 0 ORIGINAL, 1 SPLIT_EINSUM, 2 SPLIT_EINSUM_V2 (tile policy only; same result);
@@ -203,8 +204,12 @@ int b200sd_attention(const void* q, const void* k, const void* v, void* out, con
  * cut the (query tile x K/V tile) work into equal per-CTA ranges ("stream-K") when whole query tiles would fill the GPU
  * badly (S = 4096: 320 tiles on 132 CTA slots).  Pieces of a split tile meet in the workspace and are merged in a fixed
  * order, so results are reproducible.  The workspace must be zero-filled once before its first use (the kernel leaves its
- * counters at zero) and must not be shared with a concurrently running attention launch. */
+ * counters at zero) and must not be shared with a concurrently running attention launch.
+ * b200sd_attention_workspace_bytes_for(d) is the size that enables stream-K for head dim d (0 for an unsupported d);
+ * b200sd_attention_workspace_bytes() is the size for d = 64, which also covers d = 40.  A smaller workspace is not an
+ * error: that launch schedules whole query tiles. */
 size_t b200sd_attention_workspace_bytes(void);
+size_t b200sd_attention_workspace_bytes_for(int32_t d);
 int b200sd_attention_ws(const void* q, const void* k, const void* v, void* out, const float* mask,
                         int32_t batch, int32_t heads, int32_t sq, int32_t sk, int32_t d,
                         int32_t ldq, int32_t ldk, int32_t ldv, int32_t ldo, float scale, int32_t impl,

@@ -22,6 +22,11 @@ SD21_BASE_UNET = dict(
     flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=1,
 )
 
+# SD 1.4 / 1.5 (CompVis/stable-diffusion-v1-4, the reference's default model): SD-2.1-base with 8 heads in every block
+# (head dims 40 / 80 / 160) and the 768-wide CLIP ViT-L/14 text states; the reference constructor's defaults
+# (unet.py:826-828).  859,520,964 parameters.
+SD15_UNET = dict(SD21_BASE_UNET, attention_head_dim=8, cross_attention_dim=768)
+
 SDXL_BASE_UNET = dict(
     sample_size=128, in_channels=4, out_channels=4,
     down_block_types=("DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D"),
@@ -44,6 +49,10 @@ TINY_UNET = dict(
     flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=1,
 )
 
+# small SD-1-style config: 8 / 8 / 4 heads of 320 / 640 / 640 channels reach every SD-1.x head dim -- down blocks 40
+# and 80, mid block 160, up blocks 80 and 40 (143.7 M parameters)
+TINY_SD1_UNET = dict(TINY_UNET, block_out_channels=(320, 640, 640), attention_head_dim=(8, 8, 4))
+
 # tiny SDXL-style config: DownBlock2D first, text_time conditioning, deeper transformer stacks
 TINY_XL_UNET = dict(
     sample_size=16, in_channels=4, out_channels=4,
@@ -63,6 +72,16 @@ SD21_CONTROLNET = dict(
     flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=1,
     conditioning_embedding_out_channels=(16, 32, 96, 256),
 )
+
+# ControlNet for an SD-1.5 base model (lllyasviel/control_v11*_sd15): 8 heads, 768-wide text states
+SD15_CONTROLNET = dict(SD21_CONTROLNET, attention_head_dim=8, cross_attention_dim=768)
+
+# SD-1-shaped tiny ControlNet: the down and mid blocks of TINY_SD1_UNET (head dims 40, 80, 160)
+TINY_SD1_CONTROLNET = dict(in_channels=4, block_out_channels=(320, 640, 640), layers_per_block=1,
+                           down_block_types=("CrossAttnDownBlock2D", "CrossAttnDownBlock2D", "DownBlock2D"),
+                           attention_head_dim=(8, 8, 4), cross_attention_dim=96, norm_num_groups=32, norm_eps=1e-5,
+                           flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=1,
+                           conditioning_embedding_out_channels=(16, 32, 96, 256))
 
 TINY_CONTROLNET = dict(
     in_channels=4, block_out_channels=(64, 128, 128), layers_per_block=1,

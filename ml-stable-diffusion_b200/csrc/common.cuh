@@ -320,6 +320,44 @@ __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t (&a)
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc)
         : "memory");
 }
+// the same for B [16 x N], N = 64 / 128 / 192 (one, two or three 64-wide MN chunks, LBO apart)
+template <int N>
+__device__ __forceinline__ void wgmma_rs_tb(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc);
+template <>
+__device__ __forceinline__ void wgmma_rs_tb<64>(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    wgmma_m64n64_rs_tb(d, a, db, acc);
+}
+template <>
+__device__ __forceinline__ void wgmma_rs_tb<128>(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc)
+        : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_rs_tb<192>(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %101, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+        "{%96, %97, %98, %99}, %100, p, 1, 1, 1;\n\t}\n"
+        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
+          B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc)
+        : "memory");
+}
 #undef B200SD_F8
 
 // D[64 x bn] (+)= A[64 x 16] * B[bn x 16]^T as 64 / 32 / 16-column pieces for a RUNTIME width (bn: multiple of 16,

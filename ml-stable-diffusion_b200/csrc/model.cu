@@ -629,8 +629,9 @@ public:
     int attention(const __half* q, int ldq, const __half* k, const __half* v, int ldkv, int heads, int sq, int sk, __half** out, int c) {
         void* o;
         MODEL_TRY(act_alloc(&o, static_cast<size_t>(B) * sq * c * 2));
-        MODEL_TRY(b200sd_attention_ws(q, k, v, o, nullptr, B, heads, sq, sk, 64, ldq, ldkv, ldkv, c, 0.125f, attn_impl, attn_ws,
-                                      attn_ws_bytes, st));
+        const int d = c / heads;  // 64 (SD 2.x, SDXL) or 40 / 80 / 160 (SD 1.x)
+        MODEL_TRY(b200sd_attention_ws(q, k, v, o, nullptr, B, heads, sq, sk, d, ldq, ldkv, ldkv, c, 1.0f / sqrtf(static_cast<float>(d)),
+                                      attn_impl, attn_ws, attn_ws_bytes, st));
         *out = static_cast<__half*>(o);
         return 0;
     }
@@ -858,9 +859,14 @@ extern "C" int b200sd_unet_create(const b200sd_unet_config* cfg, const b200sd_we
     B200SD_REQUIRE(cfg && weights && out && n_weights > 0, "b200sd_unet_create: null argument");
     B200SD_REQUIRE(cfg->n_blocks >= 1 && cfg->n_blocks <= 8 && cfg->batch >= 1 && cfg->height >= 1 && cfg->width >= 1 && cfg->seq_len >= 1,
                    "b200sd_unet_create: bad geometry");
-    for (int i = 0; i < cfg->n_blocks; ++i)
-        B200SD_REQUIRE(cfg->block_out_channels[i] % cfg->attention_heads[i] == 0 && cfg->block_out_channels[i] / cfg->attention_heads[i] == 64,
-                       "b200sd_unet_create: the attention kernel needs head dim 64 (block %d)", i);
+    size_t attn_ws_bytes = 0;  // stream-K workspace for the largest head dim of the net
+    for (int i = 0; i < cfg->n_blocks; ++i) {
+        const int c = cfg->block_out_channels[i], heads = cfg->attention_heads[i];
+        B200SD_REQUIRE(heads > 0 && c % heads == 0 && b200sd_attention_workspace_bytes_for(c / heads) > 0,
+                       "b200sd_unet_create: block %d has head dim %d/%d; the attention kernel supports 40, 64, 80 and 160", i, c,
+                       heads);
+        attn_ws_bytes = std::max(attn_ws_bytes, b200sd_attention_workspace_bytes_for(c / heads));
+    }
     auto h = std::make_unique<b200sd_unet>();
     UNet& u = h->impl;
     u.cfg = *cfg;
@@ -893,7 +899,7 @@ extern "C" int b200sd_unet_create(const b200sd_unet_config* cfg, const b200sd_we
     if (int rc = u.dev_alloc(&tk, (1 << 16) * sizeof(unsigned int))) return rc;
     B200SD_CHECK_CUDA(cudaMemset(tk, 0, (1 << 16) * sizeof(unsigned int)));
     u.tickets = static_cast<unsigned int*>(tk);
-    u.attn_ws_bytes = b200sd_attention_workspace_bytes();
+    u.attn_ws_bytes = attn_ws_bytes;
     if (int rc = u.dev_alloc(&u.attn_ws, u.attn_ws_bytes)) return rc;
     B200SD_CHECK_CUDA(cudaMemset(u.attn_ws, 0, u.attn_ws_bytes));
     if (u.mats.count("kv")) {

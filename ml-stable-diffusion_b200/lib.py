@@ -88,6 +88,7 @@ _SIGNATURES = {
                                    C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_float, C.c_int32, C.c_void_p]),
     "b200sd_attention_workspace_bytes": (C.c_size_t, []),
+    "b200sd_attention_workspace_bytes_for": (C.c_size_t, [C.c_int32]),
     "b200sd_attention_ws": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -507,16 +508,19 @@ def layer_norm(x, gamma, beta, eps=1e-5, out=None):
     return out
 
 
+ATTENTION_HEAD_DIMS = (40, 64, 80, 160)  # head dims the attention kernel is built for (include/b200sd.h)
+
+
 def attention(q, k, v, batch, heads, sq, sk, d=64, mask=None, impl=0, out=None, scale=None, causal=False):
     """q: view [batch*sq, >=heads*d] (row stride = q.stride(0)), k/v: [batch*sk, ...]; out [batch*sq, heads*d].
-    causal: key j is visible to query i only if j <= i (CLIP text encoder)."""
+    d: head dim, one of ATTENTION_HEAD_DIMS.  causal: key j is visible to query i only if j <= i (CLIP text encoder)."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         if t.dtype != torch.float16 or not t.is_cuda or t.stride(-1) != 1:
             raise B200SDError(f"attention {nm}: expected CUDA fp16 with unit inner stride")
     if out is None:
         out = torch.empty(batch * sq, heads * d, dtype=torch.float16, device=q.device)
     scale = float(d) ** -0.5 if scale is None else float(scale)
-    ws = _attention_workspace(q.device)
+    ws = _attention_workspace(q.device, d)
     _check(load().b200sd_attention_ws(_ptr(q), _ptr(k), _ptr(v), _ptr(out), _ptr(mask), batch, heads, sq, sk, d,
                                       q.stride(0), k.stride(0), v.stride(0), out.stride(0), scale,
                                       int(impl) | (0x100 if causal else 0), _ptr(ws), ws.numel(),
@@ -525,17 +529,30 @@ def attention(q, k, v, batch, heads, sq, sk, d=64, mask=None, impl=0, out=None, 
 
 
 _attn_ws = {}
+_attn_ws_retired = []  # outgrown workspaces: graphs captured earlier still point at them
 
 
-def _attention_workspace(device):
+def _attention_workspace(device, d=64):
     """Zero-filled once per device: the stream-K pieces of split query tiles meet here; its counters return to zero at
-    the end of every launch.  Launches on one stream are ordered, which is the only way this package launches."""
+    the end of every launch.  Launches on one stream are ordered, which is the only way this package launches.
+    The partials grow with the head dim d: the buffer is replaced by a larger one the first time a d needs more, except
+    during a CUDA-graph capture, where the launch then schedules whole query tiles (engines reserve their largest d when
+    they are built, see reserve_attention_workspace)."""
     key = device.index if device.index is not None else torch.cuda.current_device()
     ws = _attn_ws.get(key)
-    if ws is None:
-        ws = torch.zeros(int(load().b200sd_attention_workspace_bytes()), dtype=torch.uint8, device=device)
+    need = int(load().b200sd_attention_workspace_bytes_for(int(d))) if d != 64 else None
+    if ws is None or (need is not None and ws.numel() < need and not torch.cuda.is_current_stream_capturing()):
+        size = max(int(load().b200sd_attention_workspace_bytes()), need or 0, 0 if ws is None else ws.numel())
+        if ws is not None:
+            _attn_ws_retired.append(ws)
+        ws = torch.zeros(size, dtype=torch.uint8, device=device)
         _attn_ws[key] = ws
     return ws
+
+
+def reserve_attention_workspace(device, d):
+    """Sizes the device's attention workspace for head dim d (outside any CUDA-graph capture)."""
+    return _attention_workspace(torch.device(device), d)
 
 
 def nchw_to_nhwc(x, c_pad=None, out=None):

@@ -115,10 +115,12 @@ class B200StableDiffusionPipeline:
                          text_encoder_cfg=None, tokenizer=None, with_vae_encoder=False):
         """Random-init weights of the named architecture (no checkpoints exist offline).  ``controlnet_cfgs``:
         list of ControlNet configs (seeded seed+2, seed+3, ...); switches the UNet to its control variant.
-        ``text_encoder_cfg``: a CLIP text config (config.OPENCLIP_H_TEXT for SD-2.x) -> the text encoder runs on the
+        ``model_version``: "sd21-base", "sd15" (SD 1.4 / 1.5), "sdxl-base" or "tiny".
+        ``text_encoder_cfg``: a CLIP text config (config.OPENCLIP_H_TEXT for SD-2.x, config.CLIP_L_TEXT for SD-1.x) -> the
+        text encoder runs on the
         device (random-init, seed+100) instead of the synthetic embedding table; ``tokenizer``: e.g. a
         ``tokenizer.BPETokenizer`` built from the checkpoint's vocab.json / merges.txt."""
-        unet_cfg = unet_cfg or {"sd21-base": C.SD21_BASE_UNET, "sdxl-base": C.SDXL_BASE_UNET,
+        unet_cfg = unet_cfg or {"sd21-base": C.SD21_BASE_UNET, "sd15": C.SD15_UNET, "sdxl-base": C.SDXL_BASE_UNET,
                                 "tiny": C.TINY_UNET}[model_version]
         vae_cfg = vae_cfg or (C.TINY_VAE if model_version == "tiny" else C.SD_VAE)
         if controlnet_cfgs:

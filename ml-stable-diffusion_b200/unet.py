@@ -117,8 +117,9 @@ class UNetEngine:
         # ResNet shortcuts (1x1 convolutions on the block input) run as extra k-blocks of conv2 instead of their own launch
         self.fold_shortcut = os.environ.get("B200SD_FOLD_SC", "1") != "0"
         for c, h in zip(boc, self.heads):
-            if c % h or c // h != 64:
-                raise L.B200SDError(f"b200sd attention kernel needs head dim 64 (got {c}/{h})")
+            if c % h or c // h not in L.ATTENTION_HEAD_DIMS:
+                raise L.B200SDError(f"b200sd attention kernel supports head dims {L.ATTENTION_HEAD_DIMS} (got {c}/{h})")
+        L.reserve_attention_workspace(self.dev, max(c // h for c, h in zip(boc, self.heads)))
         self._pack(state_dict)
 
     # ------------------------------------------------------------------ packing
@@ -270,12 +271,12 @@ class UNetEngine:
         for blk in t["blocks"]:
             n1 = L.layer_norm(tok, blk["ln1g"], blk["ln1b"])
             qkv = L.linear(n1, blk["qkv"], static_w=True)
-            a = L.attention(qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:], batch, heads, s, s, impl=impl)
+            a = L.attention(qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:], batch, heads, s, s, d=c // heads, impl=impl)
             tok = L.linear(a, blk["o1"], blk["o1b"], tok, static_w=True)
             n2 = L.layer_norm(tok, blk["ln2g"], blk["ln2b"])
             q = L.linear(n2, blk["q2"], static_w=True)
             ko = blk["kv_off"]
-            a = L.attention(q, kv_all[:, ko:ko + c], kv_all[:, ko + c:ko + 2 * c], batch, heads, s, s_ctx, impl=impl)
+            a = L.attention(q, kv_all[:, ko:ko + c], kv_all[:, ko + c:ko + 2 * c], batch, heads, s, s_ctx, d=c // heads, impl=impl)
             tok = L.linear(a, blk["o2"], blk["o2b"], tok, static_w=True)
             n3 = L.layer_norm(tok, blk["ln3g"], blk["ln3b"])
             g = L.linear(n3, blk["gg"], blk["ggb"], geglu=True, static_w=True)
@@ -353,12 +354,12 @@ class UNetEngine:
         nblk = len(t["blocks"])
         for bi, blk in enumerate(t["blocks"]):
             qkv = L.linear(tok, blk["qkv_ln"], blk["qkv_lnb"], ln=ln_of(rs, blk, "qkv"), static_w=True)
-            a = L.attention(qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:], batch, heads, s, s, impl=impl)
+            a = L.attention(qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:], batch, heads, s, s, d=c // heads, impl=impl)
             rs = {}
             tok = L.linear(a, blk["o1"], blk["o1b"], tok, static_w=True, rowstats=rs)
             q = L.linear(tok, blk["q2_ln"], blk["q2_lnb"], ln=ln_of(rs, blk, "q2"), static_w=True)
             ko = blk["kv_off"]
-            a = L.attention(q, kv_all[:, ko:ko + c], kv_all[:, ko + c:ko + 2 * c], batch, heads, s, s_ctx, impl=impl)
+            a = L.attention(q, kv_all[:, ko:ko + c], kv_all[:, ko + c:ko + 2 * c], batch, heads, s, s_ctx, d=c // heads, impl=impl)
             rs = {}
             tok = L.linear(a, blk["o2"], blk["o2b"], tok, static_w=True, rowstats=rs)
             g = L.linear(tok, blk["gg_ln"], blk["gg_lnb"], geglu=True, ln=ln_of(rs, blk, "gg"), static_w=True)
