@@ -242,7 +242,8 @@ int b200sd_embed_tokens(const float* ids, const void* token_embedding, const voi
  *     x_prev = cx * x + ce * eps' + sum_i ch[i] * hist[i]
  *     x0     = x0_cx * x + x0_ce * eps' + sum_i x0_ch[i] * hist[i]     (denoised estimate)
  * whose fp32 coefficients the host derives per step for DDIM (eta=0), DPM-Solver++(2M) and
- * PNDM/PLMS (Scheduler.swift:218-343, DPMSolverMultistepScheduler.swift:135-244).  `hist` is a
+ * PNDM/PLMS (Scheduler.swift:218-343, DPMSolverMultistepScheduler.swift:135-244), and for the Euler,
+ * Euler-ancestral and LMS samplers of diffusers 0.30.2 (there x is the model input x / sqrt(sigma^2 + 1)).  `hist` is a
  * 4-slot ring of latent-sized fp32 buffers holding past eps' (PLMS `ets`), past x0
  * (DPM `modelOutputs`) or a saved sample (PLMS `currentSample`); all history reads of a step happen
  * before its pushes.  noise_pred: fp32 NCHW [2*n, c, h, w] (uncond batch first); latents fp32
@@ -266,6 +267,19 @@ int b200sd_cfg_scheduler_step(const float* noise_pred, float* latents, float* hi
                               float* denoised /* x0 out or NULL */, void* unet_in, int32_t c_pad,
                               int32_t n, int32_t c, int32_t h, int32_t w,
                               const b200sd_step_coeffs* coeffs /* host */, void* stream);
+
+/* The same step plus ancestral noise (diffusers EulerAncestralDiscreteScheduler.step: prev_sample + noise * sigma_up):
+ *     x_prev += noise_scale * z[i]      before x_prev is written to `latents` and both halves of `unet_in`
+ * where z[i] is the standard normal of the Philox-4x32-10 stream that rng.NvRandomSource draws
+ * (NvRandomSource.swift): key = *philox_key, counter = (philox_offset, 0, i, 0), i the NCHW index over all n images,
+ * u = w0 / 2^32 + 2^-33, v = w1 * pi / 2^31 + pi / 2^32, z = sqrt(-2 ln u) sin v.  A step therefore draws what
+ * NvRandomSource(key)'s philox_offset-th normal_array(n*c*h*w) call returns.  The key is read from device memory
+ * (one uint32_t), so a captured CUDA graph serves every seed: fill the key before replay, offsets stay baked in. */
+int b200sd_cfg_scheduler_step_noised(const float* noise_pred, float* latents, float* hist /* [4][numel] */,
+                                     float* denoised /* x0 out or NULL */, void* unet_in, int32_t c_pad,
+                                     int32_t n, int32_t c, int32_t h, int32_t w,
+                                     const b200sd_step_coeffs* coeffs /* host */, float noise_scale,
+                                     const uint32_t* philox_key /* device */, uint32_t philox_offset, void* stream);
 
 /* VAE decoder input: out = post_quant_conv(z * inv_scale) as NHWC fp16 padded to c_pad channels
  * (pipeline.py:313-316 `z / 0.18215`; torch2coreml.py:590-594 post_quant_conv); z fp32 NCHW, c <= 8,

@@ -211,10 +211,36 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
 }
 
 // ---- fused CFG + scheduler step ------------------------------------------------------------------
-// One thread per latent element (n*c*h*w, NCHW fp32).  See include/b200sd.h for the algebra.
+// Standard normal number `idx` of noise draw `offset` under `key`: Philox-4x32-10 with counter (offset, 0, idx, 0), then
+// Box-Muller on the first two words -- the rng.NvRandomSource stream (NvRandomSource.swift), so
+// NvRandomSource(key) at that offset reproduces it on the host.  The transform runs in double, like the host twin.
+__device__ __forceinline__ float philox_normal(uint32_t key, uint32_t offset, uint32_t idx) {
+    uint32_t c0 = offset, c1 = 0u, c2 = idx, c3 = 0u, k0 = key, k1 = 0u;
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t hi0 = __umulhi(c0, 0xD2511F53u), lo0 = c0 * 0xD2511F53u;
+        const uint32_t hi1 = __umulhi(c2, 0xCD9E8D57u), lo1 = c2 * 0xCD9E8D57u;
+        c0 = hi1 ^ c1 ^ k0;
+        c1 = lo1;
+        c2 = hi0 ^ c3 ^ k1;
+        c3 = lo0;
+        k0 += 0x9E3779B9u;
+        k1 += 0xBB67AE85u;
+    }
+    const double u = static_cast<double>(c0) * (1.0 / 4294967296.0) + (1.0 / 8589934592.0);
+    // sin(v), v = c1 * pi / 2^31 + pi / 2^32, as sinpi of the exact v / pi (no large-argument reduction)
+    const double v_over_pi = static_cast<double>(c1) * (1.0 / 2147483648.0) + (1.0 / 4294967296.0);
+    return static_cast<float>(sqrt(-2.0 * log(u)) * sinpi(v_over_pi));
+}
+
+// One thread per latent element (n*c*h*w, NCHW fp32).  See include/b200sd.h for the algebra.  kNoise (ancestral
+// samplers): x_prev += noise_scale * z with z = philox_normal(*philox_key, philox_offset, i); the kNoise = false
+// instantiation never reads the three trailing parameters.
+template <bool kNoise>
 __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __restrict__ latents,
                                 float* __restrict__ hist, float* __restrict__ denoised, __half* __restrict__ unet_in,
-                                int c_pad, int n, int c, int hw, b200sd_step_coeffs k) {
+                                int c_pad, int n, int c, int hw, b200sd_step_coeffs k, float noise_scale,
+                                const uint32_t* __restrict__ philox_key, uint32_t philox_offset) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int numel = n * c * hw;
@@ -244,6 +270,7 @@ __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __r
     if (k.push_eps_slot >= 0) hist[static_cast<size_t>(k.push_eps_slot) * numel + i] = eps;
     if (k.push_x0_slot >= 0) hist[static_cast<size_t>(k.push_x0_slot) * numel + i] = x0;
     if (k.push_x_slot >= 0) hist[static_cast<size_t>(k.push_x_slot) * numel + i] = x;
+    if constexpr (kNoise) xp += noise_scale * philox_normal(*philox_key, philox_offset, static_cast<uint32_t>(i));
     if (denoised) denoised[i] = x0;
     latents[i] = xp;
     if (unet_in) {
@@ -452,9 +479,30 @@ extern "C" int b200sd_cfg_scheduler_step(const float* noise_pred, float* latents
                        (hist || (coeffs->push_eps_slot < 0 && coeffs->push_x0_slot < 0 && coeffs->push_x_slot < 0)),
                    "b200sd_cfg_scheduler_step: bad history ring slot");
     const int numel = n * c * h * w;
-    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred, latents, hist, denoised,
+    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<false>, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred, latents, hist, denoised,
                                                              reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
-                                                             *coeffs));
+                                                             *coeffs, 0.f, static_cast<const uint32_t*>(nullptr), 0u));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_cfg_scheduler_step_noised(const float* noise_pred, float* latents, float* hist, float* denoised,
+                                                void* unet_in, int32_t c_pad, int32_t n, int32_t c, int32_t h,
+                                                int32_t w, const b200sd_step_coeffs* coeffs, float noise_scale,
+                                                const uint32_t* philox_key, uint32_t philox_offset, void* stream_) {
+    if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(noise_pred && latents && coeffs && philox_key, "b200sd_cfg_scheduler_step_noised: null pointer");
+    B200SD_REQUIRE(coeffs->n_hist >= 0 && coeffs->n_hist <= 4 && (coeffs->n_hist == 0 || hist),
+                   "b200sd_cfg_scheduler_step_noised: bad history arguments");
+    B200SD_REQUIRE(coeffs->push_eps_slot < 4 && coeffs->push_x0_slot < 4 && coeffs->push_x_slot < 4 &&
+                       (hist || (coeffs->push_eps_slot < 0 && coeffs->push_x0_slot < 0 && coeffs->push_x_slot < 0)),
+                   "b200sd_cfg_scheduler_step_noised: bad history ring slot");
+    const int numel = n * c * h * w;
+    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<true>, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred,
+                                    latents, hist, denoised, reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
+                                    *coeffs, noise_scale, philox_key, philox_offset));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;

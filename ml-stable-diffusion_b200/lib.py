@@ -106,6 +106,10 @@ _SIGNATURES = {
     "b200sd_cfg_scheduler_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                             C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(StepCoeffs),
                                             C.c_void_p]),
+    "b200sd_cfg_scheduler_step_noised": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                   C.POINTER(StepCoeffs), C.c_float, C.c_void_p, C.c_uint32,
+                                                   C.c_void_p]),
     "b200sd_image_postprocess": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
 }
@@ -633,6 +637,23 @@ def cfg_scheduler_step(noise_pred, latents, coeffs: StepCoeffs, hist=None, denoi
     _check(load().b200sd_cfg_scheduler_step(_ptr(noise_pred), _ptr(latents), _ptr(hist), _ptr(denoised),
                                             _ptr(unet_in), c_pad, n, c, h, w, C.byref(coeffs), _stream()),
            "b200sd_cfg_scheduler_step")
+    return latents
+
+
+def cfg_scheduler_step_noised(noise_pred, latents, coeffs: StepCoeffs, noise_scale, key, offset, hist=None,
+                              denoised=None, unet_in=None):
+    """``cfg_scheduler_step`` plus ``noise_scale * z``, z the Philox normals of ``rng.NvRandomSource(key)``'s
+    ``offset``-th draw; ``key``: a one-element int32 / uint32 CUDA tensor holding the key's bits."""
+    _req(noise_pred, torch.float32, "cfg_scheduler_step_noised noise_pred")
+    _req(latents, torch.float32, "cfg_scheduler_step_noised latents")
+    if not (key.is_cuda and key.numel() == 1 and key.element_size() == 4):
+        raise B200SDError("cfg_scheduler_step_noised: key must be a one-element 4-byte CUDA tensor")
+    n, c, h, w = latents.shape
+    c_pad = 0 if unet_in is None else unet_in.shape[-1]
+    _check(load().b200sd_cfg_scheduler_step_noised(_ptr(noise_pred), _ptr(latents), _ptr(hist), _ptr(denoised),
+                                                   _ptr(unet_in), c_pad, n, c, h, w, C.byref(coeffs), float(noise_scale),
+                                                   _ptr(key), int(offset) & 0xFFFFFFFF, _stream()),
+           "b200sd_cfg_scheduler_step_noised")
     return latents
 
 

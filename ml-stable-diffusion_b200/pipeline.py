@@ -107,6 +107,10 @@ class B200StableDiffusionPipeline:
         self._denoised = torch.zeros(n, c, h, w, dtype=torch.float32, device=dev)
         self._ctx = torch.zeros(2 * n, d_ctx, 1, unet.seq, dtype=torch.float16, device=dev)
         self._t = torch.zeros(2 * n, dtype=torch.float32, device=dev)
+        # ancestral samplers: Philox key of the step noise (filled before each loop, so one loop graph serves every
+        # seed) and the draw number of step 0 (part of the graph key: offsets are baked into the graph)
+        self._noise_key = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._noise_base = 0
 
     # ---------------------------------------------------------------- factory
     @classmethod
@@ -215,6 +219,13 @@ class B200StableDiffusionPipeline:
         enc1, tok1 = text_pair("text_encoder", "tokenizer")
         enc2, tok2 = text_pair("text_encoder_2", "tokenizer_2")
         sched = scheduler_override
+        sched_kw = None
+        sched_cfg = os.path.join(model_dir, "scheduler", "scheduler_config.json")
+        if sched in S.SIGMA_SCHEDULERS and os.path.exists(sched_cfg):
+            # SCHEDULER_MAP[name].from_config(pytorch_pipe.scheduler.config) (pipeline.py:672-676): spacing, offset
+            # and betas come from the checkpoint (SDXL: "leading", offset 1)
+            with open(sched_cfg) as fh:
+                sched_kw = S.sigma_scheduler_kwargs(json.load(fh))
         if sched is None:
             with open(os.path.join(model_dir, "scheduler", "scheduler_config.json")) as fh:
                 name = json.load(fh).get("_class_name", "PNDMScheduler")
@@ -240,7 +251,7 @@ class B200StableDiffusionPipeline:
             force_zeros_for_empty_prompt = xl   # the reference's CLI sets it for SDXL only (pipeline.py:744-755)
         return cls(unet, vae, scheduler=sched, text_encoder=enc1, tokenizer=tok1, text_encoder_2=enc2, tokenizer_2=tok2,
                    xl=xl, controlnet=nets, vae_encoder=venc, force_zeros_for_empty_prompt=force_zeros_for_empty_prompt,
-                   unet_refiner=refiner)
+                   unet_refiner=refiner, scheduler_kwargs=sched_kw)
 
     # ---------------------------------------------------------------- reference-named helpers
     def check_inputs(self, prompt, height, width, callback_steps):
@@ -322,11 +333,14 @@ class B200StableDiffusionPipeline:
             emb, pooled = np.concatenate([emb, emb], 0), np.concatenate([pooled, pooled], 0)
         return np.ascontiguousarray(emb.transpose(0, 2, 1)[:, :, None, :]).astype(np.float16), pooled
 
-    def prepare_latents(self, batch, channels, height, width, latents=None, seed=None, rng="numpy"):
+    def prepare_latents(self, batch, channels, height, width, latents=None, seed=None, rng="numpy",
+                        init_noise_sigma=1.0):
         """pipeline.py:322-344: np.random.randn(...).astype(fp16) * init_noise_sigma (the global numpy stream, seeded by
         the caller like pipeline.py:725-726).  With ``seed``: the Swift pipeline's ``generateLatentSamples``
         (StableDiffusionPipeline.swift:361-379): one draw of C*h*w normals per image from the chosen
-        ``StableDiffusionRNG`` source (numpy / torch / nvidia, rng.py), so a seed reproduces the reference CLIs' latents."""
+        ``StableDiffusionRNG`` source (numpy / torch / nvidia, rng.py), so a seed reproduces the reference CLIs' latents.
+        ``init_noise_sigma``: the scheduler's (1 for DDIM / DPM-Solver++ / PNDM, sigma_max or sqrt(sigma_max^2 + 1) for
+        the Euler / LMS samplers)."""
         shape = (batch, channels, height // self.vae_scale_factor, width // self.vae_scale_factor)
         if latents is None and seed is not None:
             from .rng import random_source
@@ -337,7 +351,7 @@ class B200StableDiffusionPipeline:
             latents = np.random.randn(*shape).astype(np.float16)
         elif tuple(latents.shape) != shape:
             raise ValueError(f"Unexpected latents shape, got {latents.shape}, expected {shape}")
-        return latents.astype(np.float32) * 1.0
+        return latents.astype(np.float32) * init_noise_sigma
 
     def prepare_control_cond(self, controlnet_cond, do_classifier_free_guidance, batch_size, num_images_per_prompt):
         """pipeline.py:345-356: each (3, H, W) condition image is repeated per image and doubled for CFG."""
@@ -420,8 +434,17 @@ class B200StableDiffusionPipeline:
             k = self._coeffs(st, guidance_scale)
             k.noise_pred_nhwc = 1
             nxt = models[i + 1] if i + 1 < len(plan) else u
-            L.cfg_scheduler_step(u._out_nhwc, self._latents, k, hist=self._hist, denoised=self._denoised,
-                                 unet_in=nxt._x_nhwc)
+            self._step(st, k, u._out_nhwc, unet_in=nxt._x_nhwc)
+
+    def _step(self, st, k, noise_pred, unet_in=None):
+        """One fused guidance + scheduler update of the loop state, with the step's noise when the plan has some."""
+        if st.noise_offset >= 0:
+            L.cfg_scheduler_step_noised(noise_pred, self._latents, k, st.noise_scale, self._noise_key,
+                                        self._noise_base + st.noise_offset, hist=self._hist, denoised=self._denoised,
+                                        unet_in=unet_in)
+        else:
+            L.cfg_scheduler_step(noise_pred, self._latents, k, hist=self._hist, denoised=self._denoised,
+                                 unet_in=unet_in)
 
     def set_control_conditions(self, controlnet_cond):
         """Copy the conditioning images (each (2B, 3, H, W)) into the ControlNets' static input buffers."""
@@ -476,17 +499,32 @@ class B200StableDiffusionPipeline:
 
     def denoise(self, text_embeddings, latents, num_inference_steps, guidance_scale, callback=None,
                 callback_steps=1, time_ids=None, text_embeds=None, return_denoised=False, record=None,
-                controlnet_cond=None, start_step=0, refiner=None, refiner_start=0.8):
+                controlnet_cond=None, start_step=0, refiner=None, refiner_start=0.8, noise_key=None, noise_offset=0):
         """Runs the N-step loop (from ``start_step``: image-to-image) entirely on the device.  ``text_embeddings`` (2B, D, 1, S) and ``latents``
         (B, C, h, w) may be numpy (copied once, before the loop) or CUDA tensors.  ``record`` (a list) receives
         (timestep, noise_pred, latents_after_step) clones per step -- a debugging / testing aid.  Without
         callback / record / ControlNet the whole loop replays as ONE CUDA graph (SURVEY 8f N1): the scheduler
-        history lives on the device and no host synchronisation happens between the first and the last step."""
+        history lives on the device and no host synchronisation happens between the first and the last step.
+        Latents in and out (and those given to ``record`` / ``callback``) are x-space; the Euler / LMS samplers loop on
+        x / sqrt(sigma^2 + 1), so their latents are divided once before the loop and multiplied back off the hot path.
+        ``noise_key`` / ``noise_offset`` (ancestral samplers): step j adds the Philox normals of
+        ``NvRandomSource(noise_key)``'s draw number ``noise_offset + j``; without a key one ``np.random.randint(2**32)``
+        is drawn."""
         sched = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs)
         plan = list(sched.plan(start=start_step)) if start_step else list(sched.plan())
         n = self.images_per_call
         self._ctx.copy_(torch.as_tensor(text_embeddings), non_blocking=True)
         self._latents.copy_(torch.as_tensor(latents), non_blocking=True)
+        if sched.input_scale(0) != 1.0:
+            self._latents.div_(sched.input_scale(0))
+        if any(st.noise_offset >= 0 for st in plan):
+            key = int(np.random.randint(2 ** 32) if noise_key is None else noise_key) & 0xFFFFFFFF
+            self._noise_key.fill_(key - (1 << 32) if key >= 1 << 31 else key)  # the key's bits as int32
+        self._noise_base = int(noise_offset)
+
+        def x_space(i):  # latents after i steps, in x-space
+            s = sched.input_scale(i)
+            return self._latents if s == 1.0 else self._latents * s
         if controlnet_cond:
             controlnet_cond = [torch.as_tensor(c).to(self.device, torch.float16) for c in controlnet_cond]
         elif self.unet._res:
@@ -512,7 +550,7 @@ class B200StableDiffusionPipeline:
                 r._text_embeds.copy_(torch.as_tensor(refiner["text_embeds"]))
                 rstep = int(np.float32(len(plan)) * np.float32(refiner_start))  # Int(Float(timeSteps.count) * refinerStart)
             key = (self.scheduler_name, int(num_inference_steps), float(guidance_scale), int(start_step),
-                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep)
+                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base)
             self._loop_graph_for(key, plan, guidance_scale, bool(controlnet_cond), rstep).replay()
             return self._denoised if return_denoised else self._latents
         if refiner is not None:
@@ -529,11 +567,11 @@ class B200StableDiffusionPipeline:
             self._coeffs(st, guidance_scale, k)
             if record is not None:
                 eps_copy = noise_pred.clone()
-            L.cfg_scheduler_step(noise_pred, self._latents, k, hist=self._hist, denoised=self._denoised)
+            self._step(st, k, noise_pred)
             if record is not None:
-                record.append((st.timestep, eps_copy, self._latents.clone()))
+                record.append((st.timestep, eps_copy, x_space(i + 1).clone()))
             if callback is not None and i % callback_steps == 0:
-                callback(i, st.timestep, self._latents)
+                callback(i, st.timestep, x_space(i + 1))
         return self._denoised if return_denoised else self._latents
 
     def decode_latents(self, latents):
@@ -589,7 +627,17 @@ class B200StableDiffusionPipeline:
                 text_embeds = torch.as_tensor(xl_pooled, dtype=torch.float32, device=self.device)
             if text_embeds is None:
                 text_embeds = torch.zeros(2 * self.images_per_call, 1280, device=self.device)
-        lat = self.prepare_latents(len(prompts), self.unet.in_channels, height, width, latents, seed=seed, rng=rng)
+        if starting_image is not None and self.scheduler_name in S.SIGMA_SCHEDULERS:
+            raise ValueError(f"image-to-image is not implemented for the {self.scheduler_name} scheduler")
+        init_sigma = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs).init_noise_sigma
+        lat = self.prepare_latents(len(prompts), self.unet.in_channels, height, width, latents, seed=seed, rng=rng,
+                                   init_noise_sigma=init_sigma)
+        # ancestral step noise: keyed by the seed, continuing the latents' Philox stream with the nvidia source; without
+        # a seed, denoise() draws the key from the global numpy stream right after the latents
+        noise_key, noise_offset = None, 0
+        if seed is not None:
+            noise_key = seed
+            noise_offset = len(prompts) if rng in ("nvidia", "nvidiaRNG") else 0
         start_step = 0
         if starting_image is not None:
             if self.vae_encoder is None:
@@ -623,7 +671,8 @@ class B200StableDiffusionPipeline:
                        "time_ids": torch.tensor(rows, dtype=torch.float32)}
         final = self.denoise(text_embeddings, lat, num_inference_steps, guidance_scale, callback, callback_steps,
                              time_ids, text_embeds, controlnet_cond=controlnet_cond or None, start_step=start_step,
-                             refiner=refiner, refiner_start=refiner_start)
+                             refiner=refiner, refiner_start=refiner_start, noise_key=noise_key,
+                             noise_offset=noise_offset)
         image = self.decode_latents(final).cpu().numpy()  # single device->host copy of the result
         has_nsfw = None  # the safety checker is out of scope (SURVEY section 2, row 19)
         if output_type == "pil":

@@ -37,6 +37,10 @@ class StepPlan:
     push_eps_slot: int = -1
     push_x0_slot: int = -1
     push_x_slot: int = -1
+    # ancestral samplers: x_prev += noise_scale * z, z the Philox normals of the step's noise draw number
+    # `noise_offset` (b200sd_cfg_scheduler_step_noised); -1: no noise this step
+    noise_scale: float = 0.0
+    noise_offset: int = -1
 
 
 def alphas_cumprod(beta_start=0.00085, beta_end=0.012, n=1000, schedule="scaled_linear"):
@@ -48,6 +52,19 @@ def alphas_cumprod(beta_start=0.00085, beta_end=0.012, n=1000, schedule="scaled_
     else:
         raise ValueError(f"unknown beta schedule {schedule}")
     return np.cumprod((1.0 - betas).astype(np.float32), dtype=np.float32)
+
+
+def alphas_cumprod_diffusers(beta_start=0.00085, beta_end=0.012, n=1000, schedule="scaled_linear"):
+    """The fp32 table of diffusers 0.30.2 (torch.linspace + torch.cumprod), which differs from ``alphas_cumprod`` in
+    the last bits (sigma_max by 1.5e-6 relative): the Euler / LMS samplers restate diffusers, so they use this one."""
+    import torch
+    if schedule == "scaled_linear":
+        betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, n, dtype=torch.float32) ** 2
+    elif schedule == "linear":
+        betas = torch.linspace(beta_start, beta_end, n, dtype=torch.float32)
+    else:
+        raise ValueError(f"unknown beta schedule {schedule}")
+    return torch.cumprod(1.0 - betas, dim=0).numpy()
 
 
 class _Base:
@@ -64,6 +81,11 @@ class _Base:
 
     def scale_model_input(self, x, t):  # identity for DDIM / PNDM / DPM (pipeline.py:504)
         return x
+
+    def input_scale(self, i: int) -> float:
+        """x = input_scale(i) * (loop state) before step i; i == len(plan) is the end of the loop.  1 for the
+        schedulers whose loop state is the latent itself."""
+        return 1.0
 
     @property
     def timesteps(self):
@@ -246,11 +268,145 @@ class PNDMScheduler(_Base):
         return out
 
 
+class _SigmaScheduler(_Base):
+    """Shared part of diffusers 0.30.2 ``EulerDiscreteScheduler``, ``EulerAncestralDiscreteScheduler`` and
+    ``LMSDiscreteScheduler`` (the classes the reference imports, pipeline.py:11-18), epsilon prediction, linear
+    interpolation, no Karras sigmas.  Defaults are ``X.from_config(<SD 1.x / 2.1-base scheduler config>)``, what the
+    reference CLI runs for ``--scheduler X``: scaled_linear betas, steps_offset 1, ``timestep_spacing="linspace"``.
+
+    These samplers work on x = x0 + sigma * noise.  The device loop keeps y = x / s, s = sqrt(sigma^2 + 1), instead:
+    y is exactly what ``scale_model_input`` hands the UNet, and every update stays linear in (y, eps, history), so
+    the plan is the same StepPlan the other schedulers produce.  The final sigma is 0, so the last y is x."""
+    SPACINGS = ("linspace", "leading", "trailing")
+
+    def __init__(self, num_inference_steps, timestep_spacing="linspace", steps_offset=1, num_train_timesteps=1000,
+                 beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear"):
+        super().__init__(num_inference_steps, num_train_timesteps, beta_start, beta_end, beta_schedule)
+        if timestep_spacing not in self.SPACINGS:
+            raise ValueError(f"timestep_spacing must be one of {self.SPACINGS}, got {timestep_spacing!r}")
+        self.timestep_spacing, self.steps_offset = timestep_spacing, int(steps_offset)
+        n, nt = self.n, self.n_train
+        if timestep_spacing == "linspace":
+            ts = np.linspace(0, nt - 1, n, dtype=np.float32)[::-1].copy()
+        elif timestep_spacing == "leading":
+            ts = (np.arange(0, n) * (nt // n)).round()[::-1].copy().astype(np.float32)
+            ts += self.steps_offset
+        else:
+            ts = np.arange(nt, 0, -nt / n).round().copy().astype(np.float32)
+            ts -= 1
+        abar = alphas_cumprod_diffusers(beta_start, beta_end, num_train_timesteps, beta_schedule)
+        table = ((1 - abar) / abar) ** 0.5
+        #: the (possibly fractional) timesteps at which sigma is interpolated
+        self.sigma_timesteps = [float(t) for t in ts]
+        #: fp32 sigmas of the steps, then the final 0
+        self.sigmas = np.concatenate([np.interp(ts, np.arange(0, len(table)), table), [0.0]]).astype(np.float32)
+        smax = self.sigmas.max()
+        self.init_noise_sigma = float(smax if timestep_spacing != "leading" else (smax * smax + np.float32(1)) ** 0.5)
+
+    def input_scale(self, i):
+        return math.sqrt(float(self.sigmas[i]) ** 2 + 1.0)
+
+    def plan(self, start=0):
+        if start:
+            raise ValueError(f"{type(self).__name__} has no image-to-image schedule")
+        out = []
+        for i, t in enumerate(self.sigma_timesteps):
+            sig, sig_next = float(self.sigmas[i]), float(self.sigmas[i + 1])
+            s, s_next = self.input_scale(i), self.input_scale(i + 1)
+            # the reference feeds the UNet np.array([t, t], np.float16) (pipeline.py:511-514)
+            st = StepPlan(float(np.float16(t)), s / s_next, 0.0, [0.0] * 4, s, -sig, [0.0] * 4)
+            self._update(st, i, sig, sig_next, s_next)
+            out.append(st)
+        return out
+
+    def _update(self, st, i, sig, sig_next, s_next):
+        """Fill ce / ch / history / noise of step i (cx = s / s', x0 = s y - sigma eps are common)."""
+        raise NotImplementedError
+
+
+class EulerDiscreteScheduler(_SigmaScheduler):
+    """x' = x + (sigma' - sigma) eps (s_churn = 0: no noise)."""
+
+    def _update(self, st, i, sig, sig_next, s_next):
+        st.ce = (sig_next - sig) / s_next
+
+
+class EulerAncestralDiscreteScheduler(_SigmaScheduler):
+    """The Euler step to sigma_down, then + sigma_up z.  Step i draws its z as noise draw number i."""
+
+    @staticmethod
+    def sigma_up_down(sig, sig_next):
+        up = math.sqrt(sig_next ** 2 * (sig ** 2 - sig_next ** 2) / sig ** 2)
+        return up, math.sqrt(sig_next ** 2 - up ** 2)
+
+    def _update(self, st, i, sig, sig_next, s_next):
+        up, down = self.sigma_up_down(sig, sig_next)
+        st.ce = (down - sig) / s_next
+        if up > 0.0:
+            st.noise_scale, st.noise_offset = up / s_next, i
+
+
+class LMSDiscreteScheduler(_SigmaScheduler):
+    """Linear multistep of order min(step + 1, 4): x' = x + sum_k c_k eps_{i-k}, c_k the integral from sigma_i to
+    sigma_{i+1} of the k-th Lagrange basis polynomial over the nodes sigma_i .. sigma_{i-order+1}.  diffusers integrates
+    with ``scipy.integrate.quad``; these cubics are integrated exactly here.  History ring: eps of step i in slot i % 3
+    (the three previous eps are all an order-4 step reads)."""
+    order = 4
+
+    def lms_coefficients(self, i):
+        order = min(i + 1, self.order)
+        nodes = [float(self.sigmas[i - m]) for m in range(order)]
+        a, b = float(self.sigmas[i]), float(self.sigmas[i + 1])
+        P = np.polynomial.polynomial
+        out = []
+        for k in range(order):
+            poly = np.array([1.0])
+            for m in range(order):
+                if m != k:
+                    poly = P.polymul(poly, np.array([-nodes[m], 1.0]) / (nodes[k] - nodes[m]))
+            prim = P.polyint(poly)
+            out.append(float(P.polyval(b, prim) - P.polyval(a, prim)))
+        return out
+
+    def _update(self, st, i, sig, sig_next, s_next):
+        c = self.lms_coefficients(i)
+        st.ce = c[0] / s_next
+        for k in range(1, len(c)):
+            st.ch[(i - k) % 3] = c[k] / s_next
+        st.n_hist = 3 if len(c) > 1 else 0
+        st.push_eps_slot = i % 3
+
+
 SCHEDULER_MAP = {
     "DDIM": DDIMScheduler,
     "DPMSolverMultistep": DPMSolverMultistepScheduler,
     "PNDM": PNDMScheduler,
+    "EulerDiscrete": EulerDiscreteScheduler,
+    "EulerAncestralDiscrete": EulerAncestralDiscreteScheduler,
+    "LMSDiscrete": LMSDiscreteScheduler,
 }
+
+#: the scheduler classes whose loop state is y = x / sqrt(sigma^2 + 1)
+SIGMA_SCHEDULERS = ("EulerDiscrete", "EulerAncestralDiscrete", "LMSDiscrete")
+
+
+def sigma_scheduler_kwargs(config: dict) -> dict:
+    """Constructor arguments of the Euler / Euler-ancestral / LMS samplers from a checkpoint's
+    ``scheduler_config.json`` (the reference's ``SCHEDULER_MAP[name].from_config(pytorch_pipe.scheduler.config)``,
+    pipeline.py:594-604, 672-676).  Settings these samplers do not implement raise a ValueError that names the key."""
+    unsupported = {
+        "prediction_type": lambda v: v not in (None, "epsilon"),
+        "use_karras_sigmas": bool,
+        "interpolation_type": lambda v: v not in (None, "linear"),
+        "timestep_type": lambda v: v == "continuous",
+        "rescale_betas_zero_snr": bool,
+        "trained_betas": lambda v: v is not None,
+    }
+    for key, bad in unsupported.items():
+        if key in config and bad(config[key]):
+            raise ValueError(f"scheduler config {key}={config[key]!r} is not supported by the Euler / LMS samplers")
+    used = ("timestep_spacing", "steps_offset", "beta_start", "beta_end", "beta_schedule", "num_train_timesteps")
+    return {key: config[key] for key in used if key in config}
 
 
 def make_scheduler(name, num_inference_steps, **kw):
@@ -259,14 +415,19 @@ def make_scheduler(name, num_inference_steps, **kw):
     return SCHEDULER_MAP[name](num_inference_steps, **kw)
 
 
-def apply_plan_host(step: StepPlan, guidance, eps_uncond, eps_text, x, hist):
-    """numpy mirror of the device kernel's arithmetic (host-logic tests only)."""
+def apply_plan_host(step: StepPlan, guidance, eps_uncond, eps_text, x, hist, noise=None):
+    """numpy mirror of the device kernel's arithmetic (host-logic tests only).  ``noise``: the step's normals z
+    (needed when ``step.noise_offset >= 0``)."""
     eps = eps_uncond + guidance * (eps_text - eps_uncond)
     xp = step.cx * x + step.ce * eps
     x0 = step.x0_cx * x + step.x0_ce * eps
     for j in range(step.n_hist):
         xp = xp + step.ch[j] * hist[j]
         x0 = x0 + step.x0_ch[j] * hist[j]
+    if step.noise_offset >= 0:
+        if noise is None:
+            raise ValueError("this step adds noise: pass its normals")
+        xp = xp + step.noise_scale * noise
     if step.push_eps_slot >= 0:
         hist[step.push_eps_slot] = eps
     if step.push_x0_slot >= 0:
