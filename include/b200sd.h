@@ -140,9 +140,13 @@ int b200sd_gemm(const b200sd_gemm_args* args, void* stream);
  * kb_total, n_tiles */
 int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4);
 /* host-only: out[0..7] = block_n, splits, kb_total, n_tiles, statistics slots per image (0: this plan cannot emit
- * column statistics), staged epilogue (0/1), pipeline stages, m_tiles */
+ * column statistics), staged epilogue (0/1), pipeline stages, m_tiles.  With halo != 0 it plans for the chunk-major
+ * tiled weights of width block_n (block_n 0: the width the halo kernel prefers), whatever wgt_tiled says */
 int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8);
-/* host-only: human-readable tiling plan (tile shape, split-K, pipeline depth) the launcher would use */
+/* host-only: human-readable tiling plan the launcher would use, "key=value" fields separated by spaces (tile shape,
+ * split-K, pipeline depth, ..., variant = epilogue instantiation of the GEMM kernel: 0 generic, 1 split-K partial,
+ * 2 GEGLU, 3 fp32 output, 4 plain, 5 staged, -1 halo convolution; halo_kind 0 / 1 / 2 and halo_wide for the halo
+ * kernel's instantiation).  Halo calls are planned like b200sd_gemm_plan_ex */
 int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size);
 /* bytes of fp32 scratch b200sd_gemm would need for these args (0 if no split-K) */
 size_t b200sd_gemm_workspace_bytes(const b200sd_gemm_args* args);

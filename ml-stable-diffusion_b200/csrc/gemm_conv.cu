@@ -1425,6 +1425,14 @@ struct GemmPlan {
     int tma_patch;
     int cs_slots;  // statistics slots per image this tiling produces (0: column statistics not available)
     int smem_bytes;
+    int variant;    // GEMM kernel: one of GemmVariant (-1 for the halo convolution)
+    int halo_kind;  // halo convolution: 0 loader warps + staged epilogue, 1 fp32 / narrow epilogue, 2 TMA patches (-1: GEMM)
+};
+
+// Epilogue instantiations of wgmma_gemm_kernel, each compiled for every width of kGemmWidths (plan_gemm sends width 16
+// to the generic one: the others need block_n % 32 == 0)
+enum GemmVariant {
+    kVariantGeneric = 0, kVariantSplitK = 1, kVariantGeglu = 2, kVariantF32 = 3, kVariantPlain = 4, kVariantStaged = 5
 };
 
 static bool cluster_splitk_enabled() {
@@ -1523,6 +1531,8 @@ static int plan_halo(const b200sd_gemm_args& a, GemmPlan& pl) {
                    "b200sd_gemm: halo epilogue tile does not fit over the pipeline memory (block_n=%d)", pl.block_n);
     pl.epi_smem = 0;
     pl.cs_slots = pl.tiles_per_img;
+    pl.variant = -1;
+    pl.halo_kind = pl.tma_patch ? 2 : (pl.staged == 0 ? 1 : 0);
     return 0;
 }
 
@@ -1680,8 +1690,10 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
         }
         if (a.residual != nullptr && !a.geglu && a.n % 8 == 0) pl.res_smem = 1;
     }
-    const bool regular = (a.act == 0) && (a.n % 16 == 0) && ((a.geglu ? a.n / 2 : a.n) % 8 == 0) && (pl.block_n % 32 == 0) &&
-                         pl.bias_mode != 2 && (a.residual == nullptr || pl.res_smem);
+    // the compile-time epilogue variants (everything but kVariantGeneric) need these shapes and operands
+    const bool regular_shape = (a.act == 0) && (a.n % 16 == 0) && ((a.geglu ? a.n / 2 : a.n) % 8 == 0) &&
+                               (pl.block_n % 32 == 0) && pl.bias_mode != 2;
+    const bool regular = regular_shape && (a.residual == nullptr || pl.res_smem);
     const int per_stage = kAStage + pl.block_n * kBK * 2;
     {
         // staged epilogue: fp16 tile in shared memory, row-contiguous residual reads / stores, statistics outputs
@@ -1718,6 +1730,16 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
     while (pl.stages * per_stage < park && pl.stages < kMaxStages) ++pl.stages;
     B200SD_REQUIRE(pl.stages * per_stage >= park, "b200sd_gemm: epilogue tile does not fit over the stages (block_n=%d)", pl.block_n);
     pl.smem_bytes = pl.stages * per_stage + (2 * kMaxStages + 4) * 8 + 16 + pl.epi_smem + 1024;
+    // compile-time epilogue variants for the hot shapes; anything irregular takes the generic kernel (split-K and the
+    // staged epilogue read the residual row-contiguously, so they need no residual tile in shared memory)
+    const bool regular_epi = regular || (regular_shape && a.residual != nullptr && (pl.splits > 1 || pl.staged));
+    if (!regular_epi) pl.variant = kVariantGeneric;
+    else if (pl.staged) pl.variant = kVariantStaged;
+    else if (pl.splits > 1) pl.variant = kVariantSplitK;
+    else if (a.geglu) pl.variant = kVariantGeglu;
+    else if (a.out_f32) pl.variant = kVariantF32;
+    else pl.variant = kVariantPlain;
+    pl.halo_kind = -1;
     return 0;
 }
 
@@ -1877,7 +1899,7 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
     }
     if (pl.halo) {
         using HaloFn = void (*)(GemmParams);
-        const int kind = pl.tma_patch ? 2 : (pl.staged == 0 ? 1 : 0);
+        const int kind = pl.halo_kind;
         const bool wide = pl.block_n > 128;  // (only the TMA-patch kind takes tiles wider than 128 columns)
         HaloFn hfn = kind == 2 ? (wide ? halo_conv_kernel<2, 128> : halo_conv_kernel<2, 64>)
                                : (kind == 1 ? halo_conv_kernel<1, 8> : halo_conv_kernel<0, 64>);
@@ -1897,25 +1919,17 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
     const int smem_bytes = pl.smem_bytes;
     const int total = pl.m_tiles * pl.n_tiles * pl.splits;
     const int grid = std::min(total, num_sms());
-    // compile-time epilogue variants for the hot shapes; anything irregular takes the generic kernel
     B200SD_REQUIRE(a.act == 0 || (a.act >= 1 && a.act <= 3 && pl.splits == 1 && !a.geglu), "b200sd_gemm: act=%d unsupported here", a.act);
-    const bool regular = (a.act == 0) && (a.n % 16 == 0) && (p.n_store % 8 == 0) && (pl.block_n % 32 == 0) && pl.bias_mode != 2 &&
-                         (a.residual == nullptr || pl.res_smem || pl.splits > 1 || pl.staged);
     const int wi = gemm_width_index(pl.block_n);
+    const int variant = pl.variant;
     KernelFn fn;
-    int variant;
-    if (!regular) {
-        fn = gemm_kernel<true, false, false, false, false>(wi), variant = 0;
-    } else if (pl.staged) {
-        fn = gemm_kernel<false, false, false, false, true>(wi), variant = 5;
-    } else if (pl.splits > 1) {
-        fn = gemm_kernel<false, false, false, true, false>(wi), variant = 1;
-    } else if (a.geglu) {
-        fn = gemm_kernel<false, true, false, false, false>(wi), variant = 2;
-    } else if (a.out_f32) {
-        fn = gemm_kernel<false, false, true, false, false>(wi), variant = 3;
-    } else {
-        fn = gemm_kernel<false, false, false, false, false>(wi), variant = 4;
+    switch (variant) {
+        case kVariantGeneric: fn = gemm_kernel<true, false, false, false, false>(wi); break;
+        case kVariantStaged: fn = gemm_kernel<false, false, false, false, true>(wi); break;
+        case kVariantSplitK: fn = gemm_kernel<false, false, false, true, false>(wi); break;
+        case kVariantGeglu: fn = gemm_kernel<false, true, false, false, false>(wi); break;
+        case kVariantF32: fn = gemm_kernel<false, false, true, false, false>(wi); break;
+        default: fn = gemm_kernel<false, false, false, false, false>(wi); break;
     }
     if (pl.splits > 1 && !pl.cluster) {
         // the separate reduce kernel applies bias / residual; the partial writer must not
@@ -1987,15 +2001,21 @@ extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {
     return 0;
 }
 
+// Planning query before the weights are tiled: a halo call plans for chunk-major tiled weights of the requested (or the
+// preferred) width.
+static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl) {
+    b200sd_gemm_args a = *args;
+    if (a.halo) {
+        if (a.block_n == 0) a.block_n = b200sd::halo_pick_block_n(a);
+        a.wgt_tiled = 1;
+    }
+    return b200sd::plan_gemm(a, pl);
+}
+
 extern "C" int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8) {
     if (!args || !out8) return 2;
     b200sd::GemmPlan pl;
-    b200sd_gemm_args a = *args;
-    if (a.halo && a.block_n == 0) {  // planning query before the weights are tiled
-        a.block_n = b200sd::halo_pick_block_n(a);
-        a.wgt_tiled = 1;
-    }
-    if (int rc = b200sd::plan_gemm(a, pl)) return rc;
+    if (int rc = plan_query(args, pl)) return rc;
     out8[0] = pl.block_n, out8[1] = pl.splits, out8[2] = pl.kb_total, out8[3] = pl.n_tiles;
     out8[4] = pl.cs_slots, out8[5] = pl.staged, out8[6] = pl.stages, out8[7] = pl.m_tiles;
     return 0;
@@ -2004,12 +2024,15 @@ extern "C" int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8) 
 extern "C" int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
     if (!args || !buf || buf_size == 0) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = b200sd::plan_gemm(*args, pl)) return rc;
+    if (int rc = plan_query(args, pl)) return rc;
+    // variant: GemmVariant of the GEMM kernel (-1: halo convolution); halo_kind / halo_wide: which halo_conv_kernel
+    // instantiation runs (-1 / 0 for the GEMM kernel); win: the halo walk over th x tw windows instead of image rows
     snprintf(buf, buf_size,
              "M=%d N=%d kb_total=%d m_tiles=%d n_tiles=%d block_n=%d splits=%d kb_per_split=%d stages=%d "
-             "box=%dx%dx%d bias_mode=%d res_smem=%d epi_smem=%d cluster=%d",
+             "box=%dx%dx%d bias_mode=%d res_smem=%d epi_smem=%d cluster=%d staged=%d variant=%d halo_kind=%d halo_wide=%d win=%d",
              pl.M, pl.N, pl.kb_total, pl.m_tiles, pl.n_tiles, pl.block_n, pl.splits, pl.kb_per_split, pl.stages,
-             pl.bn_img, pl.bh, pl.bw, pl.bias_mode, pl.res_smem, pl.epi_smem, pl.cluster);
+             pl.bn_img, pl.bh, pl.bw, pl.bias_mode, pl.res_smem, pl.epi_smem, pl.cluster, pl.staged, pl.variant, pl.halo_kind,
+             pl.halo && pl.block_n > 128 ? 1 : 0, pl.halo ? pl.win : 0);
     return 0;
 }
 

@@ -204,13 +204,29 @@ def gemm_args(mode, a0, wgt, out, *, a1=None, bias=None, residual=None, m=0, n=0
 
 
 def describe_plan(mode, m=0, n=0, c0=0, c1=0, n_img=0, h=0, w=0, stride=1, geglu=False, has_bias=True,
-                  has_residual=False, bias_rows=0, split_k=0, block_n=0) -> str:
-    """Host-only: the tiling the launcher would choose (no GPU needed)."""
+                  has_residual=False, bias_rows=0, split_k=0, block_n=0, out_f32=False, act=0, pad_after_only=False,
+                  rowstats=False, stats=False, cs_hw=0, ln=False, c2=0, c3=0, halo=0, upsample=False, gn=False) -> str:
+    """Host-only: the tiling the launcher would choose (no GPU needed).  The flags mirror linear() / conv3x3():
+    rowstats / stats (with cs_hw, the rows per image of a linear) ask for the statistics outputs, ln for the LayerNorm
+    fold, c2 / c3 are the folded shortcut's channels, halo / upsample / gn select the halo convolution (mode 0 with halo:
+    its 1x1 form; m = n_img * h * w)."""
     a = GemmArgs()
     a.mode, a.m, a.n, a.c0, a.c1, a.n_img, a.h, a.w, a.stride = mode, m, n, c0, c1, n_img, h, w, stride
     a.geglu, a.bias_rows, a.split_k, a.block_n = int(geglu), bias_rows, split_k, block_n
-    a.bias = 1 if has_bias else None       # only tested for null-ness by the planner
+    a.out_f32, a.act, a.pad_after_only = int(out_f32), act, int(pad_after_only)
+    # pointers are only tested for null-ness by the planner
+    a.bias = 1 if has_bias else None
     a.residual = 1 if has_residual else None
+    if stats:
+        a.cs_partial, a.cs_hw = 1, cs_hw
+    if rowstats:
+        a.rs_out = 1
+    if ln:
+        a.ln_stat, a.ln_wg, a.ln_parts = 1, 1, 1
+    a.c2, a.c3 = c2, c3
+    a.halo, a.upsample2x, a.gn_groups = int(halo), int(upsample), 32 if gn else 0
+    if stats or rowstats or ln or gn:
+        a.split_k = 1  # as linear() / conv3x3() ask for the fused outputs
     buf = C.create_string_buffer(512)
     _check(load().b200sd_gemm_describe_plan(C.byref(a), buf, 512), "b200sd_gemm_describe_plan")
     return buf.value.decode()
