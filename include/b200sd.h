@@ -12,6 +12,8 @@
  *   - plain pointers + sizes, no torch types; all pointers are DEVICE pointers unless noted;
  *   - activations are fp16, channels-last: images NHWC, token matrices [rows, channels];
  *   - weights fp16, bias / statistics / scheduler scalars fp32;
+ *   - an entry point with a `_bf16` twin has the same signature there, and every pointer it documents as fp16 is
+ *     bf16 instead (VAEs whose activations exceed fp16's range, e.g. the stock SDXL VAE);
  *   - every function returns 0 on success, non-zero on failure with the message available
  *     from b200sd_last_error(); nothing falls back to a CPU path;
  *   - `stream` is a cudaStream_t passed as void*.
@@ -136,6 +138,10 @@ typedef struct {
 } b200sd_gemm_args;
 
 int b200sd_gemm(const b200sd_gemm_args* args, void* stream);
+/* bf16 twin: a0 / a1 / wgt / residual and a 16-bit out are bf16.  Supports modes 0 / 1, stride 1 / 2, pad_after_only,
+ * bias, residual, out_f32 and wgt_tiled; rejects geglu, split_k > 1, halo / upsample2x, gn_*, cs_* / rs_out, ln_*,
+ * a2 / a3 and act with an error naming the field.  It never splits K and needs no workspace. */
+int b200sd_gemm_bf16(const b200sd_gemm_args* args, void* stream);
 /* host-only: block_n / split count / k-block count the launcher would choose: out[0..3] = block_n, splits,
  * kb_total, n_tiles */
 int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4);
@@ -143,11 +149,13 @@ int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4);
  * column statistics), staged epilogue (0/1), pipeline stages, m_tiles.  With halo != 0 it plans for the chunk-major
  * tiled weights of width block_n (block_n 0: the width the halo kernel prefers), whatever wgt_tiled says */
 int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8);
+int b200sd_gemm_plan_ex_bf16(const b200sd_gemm_args* args, int32_t* out8);
 /* host-only: human-readable tiling plan the launcher would use, "key=value" fields separated by spaces (tile shape,
  * split-K, pipeline depth, ..., variant = epilogue instantiation of the GEMM kernel: 0 generic, 1 split-K partial,
  * 2 GEGLU, 3 fp32 output, 4 plain, 5 staged, -1 halo convolution; halo_kind 0 / 1 / 2 and halo_wide for the halo
  * kernel's instantiation).  Halo calls are planned like b200sd_gemm_plan_ex */
 int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size);
+int b200sd_gemm_describe_plan_bf16(const b200sd_gemm_args* args, char* buf, size_t buf_size);
 /* bytes of fp32 scratch b200sd_gemm would need for these args (0 if no split-K) */
 size_t b200sd_gemm_workspace_bytes(const b200sd_gemm_args* args);
 
@@ -172,6 +180,9 @@ int b200sd_timestep_embedding(const float* timesteps, float* out, int32_t m, int
 int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
                       int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
                       void* out, float* stats_ws, size_t stats_ws_bytes, void* stream);
+int b200sd_group_norm_bf16(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
+                           int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
+                           void* out, float* stats_ws, size_t stats_ws_bytes, void* stream);
 size_t b200sd_group_norm_workspace_bytes(int32_t n_img, int32_t hw, int32_t c, int32_t groups);
 /* GroupNorm (+SiLU, + concat) from PRODUCER-SIDE statistics: chan0 / chan1 are the per-channel (sum, sum of squares)
  * [n_img][c][2] a b200sd_gemm call left behind (cs_chan); no statistics pass, one read + one write of the tensor.  Used
@@ -189,6 +200,7 @@ int b200sd_layer_norm(const void* x, const float* gamma, const float* beta, void
  * decoder's single-head d=512 mid-block attention (diffusers AutoencoderKL via torch2coreml.py:584-594),
  * whose Q K^T and P V products run on b200sd_gemm. */
 int b200sd_softmax_rows(const float* in, void* out, int32_t rows, int32_t cols, float scale, void* stream);
+int b200sd_softmax_rows_bf16(const float* in, void* out, int32_t rows, int32_t cols, float scale, void* stream);
 
 /* ---- attention ------------------------------------------------------------------------------
  * softmax(q k^T / sqrt(d) [+ mask]) v per (batch, head): attention.py:24-168 (all three
@@ -223,10 +235,12 @@ int b200sd_attention_ws(const void* q, const void* k, const void* v, void* out, 
 /* NCHW (fp16 or fp32) -> NHWC fp16 with channel padding to c_pad (zeros) */
 int b200sd_nchw_to_nhwc(const void* in, int32_t in_f32, void* out, int32_t n, int32_t c, int32_t h,
                         int32_t w, int32_t c_pad, void* stream);
+int b200sd_nchw_to_nhwc_bf16(const void* in, int32_t in_f32, void* out, int32_t n, int32_t c, int32_t h,
+                             int32_t w, int32_t c_pad, void* stream);
 /* NHWC fp32/fp16 [n,h,w,c_pad] -> NCHW fp32 [n,c,h,w] (first c channels) */
 int b200sd_nhwc_to_nchw_f32(const void* in, int32_t in_f32, float* out, int32_t n, int32_t c, int32_t h,
                             int32_t w, int32_t c_pad, void* stream);
-/* nearest x2 upsample NHWC fp16 (F.interpolate, unet.py:499) */
+/* nearest x2 upsample NHWC fp16 (F.interpolate, unet.py:499); a byte copy, so bf16 tensors use it as well */
 int b200sd_upsample2x(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c, void* stream);
 /* out = a + b (fp16; ControlNet residual injection unet.py:1009-1022) */
 int b200sd_add(const void* a, const void* b, void* out, size_t numel, void* stream);
@@ -290,6 +304,8 @@ int b200sd_cfg_scheduler_step_noised(const float* noise_pred, float* latents, fl
  * w fp32 [c, c], b fp32 [c]. */
 int b200sd_latent_prep(const float* z, const float* w, const float* b, float inv_scale, void* out, int32_t n,
                        int32_t c, int32_t h, int32_t wd, int32_t c_pad, void* stream);
+int b200sd_latent_prep_bf16(const float* z, const float* w, const float* b, float inv_scale, void* out, int32_t n,
+                            int32_t c, int32_t h, int32_t wd, int32_t c_pad, void* stream);
 
 /* VAE post-process: clip(x/2+0.5,0,1) (pipeline.py:317) NHWC fp16/32 -> NHWC fp32 [n,h,w,3] and/or u8 */
 int b200sd_image_postprocess(const void* in, int32_t in_f32, int32_t c_pad, float* out_f32, uint8_t* out_u8,

@@ -94,6 +94,10 @@ TINY_CONTROLNET = dict(
 SD_VAE = dict(latent_channels=4, out_channels=3, block_out_channels=(128, 256, 512, 512),
               layers_per_block=2, norm_num_groups=32, scaling_factor=0.18215)
 
+# The stock SDXL VAE (SDXL-base 1.0 and the refiner): SD's architecture with other weights; its decoder activations
+# exceed fp16's range, so its config sets force_upcast and the pipeline runs it in bf16 (pipeline.vae_dtype).
+SDXL_VAE = dict(SD_VAE, scaling_factor=0.13025, force_upcast=True)
+
 TINY_VAE = dict(latent_channels=4, out_channels=3, block_out_channels=(64, 64, 128),
                 layers_per_block=1, norm_num_groups=32, scaling_factor=0.18215)
 

@@ -3,6 +3,7 @@
 #pragma once
 
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,7 +36,8 @@ void set_error(const char* fmt, ...);
     } while (0)
 
 // Encodes a tiled fp16 tensor map (SWIZZLE_128B).  dims/strides innermost first; strides in
-// bytes for dims 1..rank-1.  Returns 0 on success.
+// bytes for dims 1..rank-1.  Returns 0 on success.  bf16 tensors use the same encoding: TMA only copies bytes, both
+// types are two bytes wide and the out-of-bounds zero fill (0x0000) is +0 in both.
 int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                     const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides);
 
@@ -189,124 +191,74 @@ __device__ __forceinline__ void wgmma_fence_regs(float* d) {
 }
 
 #define B200SD_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-// D[64 x N] (+)= A[64 x 16] (smem, K-major) * B[N x 16]^T (smem, K-major) as ONE wgmma; fp16 in, fp32 accumulate.
+// D[64 x N] (+)= A[64 x 16] (smem, K-major) * B[N x 16]^T (smem, K-major) as ONE wgmma; 16-bit operands of type T
+// (fp16, or bf16 for the VAEs whose activations overflow fp16), fp32 accumulate.
 // N / 2 accumulators per thread (thread t of the warpgroup): d[4 j + e] = (row 16 (t / 32) + (t % 32) / 4 + 8 (e / 2),
 // column 8 j + 2 (t % 4) + e % 2).  Specialised for the widths the kernels issue.
-template <int N>
+template <int N, typename T = __half>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t acc);
-template <>
-__device__ __forceinline__ void wgmma_ss<16>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7"
-        "}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<32>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
-        "}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
-        "}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<96>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
-        "}, %48, %49, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<128>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-        "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<160>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
-        "}, %80, %81, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
-          B200SD_F8(64), B200SD_F8(72)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<192>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
-        "}, %96, %97, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
-          B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<256>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p, 1, 1, 0, 0;\n\t}\n"
-        : B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56),
-          B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88), B200SD_F8(96), B200SD_F8(104), B200SD_F8(112), B200SD_F8(120)
-        : "l"(da), "l"(db), "r"(acc)
-        : "memory");
-}
+// one specialisation per (width, operand type): TY is the PTX type of both operands
+#define B200SD_WGMMA_SS(N, T, TY, REGS, IP, IA, IB, ...)                                                             \
+    template <>                                                                                                      \
+    __device__ __forceinline__ void wgmma_ss<N, T>(float* d, uint64_t da, uint64_t db, uint32_t acc) {               \
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IP ", 0;\n\t"                                          \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." TY "." TY " {" REGS "}, %" #IA ", %" #IB        \
+                     ", p, 1, 1, 0, 0;\n\t}\n"                                                                         \
+                     : __VA_ARGS__                                                                                   \
+                     : "l"(da), "l"(db), "r"(acc)                                                                    \
+                     : "memory");                                                                                    \
+    }
+#define B200SD_WGMMA_SS_BOTH(N, REGS, IP, IA, IB, ...)                  \
+    B200SD_WGMMA_SS(N, __half, "f16", REGS, IP, IA, IB, __VA_ARGS__)   \
+    B200SD_WGMMA_SS(N, __nv_bfloat16, "bf16", REGS, IP, IA, IB, __VA_ARGS__)
+B200SD_WGMMA_SS_BOTH(16,
+                     "%0, %1, %2, %3, %4, %5, %6, %7",
+                     10, 8, 9, B200SD_F8(0))
+B200SD_WGMMA_SS_BOTH(32,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15",
+                     18, 16, 17, B200SD_F8(0), B200SD_F8(8))
+B200SD_WGMMA_SS_BOTH(64,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31",
+                     34, 32, 33, B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24))
+B200SD_WGMMA_SS_BOTH(96,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47",
+                     50, 48, 49, B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40))
+B200SD_WGMMA_SS_BOTH(128,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63",
+                     66, 64, 65, B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56))
+B200SD_WGMMA_SS_BOTH(160,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79",
+                     82, 80, 81, B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56), B200SD_F8(64), B200SD_F8(72))
+B200SD_WGMMA_SS_BOTH(192,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95",
+                     98, 96, 97, B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56), B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88))
+B200SD_WGMMA_SS_BOTH(256,
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+                     "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+                     "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127",
+                     130, 128, 129, B200SD_F8(0), B200SD_F8(8), B200SD_F8(16), B200SD_F8(24), B200SD_F8(32), B200SD_F8(40), B200SD_F8(48), B200SD_F8(56), B200SD_F8(64), B200SD_F8(72), B200SD_F8(80), B200SD_F8(88), B200SD_F8(96), B200SD_F8(104), B200SD_F8(112), B200SD_F8(120))
+#undef B200SD_WGMMA_SS_BOTH
+#undef B200SD_WGMMA_SS
 
 // A from registers (fp16 pairs in the accumulator layout of a 64 x 16 tile), B [16 x 64] from smem, MN-major
 __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
@@ -424,6 +376,30 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
 }
+
+// The 16-bit activation types: fp16 everywhere, bf16 (fp32's exponent range) for the VAEs whose activations exceed
+// fp16's 65504.  Conversions in the form the fp16 kernels were written in, so their fp16 code is unchanged.
+template <typename T>
+struct Elem16;
+template <>
+struct Elem16<__half> {
+    using T2 = __half2;
+    static __device__ __forceinline__ float2 to_float2(T2 v) { return __half22float2(v); }
+    static __device__ __forceinline__ float to_float(__half v) { return __half2float(v); }
+    static __device__ __forceinline__ __half from_float(float v) { return __float2half_rn(v); }
+    static __device__ __forceinline__ uint32_t pack2(float a, float b) { return pack_half2(a, b); }
+};
+template <>
+struct Elem16<__nv_bfloat16> {
+    using T2 = __nv_bfloat162;
+    static __device__ __forceinline__ float2 to_float2(T2 v) { return __bfloat1622float2(v); }
+    static __device__ __forceinline__ float to_float(__nv_bfloat16 v) { return __bfloat162float(v); }
+    static __device__ __forceinline__ __nv_bfloat16 from_float(float v) { return __float2bfloat16_rn(v); }
+    static __device__ __forceinline__ uint32_t pack2(float a, float b) {
+        __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+        return *reinterpret_cast<uint32_t*>(&h);
+    }
+};
 #endif  // __CUDACC__
 
 }  // namespace b200sd

@@ -13,9 +13,9 @@ static inline int grid_for(size_t n, int threads) {
     return static_cast<int>(std::min<size_t>((n + threads - 1) / threads, static_cast<size_t>(num_sms()) * 16));
 }
 
-// ---- NCHW -> NHWC fp16 (pad channels) -------------------------------------------------------
-template <typename T>
-__global__ void nchw_to_nhwc_kernel(const T* __restrict__ in, __half* __restrict__ out, int n, int c, int hw,
+// ---- NCHW -> NHWC fp16 / bf16 (pad channels) ------------------------------------------------
+template <typename T, typename TO = __half>
+__global__ void nchw_to_nhwc_kernel(const T* __restrict__ in, TO* __restrict__ out, int n, int c, int hw,
                                     int c_pad) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
@@ -28,7 +28,7 @@ __global__ void nchw_to_nhwc_kernel(const T* __restrict__ in, __half* __restrict
         const int b = static_cast<int>(px / hw);
         float v = 0.f;
         if (ch < c) v = static_cast<float>(in[(static_cast<size_t>(b) * c + ch) * hw + p]);
-        out[i] = __float2half_rn(v);
+        out[i] = Elem16<TO>::from_float(v);
     }
 }
 
@@ -303,9 +303,10 @@ __global__ void image_post_kernel(const T* __restrict__ in, int c_pad, float* __
 }
 
 
-// ---- latent prep for the VAE decoder: z/scaling -> post_quant_conv (1x1, <= 8 channels) -> NHWC fp16 ----
+// ---- latent prep for the VAE decoder: z/scaling -> post_quant_conv (1x1, <= 8 channels) -> NHWC fp16 / bf16 ----
+template <typename TO>
 __global__ void latent_prep_kernel(const float* __restrict__ z, const float* __restrict__ w /* [c, c] */,
-                                   const float* __restrict__ b, float inv_scale, __half* __restrict__ out, int n, int c,
+                                   const float* __restrict__ b, float inv_scale, TO* __restrict__ out, int n, int c,
                                    int hw, int c_pad) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
@@ -321,7 +322,7 @@ __global__ void latent_prep_kernel(const float* __restrict__ z, const float* __r
             acc = b ? b[co] : 0.f;
             for (int ci = 0; ci < c; ++ci) acc += w[co * c + ci] * v[ci];
         }
-        out[static_cast<size_t>(i) * c_pad + co] = __float2half_rn(acc);
+        out[static_cast<size_t>(i) * c_pad + co] = Elem16<TO>::from_float(acc);
     }
 }
 
@@ -329,23 +330,34 @@ __global__ void latent_prep_kernel(const float* __restrict__ z, const float* __r
 
 using namespace b200sd;
 
-extern "C" int b200sd_nchw_to_nhwc(const void* in, int32_t in_f32, void* out, int32_t n, int32_t c, int32_t h,
-                                   int32_t w, int32_t c_pad, void* stream_) {
+// TO: the output type (fp16 for b200sd_nchw_to_nhwc, bf16 for b200sd_nchw_to_nhwc_bf16)
+template <typename TO>
+static int nchw_to_nhwc(const void* in, int32_t in_f32, void* out, int32_t n, int32_t c, int32_t h, int32_t w,
+                        int32_t c_pad, void* stream_) {
     if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     B200SD_REQUIRE(in && out && c_pad >= c, "b200sd_nchw_to_nhwc: bad arguments");
     const size_t total = static_cast<size_t>(n) * h * w * c_pad;
     if (in_f32)
-        B200SD_CHECK_CUDA(launch_kernel(nchw_to_nhwc_kernel<float>, dim3(grid_for(total, 256)), dim3(256), 0, stream, reinterpret_cast<const float*>(in),
-                                                                             reinterpret_cast<__half*>(out), n, c,
+        B200SD_CHECK_CUDA(launch_kernel(nchw_to_nhwc_kernel<float, TO>, dim3(grid_for(total, 256)), dim3(256), 0, stream, reinterpret_cast<const float*>(in),
+                                                                             reinterpret_cast<TO*>(out), n, c,
                                                                              h * w, c_pad));
     else
-        B200SD_CHECK_CUDA(launch_kernel(nchw_to_nhwc_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), 0, stream, reinterpret_cast<const __half*>(in),
-                                                                              reinterpret_cast<__half*>(out), n, c,
+        B200SD_CHECK_CUDA(launch_kernel(nchw_to_nhwc_kernel<__half, TO>, dim3(grid_for(total, 256)), dim3(256), 0, stream, reinterpret_cast<const __half*>(in),
+                                                                              reinterpret_cast<TO*>(out), n, c,
                                                                               h * w, c_pad));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;
+}
+
+extern "C" int b200sd_nchw_to_nhwc(const void* in, int32_t in_f32, void* out, int32_t n, int32_t c, int32_t h,
+                                   int32_t w, int32_t c_pad, void* stream) {
+    return nchw_to_nhwc<__half>(in, in_f32, out, n, c, h, w, c_pad, stream);
+}
+extern "C" int b200sd_nchw_to_nhwc_bf16(const void* in, int32_t in_f32, void* out, int32_t n, int32_t c, int32_t h,
+                                        int32_t w, int32_t c_pad, void* stream) {
+    return nchw_to_nhwc<__nv_bfloat16>(in, in_f32, out, n, c, h, w, c_pad, stream);
 }
 
 extern "C" int b200sd_nhwc_to_nchw_f32(const void* in, int32_t in_f32, float* out, int32_t n, int32_t c, int32_t h,
@@ -398,6 +410,7 @@ extern "C" int b200sd_embed_tokens(const float* ids, const void* token_embedding
     return 0;
 }
 
+// nearest x2 upsample: a 16-byte copy per vector, so it serves fp16 and bf16 tensors alike
 extern "C" int b200sd_upsample2x(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c,
                                  void* stream_) {
     if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
@@ -525,15 +538,25 @@ extern "C" int b200sd_image_postprocess(const void* in, int32_t in_f32, int32_t 
     return 0;
 }
 
-extern "C" int b200sd_latent_prep(const float* z, const float* w, const float* b, float inv_scale, void* out,
-                                  int32_t n, int32_t c, int32_t h, int32_t wd, int32_t c_pad, void* stream_) {
+template <typename TO>
+static int latent_prep(const float* z, const float* w, const float* b, float inv_scale, void* out, int32_t n, int32_t c,
+                       int32_t h, int32_t wd, int32_t c_pad, void* stream_) {
     if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     B200SD_REQUIRE(z && w && out && c >= 1 && c <= 8 && c_pad >= c, "b200sd_latent_prep: bad arguments");
     const int total = n * h * wd;
-    B200SD_CHECK_CUDA(launch_kernel(latent_prep_kernel, dim3((total + 255) / 256), dim3(256), 0, stream, z, w, b, inv_scale, reinterpret_cast<__half*>(out), n,
+    B200SD_CHECK_CUDA(launch_kernel(latent_prep_kernel<TO>, dim3((total + 255) / 256), dim3(256), 0, stream, z, w, b, inv_scale, reinterpret_cast<TO*>(out), n,
                                                                c, h * wd, c_pad));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;
+}
+
+extern "C" int b200sd_latent_prep(const float* z, const float* w, const float* b, float inv_scale, void* out,
+                                  int32_t n, int32_t c, int32_t h, int32_t wd, int32_t c_pad, void* stream) {
+    return latent_prep<__half>(z, w, b, inv_scale, out, n, c, h, wd, c_pad, stream);
+}
+extern "C" int b200sd_latent_prep_bf16(const float* z, const float* w, const float* b, float inv_scale, void* out,
+                                       int32_t n, int32_t c, int32_t h, int32_t wd, int32_t c_pad, void* stream) {
+    return latent_prep<__nv_bfloat16>(z, w, b, inv_scale, out, n, c, h, wd, c_pad, stream);
 }

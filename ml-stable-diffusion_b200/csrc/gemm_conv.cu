@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cmath>
 #include <stdlib.h>
+#include <type_traits>
 
 namespace b200sd {
 
@@ -169,9 +170,11 @@ __device__ __forceinline__ void split_range(const GemmParams& p, int split, int&
 // `bias` / `res` are already resolved to this row and column (shared or global memory); null = absent.
 // kGeneric = false: compile-time variant for the hot shapes (N % 16 == 0, 16-byte aligned rows): straight-line
 // vector code only, which keeps the kernel small enough for the instruction cache of these microsecond kernels.
-template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial>
+// T: the 16-bit type of the residual and of a 16-bit output (fp16, or bf16 for the overflow-prone VAEs).
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial>
 __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&acc)[16], int out_row, int col0,
-                                                 int split, const float* bias, const __half* res, float2& rowacc) {
+                                                 int split, const float* bias, const T* res, float2& rowacc) {
+    using E = Elem16<T>;
     const bool partial = kGeneric ? (p.partial != nullptr) : kPartial;
     const bool geglu = kGeneric ? (p.geglu != 0) : kGeglu;
     const bool out_f32 = kGeneric ? (p.out_f32 != 0) : kOutF32;
@@ -226,10 +229,10 @@ __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&ac
             for (int j = 0; j < 16; j += 8) {
                 if (j < nvals) {
                     const uint4 rv = *reinterpret_cast<const uint4*>(res + j);
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&rv);
+                    const typename E::T2* h2 = reinterpret_cast<const typename E::T2*>(&rv);
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
-                        const float2 f = __half22float2(h2[q]);
+                        const float2 f = E::to_float2(h2[q]);
                         acc[j + 2 * q] += f.x;
                         acc[j + 2 * q + 1] += f.y;
                     }
@@ -238,7 +241,7 @@ __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&ac
         } else {
 #pragma unroll
             for (int j = 0; j < 16; ++j)
-                if (j < nvals && ocol0 + j < ld) acc[j] += __half2float(res[j]);
+                if (j < nvals && ocol0 + j < ld) acc[j] += E::to_float(res[j]);
         }
     }
     if (out_f32) {
@@ -254,22 +257,22 @@ __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&ac
                 if (j < nvals && ocol0 + j < ld) o[j] = acc[j];
         }
     } else {
-        __half* o = reinterpret_cast<__half*>(p.out) + off;
+        T* o = reinterpret_cast<T*>(p.out) + off;
         if (vec_ok) {
 #pragma unroll
             for (int j = 0; j < 16; j += 8) {
                 if (j < nvals) {
                     uint4 pk;
-                    pk.x = pack_half2(acc[j], acc[j + 1]);
-                    pk.y = pack_half2(acc[j + 2], acc[j + 3]);
-                    pk.z = pack_half2(acc[j + 4], acc[j + 5]);
-                    pk.w = pack_half2(acc[j + 6], acc[j + 7]);
+                    pk.x = E::pack2(acc[j], acc[j + 1]);
+                    pk.y = E::pack2(acc[j + 2], acc[j + 3]);
+                    pk.z = E::pack2(acc[j + 4], acc[j + 5]);
+                    pk.w = E::pack2(acc[j + 6], acc[j + 7]);
                     *reinterpret_cast<uint4*>(o + j) = pk;
                     if (p.rs_out != nullptr) {  // per-row sums of the ROUNDED outputs for the consumer's LayerNorm
-                        const __half2* h2 = reinterpret_cast<const __half2*>(&pk);
+                        const typename E::T2* h2 = reinterpret_cast<const typename E::T2*>(&pk);
 #pragma unroll
                         for (int q = 0; q < 4; ++q) {
-                            const float2 f = __half22float2(h2[q]);
+                            const float2 f = E::to_float2(h2[q]);
                             rowacc.x += f.x + f.y;
                             rowacc.y = fmaf(f.x, f.x, fmaf(f.y, f.y, rowacc.y));
                         }
@@ -279,7 +282,7 @@ __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&ac
         } else {
 #pragma unroll
             for (int j = 0; j < 16; ++j)
-                if (j < nvals && ocol0 + j < ld) o[j] = __float2half_rn(acc[j]);
+                if (j < nvals && ocol0 + j < ld) o[j] = E::from_float(acc[j]);
         }
     }
 }
@@ -552,7 +555,7 @@ __device__ __forceinline__ void staged_epilogue(const GemmParams& p, const TileC
 // k-blocks [kb0, kb1) of the ring.  A stage is released (one arrival per warpgroup) once the wgmma that read it retired;
 // one k-block stays in flight behind the one being issued.  One unconditional m64nkBNk16 per k16 step: ptxas only
 // pipelines wgmma whose accumulator registers no predicated instruction writes.
-template <int kBN>
+template <typename T, int kBN>
 __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[kBN / 2], const uint8_t* smem_a,
                                               const uint8_t* smem_b, uint64_t* full_bar,
                                               uint64_t* empty_bar, int kb0, int kb1, int& stage, uint32_t& phase,
@@ -566,7 +569,7 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k)
-            wgmma_ss<kBN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb > kb0 || k > 0) ? 1u : 0u);
+            wgmma_ss<kBN, T>(acc, adesc + 2 * k, bdesc + 2 * k, (kb > kb0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();
         if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
@@ -686,8 +689,9 @@ __device__ __forceinline__ void cluster_splitk_reduce(const GemmParams& p, const
     }
 }
 
+// T: operand / 16-bit output type (__half; __nv_bfloat16 for the generic, plain and fp32-output variants only).
 // kBN: tile width (columns); p.block_n == kBN.  Each consumer thread holds kBN / 2 fp32 accumulators.
-template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN>
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN>
 __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __grid_constant__ GemmParams p) {
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
     // integer-rounded pointer -- lets the compiler emit LDS / STS for everything derived from it; rounding through
@@ -870,7 +874,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
             }
             const int bias_base = (p.bias_mode == 2 && p.bias_rows > 0 && valid) ? (out_row / p.bias_rows) * p.bias_stride : 0;
 
-            gemm_mainloop<kBN>(p, acc, smem_a, smem_b, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
+            gemm_mainloop<T, kBN>(p, acc, smem_a, smem_b, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
 
             if (p.res_smem) cp_async_wait_all();
             epi_bar_sync();  // every wgmma of the tile retired: the stages may be overwritten; staged operands visible
@@ -904,11 +908,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
                         const float* bptr = nullptr;
                         if (p.bias_mode == 1) bptr = bias_s + bias_sel * p.block_n + c;
                         else if (kGeneric && p.bias_mode == 2) bptr = p.bias + bias_base + ncol0 + c;
-                        const __half* rptr = nullptr;
-                        if (p.res_smem) rptr = res_s + row * ldr + c;
+                        const T* rptr = nullptr;
+                        if (p.res_smem) rptr = reinterpret_cast<const T*>(res_s + row * ldr + c);
                         else if (kGeneric && p.residual != nullptr)
-                            rptr = p.residual + static_cast<size_t>(out_row) * p.n_store + ((ncol0 + c) >> (p.geglu ? 1 : 0));
-                        epilogue_store16<kGeneric, kGeglu, kOutF32, kPartial>(p, a16, out_row, ncol0 + c, t.split, bptr, rptr, rowacc);
+                            rptr = reinterpret_cast<const T*>(p.residual + static_cast<size_t>(out_row) * p.n_store +
+                                                              ((ncol0 + c) >> (p.geglu ? 1 : 0)));
+                        epilogue_store16<T, kGeneric, kGeglu, kOutF32, kPartial>(p, a16, out_row, ncol0 + c, t.split, bptr, rptr, rowacc);
                     };
                     auto process32 = [&](const uint32_t (&v)[32], int c) {
                         if (!valid) return;
@@ -968,9 +973,17 @@ static int gemm_width_index(int bn) {
     return -1;
 }
 using KernelFn = void (*)(GemmParams);
-template <bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged>
+// The instantiation for one width.  bf16 (the VAEs that overflow fp16) is compiled for the generic variant at every
+// width and for the plain / fp32-output variants at the widths >= 32 (plan_gemm sends width 16 to the generic one):
+// 8 + 7 + 7 = 22 kernels; the fp16 variants keep all eight widths.
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN>
+static constexpr KernelFn gemm_fn() {
+    if constexpr (kBN == 16 && !kGeneric && !std::is_same<T, __half>::value) return nullptr;
+    else return wgmma_gemm_kernel<T, kGeneric, kGeglu, kOutF32, kPartial, kStaged, kBN>;
+}
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged>
 static KernelFn gemm_kernel(int width_index) {
-#define B200SD_GEMM_FN(bn) wgmma_gemm_kernel<kGeneric, kGeglu, kOutF32, kPartial, kStaged, bn>
+#define B200SD_GEMM_FN(bn) gemm_fn<T, kGeneric, kGeglu, kOutF32, kPartial, kStaged, bn>()
     static const KernelFn fns[kNumGemmWidths] = {B200SD_GEMM_FN(256), B200SD_GEMM_FN(192), B200SD_GEMM_FN(160),
                                                  B200SD_GEMM_FN(128), B200SD_GEMM_FN(96),  B200SD_GEMM_FN(64),
                                                  B200SD_GEMM_FN(32),  B200SD_GEMM_FN(16)};
@@ -1355,7 +1368,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) halo_conv_kernel(const __grid
                                 const float* bptr = p.bias != nullptr ? bias_s + cc : nullptr;
                                 const __half* rptr = p.residual != nullptr
                                     ? p.residual + static_cast<size_t>(out_row) * p.n_store + ncol0 + cc : nullptr;
-                                epilogue_store16<true, false, false, false>(p, a16, out_row, ncol0 + cc, 0, bptr, rptr, rowacc);
+                                epilogue_store16<__half, true, false, false, false>(p, a16, out_row, ncol0 + cc, 0, bptr, rptr, rowacc);
                             }
                         }
                     }
@@ -1555,8 +1568,25 @@ static int halo_pick_block_n(const b200sd_gemm_args& a) {
     return best_bn;
 }
 
-static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
+// bf16: the operands, the residual and a 16-bit output are bf16 (b200sd_gemm_bf16).  That path serves the VAEs whose
+// activations overflow fp16: modes 0 / 1, stride 1 / 2, pad_after_only, bias, residual, fp32 output and tiled weights,
+// on the generic, plain and fp32-output epilogues.  Everything else is rejected by name, and the plan never takes
+// split-K (workspace or cluster) or the staged epilogue, whatever the environment switches say.
+static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false) {
     B200SD_REQUIRE(a.mode == 0 || a.mode == 1, "b200sd_gemm: bad mode %d", a.mode);
+    if (bf16) {
+        B200SD_REQUIRE(!a.geglu, "b200sd_gemm_bf16: geglu is not supported in bf16");
+        B200SD_REQUIRE(a.split_k <= 1, "b200sd_gemm_bf16: split_k=%d is not supported in bf16 (0 or 1)", a.split_k);
+        B200SD_REQUIRE(!a.halo && !a.upsample2x, "b200sd_gemm_bf16: halo / upsample2x are not supported in bf16");
+        B200SD_REQUIRE(a.gn_groups == 0 && !a.gn_chan0 && !a.gn_chan1 && !a.gn_gamma && !a.gn_beta,
+                       "b200sd_gemm_bf16: gn_* (fused GroupNorm) is not supported in bf16");
+        B200SD_REQUIRE(!a.cs_partial && !a.cs_chan && !a.cs_tickets && !a.rs_out,
+                       "b200sd_gemm_bf16: cs_* / rs_out (statistics outputs) are not supported in bf16");
+        B200SD_REQUIRE(a.ln_parts == 0 && !a.ln_stat && !a.ln_wg, "b200sd_gemm_bf16: ln_* (LayerNorm fold) is not supported in bf16");
+        B200SD_REQUIRE(!a.a2 && !a.a3 && a.c2 == 0 && a.c3 == 0,
+                       "b200sd_gemm_bf16: a2 / a3 (folded shortcut) are not supported in bf16");
+        B200SD_REQUIRE(a.act == 0, "b200sd_gemm_bf16: act=%d is not supported in bf16", a.act);
+    }
     B200SD_REQUIRE(!a.pad_after_only || (a.mode == 1 && a.stride == 2), "b200sd_gemm: pad_after_only is for stride-2 convolutions");
     B200SD_REQUIRE(a.c0 > 0 && a.c0 % 8 == 0 && a.c1 >= 0 && a.c1 % 8 == 0,
                    "b200sd_gemm: channel counts must be positive multiples of 8 (c0=%d c1=%d)", a.c0, a.c1);
@@ -1615,7 +1645,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
     // spread of a single shape), so they were kept.  The largest misses: conv 2560->1280 at 8x8 (1.3x) and linear
     // 1280->1280 at M = 512 (1.25x). ----
     const int sms = num_sms();
-    const bool can_split = !a.geglu && a.n % 4 == 0 && a.act == 0 && !want_stats && a.ln_parts == 0;
+    const bool can_split = !bf16 && !a.geglu && a.n % 4 == 0 && a.act == 0 && !want_stats && a.ln_parts == 0;
     auto epi_cycles = [&](int bn) { return 400.0 + (bn / 32.0) * (a.geglu ? 520.0 : 230.0); };
     auto kb_cycles = [&](int bn) { return std::max(2.0 * bn, (kAStage + 128.0 * bn) / 38.0); };
     double best_t = 1e30;
@@ -1697,7 +1727,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl) {
     const int per_stage = kAStage + pl.block_n * kBK * 2;
     {
         // staged epilogue: fp16 tile in shared memory, row-contiguous residual reads / stores, statistics outputs
-        const bool eligible = regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
+        const bool eligible = !bf16 && regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
         // column statistics need the staged epilogue; row statistics alone ride on the register epilogue (every thread
         // owns a row there), which keeps the residual tile prefetched in shared memory during the main loop
         pl.staged = (eligible && (a.cs_partial != nullptr || (a.residual != nullptr && staged_enabled()))) ? 1 : 0;
@@ -1749,9 +1779,9 @@ static size_t plan_workspace(const GemmPlan& pl) {
 
 extern void count_launch(int n);
 
-static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
+static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16) {
     GemmPlan pl;
-    if (int rc = plan_gemm(a, pl)) return rc;
+    if (int rc = plan_gemm(a, pl, bf16)) return rc;
     B200SD_REQUIRE(a.a0 && a.wgt && a.out, "b200sd_gemm: null pointer");
     B200SD_REQUIRE(a.c1 == 0 || a.a1, "b200sd_gemm: a1 is null but c1 > 0");
     const size_t ws = plan_workspace(pl);
@@ -1922,24 +1952,35 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
     B200SD_REQUIRE(a.act == 0 || (a.act >= 1 && a.act <= 3 && pl.splits == 1 && !a.geglu), "b200sd_gemm: act=%d unsupported here", a.act);
     const int wi = gemm_width_index(pl.block_n);
     const int variant = pl.variant;
-    KernelFn fn;
-    switch (variant) {
-        case kVariantGeneric: fn = gemm_kernel<true, false, false, false, false>(wi); break;
-        case kVariantStaged: fn = gemm_kernel<false, false, false, false, true>(wi); break;
-        case kVariantSplitK: fn = gemm_kernel<false, false, false, true, false>(wi); break;
-        case kVariantGeglu: fn = gemm_kernel<false, true, false, false, false>(wi); break;
-        case kVariantF32: fn = gemm_kernel<false, false, true, false, false>(wi); break;
-        default: fn = gemm_kernel<false, false, false, false, false>(wi); break;
+    KernelFn fn = nullptr;
+    if (bf16) {  // plan_gemm gives bf16 only these three variants
+        switch (variant) {
+            case kVariantGeneric: fn = gemm_kernel<__nv_bfloat16, true, false, false, false, false>(wi); break;
+            case kVariantF32: fn = gemm_kernel<__nv_bfloat16, false, false, true, false, false>(wi); break;
+            case kVariantPlain: fn = gemm_kernel<__nv_bfloat16, false, false, false, false, false>(wi); break;
+            default: break;
+        }
+    } else {
+        switch (variant) {
+            case kVariantGeneric: fn = gemm_kernel<__half, true, false, false, false, false>(wi); break;
+            case kVariantStaged: fn = gemm_kernel<__half, false, false, false, false, true>(wi); break;
+            case kVariantSplitK: fn = gemm_kernel<__half, false, false, false, true, false>(wi); break;
+            case kVariantGeglu: fn = gemm_kernel<__half, false, true, false, false, false>(wi); break;
+            case kVariantF32: fn = gemm_kernel<__half, false, false, true, false, false>(wi); break;
+            default: fn = gemm_kernel<__half, false, false, false, false, false>(wi); break;
+        }
     }
+    B200SD_REQUIRE(fn != nullptr, "b200sd_gemm: no %s kernel for variant %d at block_n %d", bf16 ? "bf16" : "fp16", variant,
+                   pl.block_n);
     if (pl.splits > 1 && !pl.cluster) {
         // the separate reduce kernel applies bias / residual; the partial writer must not
         p.bias = nullptr;
         p.residual = nullptr;
     }
-    static bool attr_set[6][kNumGemmWidths] = {};
-    if (!attr_set[variant][wi]) {
+    static bool attr_set[2][6][kNumGemmWidths] = {};
+    if (!attr_set[bf16][variant][wi]) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set[variant][wi] = true;
+        attr_set[bf16][variant][wi] = true;
     }
     if (pl.cluster) {
         B200SD_REQUIRE(variant == 1, "b200sd_gemm: cluster split-K needs the regular epilogue variant");
@@ -1984,14 +2025,17 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream) {
 
 }  // namespace b200sd
 
-extern "C" int b200sd_gemm(const b200sd_gemm_args* args, void* stream) {
+static int gemm_entry(const b200sd_gemm_args* args, void* stream, bool bf16) {
     if (!b200sd::launch_class_enabled(1)) return 0;  // bench.py's per-class timing graphs
     if (!args) {
-        b200sd::set_error("b200sd_gemm: args is null");
+        b200sd::set_error(bf16 ? "b200sd_gemm_bf16: args is null" : "b200sd_gemm: args is null");
         return 2;
     }
-    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream));
+    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream), bf16);
 }
+
+extern "C" int b200sd_gemm(const b200sd_gemm_args* args, void* stream) { return gemm_entry(args, stream, false); }
+extern "C" int b200sd_gemm_bf16(const b200sd_gemm_args* args, void* stream) { return gemm_entry(args, stream, true); }
 
 extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {
     if (!args || !out4) return 2;
@@ -2003,28 +2047,31 @@ extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {
 
 // Planning query before the weights are tiled: a halo call plans for chunk-major tiled weights of the requested (or the
 // preferred) width.
-static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl) {
+static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl, bool bf16) {
     b200sd_gemm_args a = *args;
-    if (a.halo) {
+    if (a.halo && !bf16) {
         if (a.block_n == 0) a.block_n = b200sd::halo_pick_block_n(a);
         a.wgt_tiled = 1;
     }
-    return b200sd::plan_gemm(a, pl);
+    return b200sd::plan_gemm(a, pl, bf16);
 }
 
-extern "C" int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8) {
+static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16) {
     if (!args || !out8) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = plan_query(args, pl)) return rc;
+    if (int rc = plan_query(args, pl, bf16)) return rc;
     out8[0] = pl.block_n, out8[1] = pl.splits, out8[2] = pl.kb_total, out8[3] = pl.n_tiles;
     out8[4] = pl.cs_slots, out8[5] = pl.staged, out8[6] = pl.stages, out8[7] = pl.m_tiles;
     return 0;
 }
 
-extern "C" int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
+extern "C" int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, false); }
+extern "C" int b200sd_gemm_plan_ex_bf16(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, true); }
+
+static int describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size, bool bf16) {
     if (!args || !buf || buf_size == 0) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = plan_query(args, pl)) return rc;
+    if (int rc = plan_query(args, pl, bf16)) return rc;
     // variant: GemmVariant of the GEMM kernel (-1: halo convolution); halo_kind / halo_wide: which halo_conv_kernel
     // instantiation runs (-1 / 0 for the GEMM kernel); win: the halo walk over th x tw windows instead of image rows
     snprintf(buf, buf_size,
@@ -2034,6 +2081,13 @@ extern "C" int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf
              pl.bn_img, pl.bh, pl.bw, pl.bias_mode, pl.res_smem, pl.epi_smem, pl.cluster, pl.staged, pl.variant, pl.halo_kind,
              pl.halo && pl.block_n > 128 ? 1 : 0, pl.halo ? pl.win : 0);
     return 0;
+}
+
+extern "C" int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
+    return describe_plan(args, buf, buf_size, false);
+}
+extern "C" int b200sd_gemm_describe_plan_bf16(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
+    return describe_plan(args, buf, buf_size, true);
 }
 
 extern "C" size_t b200sd_gemm_workspace_bytes(const b200sd_gemm_args* args) {

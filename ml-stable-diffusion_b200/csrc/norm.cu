@@ -18,12 +18,13 @@ extern void count_launch(int n);
 
 static constexpr int kGnMaxImages = 1024;
 
-__device__ __forceinline__ void load8(const __half* src, float (&f)[8]) {
+template <typename T>
+__device__ __forceinline__ void load8(const T* src, float (&f)[8]) {
     const uint4 raw = *reinterpret_cast<const uint4*>(src);
-    const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
+    const typename Elem16<T>::T2* h2 = reinterpret_cast<const typename Elem16<T>::T2*>(&raw);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-        const float2 t = __half22float2(h2[q]);
+        const float2 t = Elem16<T>::to_float2(h2[q]);
         f[2 * q] = t.x;
         f[2 * q + 1] = t.y;
     }
@@ -35,8 +36,9 @@ __device__ __forceinline__ void load8(const __half* src, float (&f)[8]) {
 // registers over the chunk's pixels with perfectly coalesced 16 B loads; a fixed-order shared-memory
 // tree folds rows -> channels -> groups (no atomics: bitwise reproducible).  The last block of each
 // image (ticket counter) merges the chunk partials in chunk order with Chan's formula and writes the
-// final (mean, rstd) per group.
-__global__ void __launch_bounds__(416) gn_stats_kernel(const __half* __restrict__ x0, const __half* __restrict__ x1,
+// final (mean, rstd) per group.  T: fp16, or bf16 for the VAEs whose activations overflow fp16 (statistics stay fp32).
+template <typename T>
+__global__ void __launch_bounds__(416) gn_stats_kernel(const T* __restrict__ x0, const T* __restrict__ x1,
                                                        int c0, int c1, int hw, int groups, int chunks, int rows,
                                                        float eps, float* __restrict__ partial /* [n][chunks][g][2] */,
                                                        float* __restrict__ final_stats /* [n][g][2] */,
@@ -59,7 +61,7 @@ __global__ void __launch_bounds__(416) gn_stats_kernel(const __half* __restrict_
 #pragma unroll
     for (int e = 0; e < 8; ++e) s[e] = q[e] = 0.f;
     const bool from0 = ch < c0;
-    const __half* base = from0 ? x0 + static_cast<size_t>(n) * hw * c0 + ch
+    const T* base = from0 ? x0 + static_cast<size_t>(n) * hw * c0 + ch
                                : x1 + static_cast<size_t>(n) * hw * c1 + (ch - c0);
     const int cs = from0 ? c0 : c1;
     const bool active = r < rows;  // the block is padded to whole warps; padding threads only help reduce
@@ -171,12 +173,13 @@ __global__ void __launch_bounds__(416) gn_stats_kernel(const __half* __restrict_
 }
 
 // ---- GroupNorm pass 2: normalise, affine, optional SiLU (and concat of the two sources) ------------
-__global__ void __launch_bounds__(256) gn_apply_kernel(const __half* __restrict__ x0, const __half* __restrict__ x1,
+template <typename T>
+__global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x0, const T* __restrict__ x1,
                                                        int c0, int c1, int hw, int groups,
                                                        const float* __restrict__ final_stats,
                                                        const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, int silu,
-                                                       __half* __restrict__ out, int px_per_block) {
+                                                       T* __restrict__ out, int px_per_block) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int C = c0 + c1;
@@ -201,8 +204,8 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __half* __restrict_
     for (int i = threadIdx.x; i < total; i += blockDim.x) {
         const int px = px0 + i / vecs;
         const int ch = (i % vecs) * 8;
-        const __half* src = (ch < c0) ? x0 + (static_cast<size_t>(n) * hw + px) * c0 + ch
-                                      : x1 + (static_cast<size_t>(n) * hw + px) * c1 + (ch - c0);
+        const T* src = (ch < c0) ? x0 + (static_cast<size_t>(n) * hw + px) * c0 + ch
+                                 : x1 + (static_cast<size_t>(n) * hw + px) * c1 + (ch - c0);
         float f[8];
         load8(src, f);
 #pragma unroll
@@ -211,10 +214,10 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __half* __restrict_
             f[e] = silu ? silu_f(y) : y;
         }
         uint4 pk;
-        pk.x = pack_half2(f[0], f[1]);
-        pk.y = pack_half2(f[2], f[3]);
-        pk.z = pack_half2(f[4], f[5]);
-        pk.w = pack_half2(f[6], f[7]);
+        pk.x = Elem16<T>::pack2(f[0], f[1]);
+        pk.y = Elem16<T>::pack2(f[2], f[3]);
+        pk.z = Elem16<T>::pack2(f[4], f[5]);
+        pk.w = Elem16<T>::pack2(f[6], f[7]);
         *reinterpret_cast<uint4*>(out + (static_cast<size_t>(n) * hw + px) * C + ch) = pk;
     }
 }
@@ -299,11 +302,12 @@ __global__ void __launch_bounds__(256) gn_apply_chan_kernel(const __half* __rest
 // through distributed shared memory in rank order -- no global barrier, no partial buffers, no atomics (bitwise
 // reproducible).  Thread t owns vector column t % vpr for all its pixels, so per-channel
 // partial sums live in registers and fold rows -> channels -> groups in a fixed order.
-template <int kRowsInFlight>
-__global__ void gn_cluster_kernel(const __half* __restrict__ x0, const __half* __restrict__ x1, int c0, int c1, int hw,
+template <typename T, int kRowsInFlight>
+__global__ void gn_cluster_kernel(const T* __restrict__ x0, const T* __restrict__ x1, int c0, int c1, int hw,
                                   int groups, int chunk_ch, int rows_per_cta, float eps,
                                   const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
-                                  __half* __restrict__ out) {
+                                  T* __restrict__ out) {
+    using E = Elem16<T>;
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     const int cs = gridDim.x, rank = blockIdx.x;
@@ -319,7 +323,7 @@ __global__ void gn_cluster_kernel(const __half* __restrict__ x0, const __half* _
     const int ch = ch0 + cv * 8;
     const bool from0 = ch < c0;
     const int ld = from0 ? c0 : c1;
-    const __half* src = from0 ? x0 + static_cast<size_t>(n) * hw * c0 + ch : x1 + static_cast<size_t>(n) * hw * c1 + (ch - c0);
+    const T* src = from0 ? x0 + static_cast<size_t>(n) * hw * c0 + ch : x1 + static_cast<size_t>(n) * hw * c1 + (ch - c0);
 
     extern __shared__ __align__(16) uint8_t csm[];
     uint4* slab = reinterpret_cast<uint4*>(csm);                                   // [rows_per_cta][vpr]
@@ -353,10 +357,10 @@ __global__ void gn_cluster_kernel(const __half* __restrict__ x0, const __half* _
                 const int px = pxb + i * TY;
                 if (px < px1) {
                     slab[(px - px0) * vpr + cv] = raw[i];
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&raw[i]);
+                    const typename E::T2* h2 = reinterpret_cast<const typename E::T2*>(&raw[i]);
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
-                        const float2 t = __half22float2(h2[q]);
+                        const float2 t = E::to_float2(h2[q]);
                         acc[2 * q] += t.x;
                         acc[2 * q + 1] += t.y;
                         acq[2 * q] = fmaf(t.x, t.x, acq[2 * q]);
@@ -414,15 +418,15 @@ __global__ void gn_cluster_kernel(const __half* __restrict__ x0, const __half* _
             sc8[e] = stat[ng + g] * gamma[ch + e];
             sh8[e] = fmaf(-mean8[e], sc8[e], beta[ch + e]);
         }
-        __half* dst = out + static_cast<size_t>(n) * hw * C + ch;
+        T* dst = out + static_cast<size_t>(n) * hw * C + ch;
 #pragma unroll 2
         for (int px = px0 + ty; px < px1; px += TY) {
             const uint4 raw = slab[(px - px0) * vpr + cv];
-            const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
+            const typename E::T2* h2 = reinterpret_cast<const typename E::T2*>(&raw);
             float f[8];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
-                const float2 t = __half22float2(h2[q]);
+                const float2 t = E::to_float2(h2[q]);
                 f[2 * q] = t.x;
                 f[2 * q + 1] = t.y;
             }
@@ -432,10 +436,10 @@ __global__ void gn_cluster_kernel(const __half* __restrict__ x0, const __half* _
                 f[e] = silu ? __fdividef(y, 1.0f + __expf(-y)) : y;
             }
             uint4 pk;
-            pk.x = pack_half2(f[0], f[1]);
-            pk.y = pack_half2(f[2], f[3]);
-            pk.z = pack_half2(f[4], f[5]);
-            pk.w = pack_half2(f[6], f[7]);
+            pk.x = E::pack2(f[0], f[1]);
+            pk.y = E::pack2(f[2], f[3]);
+            pk.z = E::pack2(f[4], f[5]);
+            pk.w = E::pack2(f[6], f[7]);
             *reinterpret_cast<uint4*>(dst + static_cast<size_t>(px) * C) = pk;
         }
     }
@@ -533,14 +537,16 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restric
 }
 
 
-// ---- row softmax: fp32 scores [rows, cols] -> fp16 probabilities (VAE mid-block attention, d=512) ----
-__global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ in, __half* __restrict__ out,
+// ---- row softmax: fp32 scores [rows, cols] -> fp16 / bf16 probabilities (VAE mid-block attention, d=512; the
+// probabilities take the type of the P V GEMM's other operand) ----
+template <typename T>
+__global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ in, T* __restrict__ out,
                                                            int cols, float scale_log2) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const size_t row = blockIdx.x;
     const float* src = in + row * cols;
-    __half* dst = out + row * cols;
+    T* dst = out + row * cols;
     __shared__ float red[8];
     float m = -INFINITY;
     for (int c = threadIdx.x; c < cols; c += blockDim.x) m = fmaxf(m, src[c] * scale_log2);
@@ -560,7 +566,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
     s = 0.f;
     for (int i = 0; i < 8; ++i) s += red[i];
     const float inv = 1.0f / s;
-    for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[c] = __float2half_rn(exp2f(src[c] * scale_log2 - m) * inv);
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[c] = Elem16<T>::from_float(exp2f(src[c] * scale_log2 - m) * inv);
 }
 
 }  // namespace b200sd
@@ -575,9 +581,11 @@ extern "C" size_t b200sd_group_norm_workspace_bytes(int32_t n_img, int32_t hw, i
     return two_kernel * sizeof(float);
 }
 
-extern "C" int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
-                                 int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
-                                 void* out, float* stats_ws, size_t stats_ws_bytes, void* stream_) {
+// b200sd_group_norm (T = __half) and b200sd_group_norm_bf16 (T = __nv_bfloat16): same plans, same kernels
+template <typename T>
+static int group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
+                      int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
+                      void* out, float* stats_ws, size_t stats_ws_bytes, void* stream_) {
     if (!b200sd::launch_class_enabled(4)) return 0;  // bench.py's per-class timing graphs
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const int C = c0 + c1;
@@ -621,7 +629,7 @@ extern "C" int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int
                              (2 * static_cast<size_t>(TY) * chunk + 2 * chunk + 4 * (chunk / cpg)) * sizeof(float);
         if (mode == 1 && vpr <= 64 && C % chunk == 0 && csmem <= 200 * 1024 && n_img <= 65535 && C / chunk <= 65535) {
             const int deep = (rows_per_cta + TY - 1) / TY >= 3 ? 1 : 0;
-            auto kern = deep ? gn_cluster_kernel<8> : gn_cluster_kernel<2>;
+            auto kern = deep ? gn_cluster_kernel<T, 8> : gn_cluster_kernel<T, 2>;
             static bool attr[2] = {false, false};
             if (!attr[deep]) {
                 B200SD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -645,11 +653,11 @@ extern "C" int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int
                 at[1].val.programmaticStreamSerializationAllowed = 1;
                 cfg.numAttrs = 2;
             }
-            B200SD_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, reinterpret_cast<const __half*>(x0),
-                                                 reinterpret_cast<const __half*>(x1), static_cast<int>(c0),
+            B200SD_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, reinterpret_cast<const T*>(x0),
+                                                 reinterpret_cast<const T*>(x1), static_cast<int>(c0),
                                                  static_cast<int>(c1), static_cast<int>(hw), static_cast<int>(groups), chunk,
                                                  rows_per_cta, eps, gamma, beta, static_cast<int>(silu),
-                                                 reinterpret_cast<__half*>(out)));
+                                                 reinterpret_cast<T*>(out)));
             B200SD_CHECK_CUDA(cudaGetLastError());
             count_launch(1);
             return 0;
@@ -664,24 +672,37 @@ extern "C" int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int
     const size_t smem1 = (static_cast<size_t>(rows) * C * 2 + static_cast<size_t>(C) * 2) * sizeof(float);
     static size_t smem1_max = 48 * 1024;
     if (smem1 > smem1_max) {
-        B200SD_CHECK_CUDA(cudaFuncSetAttribute(gn_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        B200SD_CHECK_CUDA(cudaFuncSetAttribute(gn_stats_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                static_cast<int>(smem1)));
         smem1_max = smem1;
     }
-    B200SD_CHECK_CUDA(launch_kernel(gn_stats_kernel, dim3(dim3(chunks, n_img)), dim3(threads), smem1, stream, 
-        reinterpret_cast<const __half*>(x0), reinterpret_cast<const __half*>(x1), c0, c1, hw, groups, chunks, rows, eps,
+    B200SD_CHECK_CUDA(launch_kernel(gn_stats_kernel<T>, dim3(dim3(chunks, n_img)), dim3(threads), smem1, stream, 
+        reinterpret_cast<const T*>(x0), reinterpret_cast<const T*>(x1), c0, c1, hw, groups, chunks, rows, eps,
         partial, final_stats, tickets));
     B200SD_CHECK_CUDA(cudaGetLastError());
     const int want_blocks = std::max(1, (num_sms() * 4) / std::max(1, n_img));
     const int px_per_block = std::max(1, (hw + want_blocks - 1) / want_blocks);
     const int blocks = (hw + px_per_block - 1) / px_per_block;
     const size_t smem2 = 2 * static_cast<size_t>(C) * sizeof(float);
-    B200SD_CHECK_CUDA(launch_kernel(gn_apply_kernel, dim3(dim3(blocks, n_img)), dim3(256), smem2, stream, 
-        reinterpret_cast<const __half*>(x0), reinterpret_cast<const __half*>(x1), c0, c1, hw, groups, final_stats,
-        gamma, beta, silu, reinterpret_cast<__half*>(out), px_per_block));
+    B200SD_CHECK_CUDA(launch_kernel(gn_apply_kernel<T>, dim3(dim3(blocks, n_img)), dim3(256), smem2, stream, 
+        reinterpret_cast<const T*>(x0), reinterpret_cast<const T*>(x1), c0, c1, hw, groups, final_stats,
+        gamma, beta, silu, reinterpret_cast<T*>(out), px_per_block));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(2);
     return 0;
+}
+
+extern "C" int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
+                                 int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
+                                 void* out, float* stats_ws, size_t stats_ws_bytes, void* stream) {
+    return group_norm<__half>(x0, x1, c0, c1, n_img, hw, groups, eps, gamma, beta, silu, out, stats_ws, stats_ws_bytes, stream);
+}
+
+extern "C" int b200sd_group_norm_bf16(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
+                                      int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
+                                      void* out, float* stats_ws, size_t stats_ws_bytes, void* stream) {
+    return group_norm<__nv_bfloat16>(x0, x1, c0, c1, n_img, hw, groups, eps, gamma, beta, silu, out, stats_ws,
+                                     stats_ws_bytes, stream);
 }
 
 extern "C" int b200sd_group_norm_apply(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
@@ -728,14 +749,21 @@ extern "C" int b200sd_layer_norm(const void* x, const float* gamma, const float*
     return 0;
 }
 
-extern "C" int b200sd_softmax_rows(const float* in, void* out, int32_t rows, int32_t cols, float scale,
-                                   void* stream_) {
+template <typename T>
+static int softmax_rows(const float* in, void* out, int32_t rows, int32_t cols, float scale, void* stream_) {
     if (!b200sd::launch_class_enabled(4)) return 0;  // bench.py's per-class timing graphs
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     B200SD_REQUIRE(in && out && rows > 0 && cols > 0, "b200sd_softmax_rows: bad arguments");
-    B200SD_CHECK_CUDA(launch_kernel(softmax_rows_kernel, dim3(rows), dim3(256), 0, stream, in, reinterpret_cast<__half*>(out), cols,
+    B200SD_CHECK_CUDA(launch_kernel(softmax_rows_kernel<T>, dim3(rows), dim3(256), 0, stream, in, reinterpret_cast<T*>(out), cols,
                                                   scale * 1.4426950408889634f));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;
+}
+
+extern "C" int b200sd_softmax_rows(const float* in, void* out, int32_t rows, int32_t cols, float scale, void* stream) {
+    return softmax_rows<__half>(in, out, rows, cols, scale, stream);
+}
+extern "C" int b200sd_softmax_rows_bf16(const float* in, void* out, int32_t rows, int32_t cols, float scale, void* stream) {
+    return softmax_rows<__nv_bfloat16>(in, out, rows, cols, scale, stream);
 }

@@ -113,6 +113,11 @@ _SIGNATURES = {
     "b200sd_image_postprocess": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
 }
+# bf16 twins (include/b200sd.h): same signatures, every fp16 pointer is bf16
+for _name in ("b200sd_gemm", "b200sd_gemm_plan_ex", "b200sd_gemm_describe_plan", "b200sd_group_norm",
+              "b200sd_softmax_rows", "b200sd_latent_prep", "b200sd_nchw_to_nhwc"):
+    _SIGNATURES[_name + "_bf16"] = _SIGNATURES[_name]
+del _name
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
@@ -175,6 +180,26 @@ def _req(t, dtype, what):
                           f"contiguous={t.is_contiguous()}")
 
 
+ACT_DTYPES = (torch.float16, torch.bfloat16)  # bf16: the VAEs whose activations overflow fp16 (force_upcast)
+
+
+def _act_dtype(x, what):
+    """The 16-bit type a call runs in: its input's (bf16, else fp16, which _req then demands)."""
+    dt = torch.bfloat16 if x.dtype == torch.bfloat16 else torch.float16
+    _req(x, dt, what)
+    return dt
+
+
+def _same16(dt, a, b, what):
+    """Every 16-bit operand of one call shares the input's type (a, b: optional operands)."""
+    if (a is not None and a.dtype != dt) or (b is not None and b.dtype != dt):
+        raise B200SDError(f"{what}: operand types differ in a {dt} call (all 16-bit operands share one type)")
+
+
+def _sfx(dt):
+    return "_bf16" if dt == torch.bfloat16 else ""
+
+
 def gemm_args(mode, a0, wgt, out, *, a1=None, bias=None, residual=None, m=0, n=0, n_img=0, h=0, w=0, stride=1,
               geglu=False, bias_rows=0, bias_stride=0, split_k=0, block_n=0, workspace=None, act=0, pad_after_only=False):
     args = GemmArgs()
@@ -205,11 +230,12 @@ def gemm_args(mode, a0, wgt, out, *, a1=None, bias=None, residual=None, m=0, n=0
 
 def describe_plan(mode, m=0, n=0, c0=0, c1=0, n_img=0, h=0, w=0, stride=1, geglu=False, has_bias=True,
                   has_residual=False, bias_rows=0, split_k=0, block_n=0, out_f32=False, act=0, pad_after_only=False,
-                  rowstats=False, stats=False, cs_hw=0, ln=False, c2=0, c3=0, halo=0, upsample=False, gn=False) -> str:
+                  rowstats=False, stats=False, cs_hw=0, ln=False, c2=0, c3=0, halo=0, upsample=False, gn=False,
+                  bf16=False) -> str:
     """Host-only: the tiling the launcher would choose (no GPU needed).  The flags mirror linear() / conv3x3():
     rowstats / stats (with cs_hw, the rows per image of a linear) ask for the statistics outputs, ln for the LayerNorm
     fold, c2 / c3 are the folded shortcut's channels, halo / upsample / gn select the halo convolution (mode 0 with halo:
-    its 1x1 form; m = n_img * h * w)."""
+    its 1x1 form; m = n_img * h * w); bf16 plans the bf16 call (b200sd_gemm_bf16)."""
     a = GemmArgs()
     a.mode, a.m, a.n, a.c0, a.c1, a.n_img, a.h, a.w, a.stride = mode, m, n, c0, c1, n_img, h, w, stride
     a.geglu, a.bias_rows, a.split_k, a.block_n = int(geglu), bias_rows, split_k, block_n
@@ -228,7 +254,8 @@ def describe_plan(mode, m=0, n=0, c0=0, c1=0, n_img=0, h=0, w=0, stride=1, geglu
     if stats or rowstats or ln or gn:
         a.split_k = 1  # as linear() / conv3x3() ask for the fused outputs
     buf = C.create_string_buffer(512)
-    _check(load().b200sd_gemm_describe_plan(C.byref(a), buf, 512), "b200sd_gemm_describe_plan")
+    name = "b200sd_gemm_describe_plan" + ("_bf16" if bf16 else "")
+    _check(getattr(load(), name)(C.byref(a), buf, 512), name)
     return buf.value.decode()
 
 
@@ -272,16 +299,17 @@ def pack_tiled(w2d, c0, c1, taps, bn, chunk_major=False, extra=(0, 0)):
     return out.contiguous()
 
 
-def plan_ex(args):
+def plan_ex(args, bf16=False):
     """(block_n, splits, kb_total, n_tiles, stat slots per image, staged, stages, m_tiles) of a call."""
     plan = (C.c_int32 * 8)()
-    _check(load().b200sd_gemm_plan_ex(C.byref(args), plan), "b200sd_gemm_plan_ex")
+    name = "b200sd_gemm_plan_ex" + ("_bf16" if bf16 else "")
+    _check(getattr(load(), name)(C.byref(args), plan), name)
     return tuple(int(v) for v in plan)
 
 
 def _maybe_tile_weights(args, wgt, taps):
     """Static weight operands are re-laid out once per (weight, block_n) and cached."""
-    bn = plan_ex(args)[0]
+    bn = plan_ex(args, bf16=wgt.dtype == torch.bfloat16)[0]
     key = (wgt.data_ptr(), bn, args.c0, args.c1, taps, bool(args.halo), args.c2, args.c3)
     hit = _tiled_cache.get(key)
     packed = None
@@ -306,6 +334,15 @@ def gemm_workspace_bytes(args) -> int:
 
 def run_gemm(args):
     _check(load().b200sd_gemm(C.byref(args), _stream()), "b200sd_gemm")
+
+
+def run_gemm_bf16(args):
+    _check(load().b200sd_gemm_bf16(C.byref(args), _stream()), "b200sd_gemm_bf16")
+
+
+def _check_out(out, dt, what):
+    if out is not None and out.dtype not in (dt, torch.float32):
+        raise B200SDError(f"{what}: {out.dtype} output in a {dt} call (fp32 or the input's type)")
 
 
 _ws_cache = {}
@@ -389,19 +426,22 @@ def _fused_args(args, x_dev, *, n_img, cout, gn=None, stats=None, cs_hw=0, ln=No
     return keep
 
 
-def linear(x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=torch.float16, split_k=0,
+def linear(x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=None, split_k=0,
            block_n=0, bias_rows=0, bias_stride=0, out=None, static_w=False, act=0, ln=None, stats=None, cs_hw=0,
            rowstats=None):
     """out[M, N] = epilogue([x | x1] @ wgt^T).  x [M, C0] fp16, wgt [N, C0(+C1)] fp16, bias fp32 [N].
+    x bf16 runs the bf16 kernels: then wgt, x1, residual and a 16-bit output are bf16 too (out_dtype None: x's type).
     static_w: `wgt` is a model weight (constant address/content) and may be re-tiled + cached.
     ln: LayerNorm of x folded into this GEMM (wgt = gamma (.) W, bias = W beta + b; dict(stat, parts, wg, eps));
     stats / rowstats: dicts that receive the per-channel / per-row sums of the output (see _fused_args)."""
-    _req(x, torch.float16, "linear x")
-    _req(wgt, torch.float16, "linear wgt")
+    dt = _act_dtype(x, "linear x")
+    _req(wgt, dt, "linear wgt")
+    _same16(dt, x1, residual, "linear x1 / residual")
     m, n = x.shape[0], wgt.shape[0]
     n_out = n // 2 if geglu else n
     if out is None:
-        out = torch.empty(m, n_out, dtype=out_dtype, device=x.device)
+        out = torch.empty(m, n_out, dtype=out_dtype or dt, device=x.device)
+    _check_out(out, dt, "linear out")
     args = gemm_args(0, x, wgt, out, a1=x1, bias=bias, residual=residual, m=m, n=n, geglu=geglu,
                      bias_rows=bias_rows, bias_stride=bias_stride, split_k=split_k, block_n=block_n, act=act)
     if ln is not None or stats is not None or rowstats is not None:
@@ -410,16 +450,20 @@ def linear(x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=
                             rowstats=rowstats, m=m)
     if static_w and TILED_WEIGHTS:
         _maybe_tile_weights(args, wgt, 1)
-    need = gemm_workspace_bytes(args)
+    bf16 = dt == torch.bfloat16
+    need = 0 if bf16 else gemm_workspace_bytes(args)  # bf16 never splits K
     if need:
         ws = _workspace(need, x.device)
         args.workspace = ws.data_ptr()
         args.workspace_bytes = ws.numel() * 4
-    run_gemm(args)
+    if bf16:
+        run_gemm_bf16(args)
+    else:
+        run_gemm(args)
     return out
 
 
-def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=torch.float16, split_k=0,
+def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=None, split_k=0,
             block_n=0, bias_rows=0, bias_stride=0, out=None, act=0, static_w=True, pad_after_only=False,
             halo=False, gn=None, upsample=False, stats=None, rowstats=None, taps=9, shortcut=None):
     """3x3 pad-1 convolution.  x NHWC fp16 [N, H, W, C0]; wgt [Cout, 9*(C0+C1)] fp16 (OHWI);
@@ -429,16 +473,20 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=to
     receives 'chan', the per-channel (sum, sum of squares) of the output for the consumer's GroupNorm; taps=1 with
     halo: a 1x1 convolution (wgt [Cout, C0+C1]) that shares the halo kernel's GroupNorm operand path.
     shortcut = (s0, s1 or None): the ResNet shortcut folded in -- wgt is [Cout, 9*(C0+C1) + Cs0 + Cs1] (the 1x1
-    shortcut matrix appended along K), bias the sum of both biases, s0 / s1 NHWC fp16 at the output resolution."""
-    _req(x, torch.float16, "conv3x3 x")
-    _req(wgt, torch.float16, "conv3x3 wgt")
+    shortcut matrix appended along K), bias the sum of both biases, s0 / s1 NHWC fp16 at the output resolution.
+    x bf16 runs the bf16 kernels (no halo / gn / upsample / stats / shortcut): wgt, x1, residual and a 16-bit output
+    are bf16 too (out_dtype None: x's type)."""
+    dt = _act_dtype(x, "conv3x3 x")
+    _req(wgt, dt, "conv3x3 wgt")
+    _same16(dt, x1, residual, "conv3x3 x1 / residual")
     nimg, h, w, _ = x.shape
     if upsample:
         h, w = 2 * h, 2 * w
     cout = wgt.shape[0]
     ho, wo = h // stride, w // stride
     if out is None:
-        out = torch.empty(nimg, ho, wo, cout, dtype=out_dtype, device=x.device)
+        out = torch.empty(nimg, ho, wo, cout, dtype=out_dtype or dt, device=x.device)
+    _check_out(out, dt, "conv3x3 out")
     if (gn is not None or upsample or taps == 1) and not halo:
         raise B200SDError("conv3x3: gn / upsample / taps=1 need halo=True")
     args = gemm_args(1 if taps == 9 else 0, x, wgt, out, a1=x1, bias=bias, residual=residual, n=cout, n_img=nimg, h=h, w=w,
@@ -449,10 +497,10 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=to
         s0, s1 = shortcut
         if stride != 1 or taps != 9 or halo or not (static_w and TILED_WEIGHTS):
             raise B200SDError("conv3x3: a folded shortcut needs the stride-1 9-tap kernel with static pre-tiled weights")
-        _req(s0, torch.float16, "conv3x3 shortcut source")
+        _req(s0, dt, "conv3x3 shortcut source")
         args.a2, args.c2 = s0.data_ptr(), s0.shape[-1]
         if s1 is not None:
-            _req(s1, torch.float16, "conv3x3 shortcut source 1")
+            _req(s1, dt, "conv3x3 shortcut source 1")
             args.a3, args.c3 = s1.data_ptr(), s1.shape[-1]
     _keep = None
     if gn is not None or stats is not None or rowstats is not None:
@@ -463,12 +511,16 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=to
         raise B200SDError("conv3x3: the halo kernel needs static pre-tiled weights")
     if static_w and TILED_WEIGHTS:
         _maybe_tile_weights(args, wgt, taps)
-    need = gemm_workspace_bytes(args)
+    bf16 = dt == torch.bfloat16
+    need = 0 if bf16 else gemm_workspace_bytes(args)  # bf16 never splits K
     if need:
         ws = _workspace(need, x.device)
         args.workspace = ws.data_ptr()
         args.workspace_bytes = ws.numel() * 4
-    run_gemm(args)
+    if bf16:
+        run_gemm_bf16(args)
+    else:
+        run_gemm(args)
     return out
 
 
@@ -492,17 +544,19 @@ def timestep_embedding(t, dim, flip_sin_to_cos=True, freq_shift=0.0):
 
 
 def group_norm(x, gamma, beta, groups, eps, silu=False, x1=None, out=None):
-    """x NHWC fp16 [N, H, W, C0] (optionally ++ x1 [N, H, W, C1]) -> normalised [N, H, W, C0+C1]."""
-    _req(x, torch.float16, "group_norm x")
+    """x NHWC fp16 or bf16 [N, H, W, C0] (optionally ++ x1 [N, H, W, C1], same type) -> normalised [N, H, W, C0+C1]
+    in x's type (fp32 statistics either way)."""
+    dt = _act_dtype(x, "group_norm x")
+    _same16(dt, x1, out, "group_norm x1 / out")
     nimg, h, w, c0 = x.shape
     c1 = 0 if x1 is None else x1.shape[-1]
     if out is None:
-        out = torch.empty(nimg, h, w, c0 + c1, dtype=torch.float16, device=x.device)
+        out = torch.empty(nimg, h, w, c0 + c1, dtype=dt, device=x.device)
     need = int(load().b200sd_group_norm_workspace_bytes(nimg, h * w, c0 + c1, groups))
     ws = _workspace(need, x.device)
-    _check(load().b200sd_group_norm(_ptr(x), _ptr(x1), c0, c1, nimg, h * w, groups, float(eps), _ptr(gamma),
-                                    _ptr(beta), int(silu), _ptr(out), _ptr(ws), ws.numel() * 4, _stream()),
-           "b200sd_group_norm")
+    name = "b200sd_group_norm" + _sfx(dt)
+    _check(getattr(load(), name)(_ptr(x), _ptr(x1), c0, c1, nimg, h * w, groups, float(eps), _ptr(gamma),
+                                 _ptr(beta), int(silu), _ptr(out), _ptr(ws), ws.numel() * 4, _stream()), name)
     return out
 
 
@@ -575,17 +629,23 @@ def reserve_attention_workspace(device, d):
     return _attention_workspace(torch.device(device), d)
 
 
-def nchw_to_nhwc(x, c_pad=None, out=None):
+def nchw_to_nhwc(x, c_pad=None, out=None, out_dtype=torch.float16):
+    """NCHW fp16 / fp32 -> NHWC out_dtype (fp16 or bf16) with the channels zero padded to c_pad; a given `out`
+    decides the type (as in softmax_rows)."""
     n, c, h, w = x.shape
     c_pad = c if c_pad is None else c_pad
     if x.dtype not in (torch.float16, torch.float32) or not x.is_contiguous():
         raise B200SDError("nchw_to_nhwc: expected contiguous fp16/fp32")
+    if out is not None:
+        out_dtype = out.dtype
+    if out_dtype not in ACT_DTYPES:
+        raise B200SDError(f"nchw_to_nhwc: out_dtype must be fp16 or bf16, got {out_dtype}")
     if out is None:
-        out = torch.empty(n, h, w, c_pad, dtype=torch.float16, device=x.device)
-    elif out.dtype != torch.float16 or not out.is_contiguous() or tuple(out.shape) != (n, h, w, c_pad):
+        out = torch.empty(n, h, w, c_pad, dtype=out_dtype, device=x.device)
+    elif out.dtype != out_dtype or not out.is_contiguous() or tuple(out.shape) != (n, h, w, c_pad):
         raise B200SDError("nchw_to_nhwc: bad output buffer")
-    _check(load().b200sd_nchw_to_nhwc(_ptr(x), int(x.dtype == torch.float32), _ptr(out), n, c, h, w, c_pad,
-                                      _stream()), "b200sd_nchw_to_nhwc")
+    name = "b200sd_nchw_to_nhwc" + _sfx(out_dtype)
+    _check(getattr(load(), name)(_ptr(x), int(x.dtype == torch.float32), _ptr(out), n, c, h, w, c_pad, _stream()), name)
     return out
 
 
@@ -600,10 +660,12 @@ def nhwc_to_nchw_f32(x, c=None, out=None):
 
 
 def upsample2x(x, out=None):
-    _req(x, torch.float16, "upsample2x x")
+    """Nearest x2 upsample of an NHWC fp16 or bf16 tensor (a byte copy: one kernel for both)."""
+    dt = _act_dtype(x, "upsample2x x")
+    _same16(dt, out, None, "upsample2x out")
     n, h, w, c = x.shape
     if out is None:
-        out = torch.empty(n, 2 * h, 2 * w, c, dtype=torch.float16, device=x.device)
+        out = torch.empty(n, 2 * h, 2 * w, c, dtype=dt, device=x.device)
     _check(load().b200sd_upsample2x(_ptr(x), _ptr(out), n, h, w, c, _stream()), "b200sd_upsample2x")
     return out
 
@@ -682,20 +744,29 @@ def image_postprocess(x, c=3, want_u8=False):
     return (of, ou) if want_u8 else of
 
 
-def softmax_rows(scores, scale, out=None):
+def softmax_rows(scores, scale, out=None, out_dtype=torch.float16):
+    """fp32 scores [rows, cols] -> probabilities in out_dtype (fp16 or bf16: the type of the P V GEMM)."""
     _req(scores, torch.float32, "softmax_rows scores")
     rows, cols = scores.shape
+    if out is not None:
+        out_dtype = out.dtype
+    if out_dtype not in ACT_DTYPES:
+        raise B200SDError(f"softmax_rows: out_dtype must be fp16 or bf16, got {out_dtype}")
     if out is None:
-        out = torch.empty(rows, cols, dtype=torch.float16, device=scores.device)
-    _check(load().b200sd_softmax_rows(_ptr(scores), _ptr(out), rows, cols, float(scale), _stream()),
-           "b200sd_softmax_rows")
+        out = torch.empty(rows, cols, dtype=out_dtype, device=scores.device)
+    name = "b200sd_softmax_rows" + _sfx(out_dtype)
+    _check(getattr(load(), name)(_ptr(scores), _ptr(out), rows, cols, float(scale), _stream()), name)
     return out
 
 
-def latent_prep(z, w, b, inv_scale, c_pad=8):
+def latent_prep(z, w, b, inv_scale, c_pad=8, out_dtype=torch.float16):
+    """fp32 NCHW latents -> post_quant_conv(z * inv_scale) as NHWC out_dtype (fp16 or bf16), c_pad channels."""
     _req(z, torch.float32, "latent_prep z")
+    if out_dtype not in ACT_DTYPES:
+        raise B200SDError(f"latent_prep: out_dtype must be fp16 or bf16, got {out_dtype}")
     n, c, h, wd = z.shape
-    out = torch.empty(n, h, wd, c_pad, dtype=torch.float16, device=z.device)
-    _check(load().b200sd_latent_prep(_ptr(z), _ptr(w), _ptr(b), float(inv_scale), _ptr(out), n, c, h, wd, c_pad,
-                                     _stream()), "b200sd_latent_prep")
+    out = torch.empty(n, h, wd, c_pad, dtype=out_dtype, device=z.device)
+    name = "b200sd_latent_prep" + _sfx(out_dtype)
+    _check(getattr(load(), name)(_ptr(z), _ptr(w), _ptr(b), float(inv_scale), _ptr(out), n, c, h, wd, c_pad, _stream()),
+           name)
     return out

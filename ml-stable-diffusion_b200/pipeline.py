@@ -30,6 +30,16 @@ from .model import UNetModel
 from .vae import VAEDecoderModel
 
 
+def vae_dtype(unet_cfg: dict, vae_cfg: dict):
+    """The VAE's activation type for a checkpoint: bf16 iff the UNet is SDXL's (``addition_embed_type ==
+    "text_time"``) and the VAE's config sets ``"force_upcast": true`` -- the stock SDXL VAE, whose decoder activations
+    exceed fp16's range (diffusers upcasts exactly these VAEs in its SDXL pipeline; the reference converts the XL VAE
+    in FLOAT32 unless a custom VAE is given).  A missing key counts as false, so the fp16-fix VAE and every SD 1.x /
+    2.x directory keep fp16.  The checkpoint decides; there is no switch."""
+    xl = unet_cfg.get("addition_embed_type") == "text_time"
+    return torch.bfloat16 if xl and vae_cfg.get("force_upcast") is True else torch.float16
+
+
 @dataclasses.dataclass
 class StableDiffusionPipelineOutput:
     images: Union[List, np.ndarray]
@@ -189,13 +199,14 @@ class B200StableDiffusionPipeline:
         unet = UNetModel(ucfg, K.load_component(model_dir, "unet", ucfg), batch=2 * images_per_call, height=h, width=w,
                          device=device)
         vsd = K.read_state_dict(os.path.join(model_dir, "vae"))
+        vdtype = vae_dtype(ucfg, vcfg)
         vae = VAEDecoderModel(vcfg, K.check_state_dict("vae_decoder", vcfg, vsd), batch=images_per_call, height=h,
-                              width=w, device=device)
+                              width=w, device=device, dtype=vdtype)
         venc = None
         if with_vae_encoder:
             from .vae import VAEEncoderModel
             venc = VAEEncoderModel(vcfg, K.check_state_dict("vae_encoder", vcfg, vsd), batch=images_per_call,
-                                   height=h * f, width=w * f, device=device)
+                                   height=h * f, width=w * f, device=device, dtype=vdtype)
 
         def text_pair(enc_dir, tok_dir):
             if not os.path.isdir(os.path.join(model_dir, enc_dir)):

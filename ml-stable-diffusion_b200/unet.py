@@ -51,12 +51,17 @@ def _w2d(sd, key):
 
 
 class _Packer:
-    def __init__(self, sd, device):
+    """Packs a state dict's weights for the kernels: GEMM / convolution weights in `dtype` (fp16; bf16 for the VAEs
+    whose activations overflow fp16), biases and norm parameters fp32."""
+
+    def __init__(self, sd, device, dtype=torch.float16):
         self.sd = sd
         self.dev = device
+        self.dtype = dtype
 
     def f16(self, t):
-        return t.detach().to(device=self.dev, dtype=torch.float16).contiguous()
+        """A 16-bit weight operand, in the packer's dtype."""
+        return t.detach().to(device=self.dev, dtype=self.dtype).contiguous()
 
     def f32(self, key):
         return self.sd[key].detach().to(device=self.dev, dtype=torch.float32).contiguous()

@@ -3,8 +3,15 @@
 Replaces the ``vae_decoder`` Core ML model the reference calls once per image
 (``pipeline.py:313-320``), whose graph is ``decoder(post_quant_conv(z))`` of diffusers'
 ``AutoencoderKL`` (``torch2coreml.py:584-594``; architecture restated in SURVEY.md Appendix B1).
-NHWC fp16 activations; the single-head d=512 mid-block attention runs as two tensor-core GEMMs
+NHWC 16-bit activations; the single-head d=512 mid-block attention runs as two tensor-core GEMMs
 around a row-softmax kernel (scores fp32), since the flash kernel is specialised for d=64.
+
+The activations are fp16 unless the engine is built with ``dtype=torch.bfloat16``.  bf16 has fp32's exponent
+range: it is for the VAEs whose checkpoint sets ``force_upcast`` (the stock SDXL VAE, whose decoder activations
+exceed fp16's 65504; diffusers upcasts that VAE to fp32, the reference converts it in FLOAT32).  Then the GEMM /
+convolution weights are bf16 and every kernel of the forward runs its bf16 instantiation: each op follows its
+input's dtype, and the three ops that read fp32 (latent_prep, nchw_to_nhwc, softmax_rows) write the engine's dtype.
+Biases, norm parameters, statistics and accumulators stay fp32 either way.
 """
 from __future__ import annotations
 
@@ -17,10 +24,13 @@ from .unet import _Packer, _w2d
 
 
 class VAEDecoderEngine:
-    def __init__(self, cfg: dict, state_dict: dict, device="cuda"):
+    def __init__(self, cfg: dict, state_dict: dict, device="cuda", dtype=torch.float16):
         L.load()
+        if dtype not in L.ACT_DTYPES:
+            raise ValueError(f"VAE dtype must be torch.float16 or torch.bfloat16, got {dtype}")
         self.cfg = dict(cfg)
         self.dev = torch.device(device)
+        self.dtype = dtype
         self.boc = list(cfg.get("block_out_channels", (128, 256, 512, 512)))
         self.lpb = cfg.get("layers_per_block", 2)
         self.latent_ch = cfg.get("latent_channels", 4)
@@ -30,7 +40,7 @@ class VAEDecoderEngine:
         self._pack(state_dict)
 
     def _pack(self, sd):
-        P = _Packer(sd, self.dev)
+        P = _Packer(sd, self.dev, self.dtype)
         w = {}
 
         def resnet(p):
@@ -87,7 +97,7 @@ class VAEDecoderEngine:
             # is added after P V instead (softmax rows sum to one, so P (V + 1 b^T) = P V + 1 b^T)
             vt = L.linear(a["v"], hn[rows])
             scores = L.linear(q[rows], k[rows], out_dtype=torch.float32)
-            prob = L.softmax_rows(scores, c ** -0.5)
+            prob = L.softmax_rows(scores, c ** -0.5, out_dtype=x.dtype)
             att = L.linear(prob, vt, a["vb"])
             L.linear(att, a["o"], a["ob"], xr[rows], out=out[rows], static_w=True)
         return out.reshape(n, h, wd, c)
@@ -96,7 +106,7 @@ class VAEDecoderEngine:
         """z: fp32 NCHW latents (unscaled, as the pipeline holds them).  Returns NHWC fp32 image
         in [-1, 1]-ish range (before the pipeline's clip)."""
         w = self.w
-        x = L.latent_prep(z, w["pq"]["w"], w["pq"]["b"], 1.0, c_pad=8)
+        x = L.latent_prep(z, w["pq"]["w"], w["pq"]["b"], 1.0, c_pad=8, out_dtype=self.dtype)
         x = L.conv3x3(x, w["conv_in"]["w"], w["conv_in"]["b"])
         x = self._resnet("decoder.mid_block.resnets.0", x)
         x = self._attention("decoder.mid_block.attentions.0", x)
@@ -114,10 +124,14 @@ class VAEDecoderEngine:
 
 class VAEDecoderModel(B200Model):
     """``vae_decoder(z) -> {"image": fp32 (B, 3, 8H, 8W)}`` (pipeline.py:313-316; z is already divided by the
-    scaling factor by the caller, exactly as in the reference)."""
+    scaling factor by the caller, exactly as in the reference).  dtype=torch.bfloat16 runs the bf16 engine and
+    declares z float32, as the reference declares the input of a VAE it converts in FLOAT32."""
 
-    def __init__(self, cfg, state_dict, batch=1, height=64, width=64, device="cuda", io_dtype=np.float16):
-        self.engine = VAEDecoderEngine(cfg, state_dict, device)
+    def __init__(self, cfg, state_dict, batch=1, height=64, width=64, device="cuda", io_dtype=np.float16,
+                 dtype=torch.float16):
+        self.engine = VAEDecoderEngine(cfg, state_dict, device, dtype=dtype)
+        if dtype == torch.bfloat16:
+            io_dtype = np.float32
         spec = {"z": {"shape": (batch, self.engine.latent_ch, height, width), "dtype": np.dtype(io_dtype)}}
         super().__init__(spec, device)
         self._z = torch.zeros(batch, self.engine.latent_ch, height, width, dtype=torch.float32, device=self.device)
@@ -145,7 +159,7 @@ class VAEEncoderEngine(VAEDecoderEngine):
     downsampling convolutions pad after the last row / column only (``pad_after_only``)."""
 
     def _pack(self, sd):
-        P = _Packer(sd, self.dev)
+        P = _Packer(sd, self.dev, self.dtype)
         w = {}
 
         def resnet(p):
@@ -187,7 +201,7 @@ class VAEEncoderEngine(VAEDecoderEngine):
     def forward(self, x):
         """x: fp32 / fp16 NCHW image in [-1, 1].  Returns NHWC fp32 moments [B, H/8, W/8, 2 * latent]."""
         w = self.w
-        h = L.conv3x3(L.nchw_to_nhwc(x, c_pad=8), w["conv_in"]["w"], w["conv_in"]["b"])
+        h = L.conv3x3(L.nchw_to_nhwc(x, c_pad=8, out_dtype=self.dtype), w["conv_in"]["w"], w["conv_in"]["b"])
         for i in range(len(self.boc)):
             for j in range(self.lpb):
                 h = self._resnet(f"encoder.down_blocks.{i}.resnets.{j}", h)
@@ -204,10 +218,14 @@ class VAEEncoderEngine(VAEDecoderEngine):
 
 class VAEEncoderModel(B200Model):
     """``vae_encoder(x) -> {"latent": fp32 (B, 2 * latent_channels, H/8, W/8)}`` (torch2coreml.py:751-756: the
-    moments; sampling and scaling happen in the caller, Encoder.swift)."""
+    moments; sampling and scaling happen in the caller, Encoder.swift).  dtype=torch.bfloat16 runs the bf16 engine
+    and declares x float32."""
 
-    def __init__(self, cfg, state_dict, batch=1, height=512, width=512, device="cuda", io_dtype=np.float16):
-        self.engine = VAEEncoderEngine(cfg, state_dict, device)
+    def __init__(self, cfg, state_dict, batch=1, height=512, width=512, device="cuda", io_dtype=np.float16,
+                 dtype=torch.float16):
+        self.engine = VAEEncoderEngine(cfg, state_dict, device, dtype=dtype)
+        if dtype == torch.bfloat16:
+            io_dtype = np.float32
         spec = {"x": {"shape": (batch, 3, height, width), "dtype": np.dtype(io_dtype)}}
         super().__init__(spec, device)
         self._x = torch.zeros(batch, 3, height, width, dtype=torch.float32, device=self.device)
