@@ -22,6 +22,13 @@ SD21_BASE_UNET = dict(
     flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=1,
 )
 
+# SD 2.0 / 2.1 768-v (stabilityai/stable-diffusion-2-1): the SD-2.1-base UNet trained at 768x768 (96x96 latents) as a
+# v-prediction model.  Its diffusers config also sets upcast_attention and use_linear_projection: the attention kernels
+# already accumulate QK^T and the softmax in fp32, which is what upcast_attention asks for, and the [out, in] weights of a
+# linear proj_in / proj_out are what the engine makes of a 1x1 convolution's anyway (checkpoint.check_state_dict accepts
+# either shape).
+SD21_UNET = dict(SD21_BASE_UNET, sample_size=96)
+
 # SD 1.4 / 1.5 (CompVis/stable-diffusion-v1-4, the reference's default model): SD-2.1-base with 8 heads in every block
 # (head dims 40 / 80 / 160) and the 768-wide CLIP ViT-L/14 text states; the reference constructor's defaults
 # (unet.py:826-828).  859,520,964 parameters.

@@ -125,17 +125,27 @@ class B200StableDiffusionPipeline:
     # ---------------------------------------------------------------- factory
     @classmethod
     def from_random_init(cls, model_version="sd21-base", images_per_call=1, device="cuda", seed=0,
-                         scheduler="DDIM", height=512, width=512, unet_cfg=None, vae_cfg=None, controlnet_cfgs=None,
-                         text_encoder_cfg=None, tokenizer=None, with_vae_encoder=False):
+                         scheduler="DDIM", height=None, width=None, unet_cfg=None, vae_cfg=None, controlnet_cfgs=None,
+                         text_encoder_cfg=None, tokenizer=None, with_vae_encoder=False, scheduler_kwargs=None):
         """Random-init weights of the named architecture (no checkpoints exist offline).  ``controlnet_cfgs``:
         list of ControlNet configs (seeded seed+2, seed+3, ...); switches the UNet to its control variant.
-        ``model_version``: "sd21-base", "sd15" (SD 1.4 / 1.5), "sdxl-base" or "tiny".
+        ``model_version``: "sd21-base", "sd21" (SD 2.0 / 2.1 768-v: 768x768 by default, v-prediction), "sd15"
+        (SD 1.4 / 1.5), "sdxl-base" or "tiny"; ``height`` / ``width`` default to 768 for "sd21" and 512 otherwise.
         ``text_encoder_cfg``: a CLIP text config (config.OPENCLIP_H_TEXT for SD-2.x, config.CLIP_L_TEXT for SD-1.x) -> the
         text encoder runs on the
         device (random-init, seed+100) instead of the synthetic embedding table; ``tokenizer``: e.g. a
-        ``tokenizer.BPETokenizer`` built from the checkpoint's vocab.json / merges.txt."""
-        unet_cfg = unet_cfg or {"sd21-base": C.SD21_BASE_UNET, "sd15": C.SD15_UNET, "sdxl-base": C.SDXL_BASE_UNET,
-                                "tiny": C.TINY_UNET}[model_version]
+        ``tokenizer.BPETokenizer`` built from the checkpoint's vocab.json / merges.txt.  ``scheduler_kwargs``: extra
+        scheduler arguments (e.g. ``{"prediction_type": "v_prediction"}``, the default for "sd21")."""
+        native = 768 if model_version == "sd21" else 512
+        height, width = height or native, width or native
+        scheduler_kwargs = dict(scheduler_kwargs or {})
+        if model_version == "sd21":
+            if scheduler not in S.PREDICTION_TYPE_SCHEDULERS:
+                raise ValueError(f"the sd21 (768-v) model is a v-prediction model; the {scheduler} scheduler runs "
+                                 f"epsilon prediction only (use one of {S.PREDICTION_TYPE_SCHEDULERS})")
+            scheduler_kwargs.setdefault("prediction_type", "v_prediction")
+        unet_cfg = unet_cfg or {"sd21-base": C.SD21_BASE_UNET, "sd21": C.SD21_UNET, "sd15": C.SD15_UNET,
+                                "sdxl-base": C.SDXL_BASE_UNET, "tiny": C.TINY_UNET}[model_version]
         vae_cfg = vae_cfg or (C.TINY_VAE if model_version == "tiny" else C.SD_VAE)
         if controlnet_cfgs:
             unet_cfg = dict(unet_cfg, support_controlnet=True)
@@ -167,7 +177,8 @@ class B200StableDiffusionPipeline:
             esd = C.random_state_dict(C.vae_encoder_param_shapes(vae_cfg), seed=seed + 50, dtype=torch.float16)
             venc = VAEEncoderModel(vae_cfg, esd, batch=images_per_call, height=height, width=width, device=device)
         return cls(unet, vae, scheduler=scheduler, xl=unet.engine.xl, controlnet=nets, text_encoder=enc,
-                   tokenizer=tokenizer, vae_encoder=venc, force_zeros_for_empty_prompt=unet.engine.xl)
+                   tokenizer=tokenizer, vae_encoder=venc, force_zeros_for_empty_prompt=unet.engine.xl,
+                   scheduler_kwargs=scheduler_kwargs)
 
     _SCHEDULER_CLASS = {"PNDMScheduler": "PNDM", "DDIMScheduler": "DDIM", "DPMSolverMultistepScheduler": "DPMSolverMultistep"}
 
@@ -244,6 +255,13 @@ class B200StableDiffusionPipeline:
                 raise ValueError(f"scheduler {name} of the checkpoint is not implemented; pass scheduler_override "
                                  f"(one of {sorted(S.SCHEDULER_MAP)})")
             sched = cls._SCHEDULER_CLASS[name]
+        if sched in S.PREDICTION_TYPE_SCHEDULERS and os.path.exists(sched_cfg):
+            # SD 2.0 / 2.1 768-v checkpoints are v-prediction models ("prediction_type": "v_prediction"); diffusers
+            # applies the key inside scheduler.step (pipeline.py:565-569), these schedulers take it in their plan
+            with open(sched_cfg) as fh:
+                pred = json.load(fh).get("prediction_type")
+            if pred is not None:
+                sched_kw = {"prediction_type": S.check_prediction_type(pred)}
         nets = None
         if controlnet_dirs:
             from .controlnet import ControlNetModel

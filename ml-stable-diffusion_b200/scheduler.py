@@ -13,6 +13,10 @@ scheduler only produces, per step, the scalars of
 plus which history slots to overwrite; ``b200sd_cfg_scheduler_step`` applies them on the device
 (one launch, also does classifier-free guidance and writes the next UNet input), so the denoising
 loop never synchronises with the host.  Coefficients are computed in float64 and rounded once.
+
+DDIM, DPM-Solver++ and PNDM also run v-prediction models (SD 2.0 / 2.1 768-v, ``prediction_type="v_prediction"``):
+diffusers 0.30.2 converts the model output v to x0 = alpha_t x - sigma_t v or eps = alpha_t v + sigma_t x inside
+``step``, which keeps every update linear in (x, v, history), so only the coefficients change.
 """
 from __future__ import annotations
 
@@ -112,12 +116,25 @@ class _Base:
         return np.float32(np.sqrt(a)) * original_sample + np.float32(np.sqrt(np.float32(1.0) - a)) * noise
 
 
-class DDIMScheduler(_Base):
-    """eta = 0, epsilon prediction, 'leading' spacing, steps_offset 1, set_alpha_to_one False."""
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+#: the scheduler classes that take ``prediction_type``
+PREDICTION_TYPE_SCHEDULERS = ("DDIM", "DPMSolverMultistep", "PNDM")
 
-    def __init__(self, num_inference_steps, steps_offset=1, **kw):
+
+def check_prediction_type(value):
+    if value not in PREDICTION_TYPES:
+        raise ValueError(f"prediction_type must be one of {PREDICTION_TYPES}, got {value!r}")
+    return value
+
+
+class DDIMScheduler(_Base):
+    """eta = 0, 'leading' spacing, steps_offset 1, set_alpha_to_one False.  ``prediction_type="v_prediction"``:
+    x0 = alpha_t x - sigma_t v and eps = sigma_t x + alpha_t v (diffusers 0.30.2 ``DDIMScheduler.step``)."""
+
+    def __init__(self, num_inference_steps, steps_offset=1, prediction_type="epsilon", **kw):
         super().__init__(num_inference_steps, **kw)
         self.steps_offset = steps_offset
+        self.prediction_type = check_prediction_type(prediction_type)
 
     def plan(self, start=0):
         ratio = self.n_train // self.n
@@ -127,18 +144,26 @@ class DDIMScheduler(_Base):
             tp = t - ratio
             a_t = self.abar[t]
             a_p = self.abar[tp] if tp >= 0 else self.abar[0]
-            x0_cx = 1.0 / math.sqrt(a_t)
-            x0_ce = -math.sqrt(1 - a_t) / math.sqrt(a_t)
-            cx = math.sqrt(a_p) * x0_cx
-            ce = math.sqrt(a_p) * x0_ce + math.sqrt(1 - a_p)
+            if self.prediction_type == "epsilon":
+                x0_cx = 1.0 / math.sqrt(a_t)
+                x0_ce = -math.sqrt(1 - a_t) / math.sqrt(a_t)
+                cx = math.sqrt(a_p) * x0_cx
+                ce = math.sqrt(a_p) * x0_ce + math.sqrt(1 - a_p)
+            else:  # x' = alpha_p x0 + sigma_p eps
+                al_t, sg_t, al_p, sg_p = math.sqrt(a_t), math.sqrt(1 - a_t), math.sqrt(a_p), math.sqrt(1 - a_p)
+                x0_cx, x0_ce = al_t, -sg_t
+                cx = al_p * al_t + sg_p * sg_t
+                ce = sg_p * al_t - al_p * sg_t
             out.append(StepPlan(t, cx, ce, [0.0] * 4, x0_cx, x0_ce, [0.0] * 4))
         return out
 
 
 class DPMSolverMultistepScheduler(_Base):
-    """DPM-Solver++(2M) midpoint, epsilon prediction, 'linspace' spacing; first step and (for < 15
+    """DPM-Solver++(2M) midpoint, 'linspace' spacing; first step and (for < 15
     steps) the last two steps are first order (DPMSolverMultistepScheduler.swift:216-244).
-    History ring: x0 of the previous step in slots 0/1.
+    History ring: x0 of the previous step in slots 0/1.  The solver works on x0 estimates, so
+    ``prediction_type="v_prediction"`` only changes how x0 is read from the model output: x0 = alpha_t x - sigma_t v
+    (diffusers 0.30.2 ``convert_model_output``).
 
     ``final_sigmas_type``: how the LAST step ends.  ``"sigma_min"``: at the first training timestep's (alpha, sigma),
     what the in-tree Swift scheduler does (``alpha_t[0] / sigma_t[0]``, DPMSolverMultistepScheduler.swift:214-222).
@@ -146,11 +171,12 @@ class DPMSolverMultistepScheduler(_Base):
     ``scheduler.step``): the final sigma is 0, the last step is always first order and lands exactly on the
     denoised estimate x0."""
 
-    def __init__(self, num_inference_steps, final_sigmas_type="sigma_min", **kw):
+    def __init__(self, num_inference_steps, final_sigmas_type="sigma_min", prediction_type="epsilon", **kw):
         super().__init__(num_inference_steps, **kw)
         if final_sigmas_type not in ("sigma_min", "zero"):
             raise ValueError(f"final_sigmas_type must be 'sigma_min' or 'zero', got {final_sigmas_type!r}")
         self.final_sigmas_type = final_sigmas_type
+        self.prediction_type = check_prediction_type(prediction_type)
 
     def plan(self, start=0):
         n = self.n
@@ -167,8 +193,11 @@ class DPMSolverMultistepScheduler(_Base):
             lower_final = (i == n - 1) and n < 15
             lower_second = (i == n - 2) and n < 15
             first = lower_order_stepped < 1 or lower_final or lower_second
-            x0_cx = 1.0 / alpha[t]
-            x0_ce = -sigma[t] / alpha[t]
+            if self.prediction_type == "epsilon":
+                x0_cx = 1.0 / alpha[t]
+                x0_ce = -sigma[t] / alpha[t]
+            else:
+                x0_cx, x0_ce = alpha[t], -sigma[t]
             h = lam[p] - lam[t]
             A = -alpha[p] * (math.exp(-h) - 1.0)
             ch = [0.0] * 4
@@ -194,13 +223,18 @@ class DPMSolverMultistepScheduler(_Base):
 
 
 class PNDMScheduler(_Base):
-    """PLMS (skip_prk_steps) epsilon prediction (Scheduler.swift:137-344): num_steps + 1 UNet calls
+    """PLMS (skip_prk_steps) (Scheduler.swift:137-344): num_steps + 1 UNet calls
     (the second timestep is visited twice).  History ring: eps in slots 0..2, the saved first
-    sample (`currentSample`) in slot 3."""
+    sample (`currentSample`) in slot 3.
 
-    def __init__(self, num_inference_steps, steps_offset=1, **kw):
+    ``prediction_type="v_prediction"`` (diffusers 0.30.2 ``_get_prev_sample``): the ring keeps the RAW model outputs v,
+    and only their Adams-Bashforth combination e is converted, with the step's sample s and (shifted) timestep t:
+    eps = alpha_t e + sigma_t s.  Converting each v before combining would give another sampler after the first step."""
+
+    def __init__(self, num_inference_steps, steps_offset=1, prediction_type="epsilon", **kw):
         super().__init__(num_inference_steps, **kw)
         self.steps_offset = steps_offset
+        self.prediction_type = check_prediction_type(prediction_type)
 
     def _prev_coeffs(self, t, tp):
         a_t = self.abar[t]
@@ -250,18 +284,23 @@ class PNDMScheduler(_Base):
                 w_cur = 55 / 24
                 w_hist = {slot_back(2): -59 / 24, slot_back(3): 37 / 24, slot_back(4): -9 / 24}
                 use_saved = False
-            # x_prev = sc * sample + mc * e ; x0 = (sample - sigma_t e) / alpha_t ; e = w_cur eps + sum w h
+            # x_prev = sc * sample + mc * eps' ; x0 = (sample - sigma_t eps') / alpha_t ; e = w_cur out + sum w h ;
+            # eps' = e (epsilon) or alpha_t e + sigma_t sample (v): x_prev = s_x sample + s_e e, x0 = x0_x sample + x0_e e
             a_t, s_t = alpha[t], sigma[t]
-            cx = 0.0 if use_saved else sc
-            x0_cx = 0.0 if use_saved else 1.0 / a_t
+            if self.prediction_type == "epsilon":
+                s_x, s_e, x0_x, x0_e = sc, mc, 1.0 / a_t, -s_t / a_t
+            else:
+                s_x, s_e, x0_x, x0_e = sc + mc * s_t, mc * a_t, a_t, -s_t
+            cx = 0.0 if use_saved else s_x
+            x0_cx = 0.0 if use_saved else x0_x
             if use_saved:
-                ch[3] += sc
-                x0_ch[3] += 1.0 / a_t
-            ce = mc * w_cur
-            x0_ce = -s_t / a_t * w_cur
+                ch[3] += s_x
+                x0_ch[3] += x0_x
+            ce = s_e * w_cur
+            x0_ce = x0_e * w_cur
             for s, wv in w_hist.items():
-                ch[s] += mc * wv
-                x0_ch[s] += -s_t / a_t * wv
+                ch[s] += s_e * wv
+                x0_ch[s] += x0_e * wv
             n_hist = 4 if (use_saved or w_hist) else 0
             out.append(StepPlan(t_unet, cx, ce, ch, x0_cx, x0_ce, x0_ch, n_hist=n_hist, push_eps_slot=push_eps,
                                 push_x_slot=push_x))

@@ -1,10 +1,11 @@
 """Iter/s of the device denoising loop for one model, with the attention kernels' share of a step.
 
-    python tools/model_bench.py --model sd15|sd21-base [--reps 3]
+    python tools/model_bench.py --model sd15|sd21-base|sd21 [--reps 3]
 
 The workload is bench.py's: random-init weights, txt2img 512x512 at UNet batch 2 (uncond, cond), 20 DDIM steps, CFG
 7.5, the 20 steps (with the per-prompt prologue) captured as one CUDA graph by bench.LoopBench and timed with
-bench.timed_replays.  The attention time is the same loop captured with only the attention class launching
+bench.timed_replays.  ``sd21`` (SD 2.0 / 2.1 768-v) runs the same UNet at 768x768 (96x96 latents) with 20 DDIM
+v-prediction steps.  The attention time is the same loop captured with only the attention class launching
 (classes=2).  Prints one JSON line: iter/s, ms per step, attention ms per step, card name, power limit and the median
 SM clock while the loop ran."""
 import argparse
@@ -32,11 +33,12 @@ def power_limit_w(index):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
-    ap.add_argument("--model", choices=("sd15", "sd21-base"), default="sd15")
+    ap.add_argument("--model", choices=("sd15", "sd21-base", "sd21"), default="sd15")
     ap.add_argument("--reps", type=int, default=3, help="replays of the 20-step graph per measurement")
     args = ap.parse_args()
 
     from b200sd import lib as L
+    from b200sd import scheduler as S
     from b200sd.pipeline import B200StableDiffusionPipeline
 
     dev = torch.device("cuda", 0)
@@ -47,9 +49,11 @@ def main():
     d_ctx = pipe.unet._ctx.shape[1]
     g = torch.Generator().manual_seed(93)
     pipe.unet._ctx.copy_(torch.cat([torch.zeros(1, d_ctx, 1, 77), torch.randn(1, d_ctx, 1, 77, generator=g)]).half())
-    lat0 = torch.randn(1, 4, 64, 64, generator=g).half().float().to(dev)
+    lat0 = torch.randn(1, 4, pipe.unet.h, pipe.unet.w, generator=g).half().float().to(dev)
     loop = bench.LoopBench(pipe, lat0)
     n = bench.N_STEPS_IMG
+    loop.plan = S.DDIMScheduler(n, **pipe.scheduler_kwargs).plan()
+    pred = pipe.scheduler_kwargs.get("prediction_type", "epsilon")
     full = loop.capture(n)
     attn = loop.capture(n, classes=2)
     sync = torch.cuda.synchronize
@@ -58,7 +62,8 @@ def main():
     ms = bench.timed_replays(full, args.reps, sync) / n
     ms_attn = bench.timed_replays(attn, args.reps, sync) / n
     clocks = sampler.stop()
-    print(json.dumps({"model": args.model, "workload": "txt2img 512x512, UNet batch 2, 20 DDIM steps, CFG 7.5, fp16",
+    workload = f"txt2img {pipe.height}x{pipe.width}, UNet batch 2, 20 DDIM steps ({pred}), CFG 7.5, fp16"
+    print(json.dumps({"model": args.model, "workload": workload,
                       "iter_per_s": round(1e3 / ms, 2), "ms_per_step": round(ms, 4),
                       "attention_ms_per_step": round(ms_attn, 4),
                       "launches_per_step": round(loop.launches_per_image / n, 1),
