@@ -299,6 +299,32 @@ int b200sd_cfg_scheduler_step_noised(const float* noise_pred, float* latents, fl
                                      const b200sd_step_coeffs* coeffs /* host */, float noise_scale,
                                      const uint32_t* philox_key /* device */, uint32_t philox_offset, void* stream);
 
+/* Inpainting (diffusers 0.30.2 StableDiffusionInpaintPipeline with a 4-channel UNet): after the update and the optional
+ * ancestral noise, the unmasked region is replaced by the original image noised to the next timestep,
+ *     x_prev = m * x_prev + (1 - m) * (a * x0_img[i] + b * z[i])
+ * before x_prev is written to `latents` and channels [0, c) of both halves of `unet_in` (channels [c, c_pad) are
+ * never written).  m: fp32 [n, h*w], the latent mask per pixel, shared by the channels (1 = repaint); x0_img, z: fp32
+ * NCHW [n, c, h, w], the encoded image and the initial noise.  (a, b) is diffusers' add_noise at the next timestep in
+ * the loop's state space (for the Euler / LMS samplers divided by sqrt(sigma^2 + 1)); the last step has a = 1,
+ * b = 0.  History pushes and `denoised` keep their pre-blend values.  The buffers are read from device memory, so a
+ * captured CUDA graph serves every mask, image and seed. */
+typedef struct {
+    const float* mask;          /* [n, h*w] */
+    const float* image_latents; /* [n, c, h, w] */
+    const float* noise;         /* [n, c, h, w] */
+    float a;
+    float b;
+} b200sd_blend_args;
+
+/* b200sd_cfg_scheduler_step_noised plus the blend; philox_key == NULL: no ancestral noise (noise_scale and
+ * philox_offset unused). */
+int b200sd_cfg_scheduler_step_blend(const float* noise_pred, float* latents, float* hist /* [4][numel] */,
+                                    float* denoised /* x0 out or NULL */, void* unet_in, int32_t c_pad,
+                                    int32_t n, int32_t c, int32_t h, int32_t w,
+                                    const b200sd_step_coeffs* coeffs /* host */, float noise_scale,
+                                    const uint32_t* philox_key /* device or NULL */, uint32_t philox_offset,
+                                    const b200sd_blend_args* blend /* host */, void* stream);
+
 /* VAE decoder input: out = post_quant_conv(z * inv_scale) as NHWC fp16 padded to c_pad channels
  * (pipeline.py:313-316 `z / 0.18215`; torch2coreml.py:590-594 post_quant_conv); z fp32 NCHW, c <= 8,
  * w fp32 [c, c], b fp32 [c]. */

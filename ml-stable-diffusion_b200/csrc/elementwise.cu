@@ -235,12 +235,15 @@ __device__ __forceinline__ float philox_normal(uint32_t key, uint32_t offset, ui
 
 // One thread per latent element (n*c*h*w, NCHW fp32).  See include/b200sd.h for the algebra.  kNoise (ancestral
 // samplers): x_prev += noise_scale * z with z = philox_normal(*philox_key, philox_offset, i); the kNoise = false
-// instantiation never reads the three trailing parameters.
-template <bool kNoise>
+// instantiation never reads noise_scale / philox_key / philox_offset.  kBlend (inpainting): after the update and the
+// noise, x_prev = m x_prev + (1 - m)(a x0_img + b z); history pushes and `denoised` keep their pre-blend values.  The
+// kBlend = false instantiations never read `blend` (appended last, so the other parameters keep their offsets).
+template <bool kNoise, bool kBlend>
 __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __restrict__ latents,
                                 float* __restrict__ hist, float* __restrict__ denoised, __half* __restrict__ unet_in,
                                 int c_pad, int n, int c, int hw, b200sd_step_coeffs k, float noise_scale,
-                                const uint32_t* __restrict__ philox_key, uint32_t philox_offset) {
+                                const uint32_t* __restrict__ philox_key, uint32_t philox_offset,
+                                b200sd_blend_args blend) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int numel = n * c * hw;
@@ -271,6 +274,12 @@ __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __r
     if (k.push_x0_slot >= 0) hist[static_cast<size_t>(k.push_x0_slot) * numel + i] = x0;
     if (k.push_x_slot >= 0) hist[static_cast<size_t>(k.push_x_slot) * numel + i] = x;
     if constexpr (kNoise) xp += noise_scale * philox_normal(*philox_key, philox_offset, static_cast<uint32_t>(i));
+    if constexpr (kBlend) {
+        // the latent mask is per pixel [n, h*w], shared by the channels
+        const float m = __ldg(blend.mask + (i / (hw * c)) * hw + i % hw);
+        const float keep = blend.a * __ldg(blend.image_latents + i) + blend.b * __ldg(blend.noise + i);
+        xp = m * xp + (1.f - m) * keep;
+    }
     if (denoised) denoised[i] = x0;
     latents[i] = xp;
     if (unet_in) {
@@ -492,9 +501,10 @@ extern "C" int b200sd_cfg_scheduler_step(const float* noise_pred, float* latents
                        (hist || (coeffs->push_eps_slot < 0 && coeffs->push_x0_slot < 0 && coeffs->push_x_slot < 0)),
                    "b200sd_cfg_scheduler_step: bad history ring slot");
     const int numel = n * c * h * w;
-    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<false>, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred, latents, hist, denoised,
+    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<false, false>, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred, latents, hist, denoised,
                                                              reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
-                                                             *coeffs, 0.f, static_cast<const uint32_t*>(nullptr), 0u));
+                                                             *coeffs, 0.f, static_cast<const uint32_t*>(nullptr), 0u,
+                                                             b200sd_blend_args{}));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;
@@ -513,9 +523,40 @@ extern "C" int b200sd_cfg_scheduler_step_noised(const float* noise_pred, float* 
                        (hist || (coeffs->push_eps_slot < 0 && coeffs->push_x0_slot < 0 && coeffs->push_x_slot < 0)),
                    "b200sd_cfg_scheduler_step_noised: bad history ring slot");
     const int numel = n * c * h * w;
-    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<true>, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred,
+    B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<true, false>, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred,
                                     latents, hist, denoised, reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
-                                    *coeffs, noise_scale, philox_key, philox_offset));
+                                    *coeffs, noise_scale, philox_key, philox_offset, b200sd_blend_args{}));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_cfg_scheduler_step_blend(const float* noise_pred, float* latents, float* hist, float* denoised,
+                                               void* unet_in, int32_t c_pad, int32_t n, int32_t c, int32_t h,
+                                               int32_t w, const b200sd_step_coeffs* coeffs, float noise_scale,
+                                               const uint32_t* philox_key, uint32_t philox_offset,
+                                               const b200sd_blend_args* blend, void* stream_) {
+    if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(noise_pred && latents && coeffs && blend, "b200sd_cfg_scheduler_step_blend: null pointer");
+    B200SD_REQUIRE(blend->mask && blend->image_latents && blend->noise,
+                   "b200sd_cfg_scheduler_step_blend: null blend buffer");
+    B200SD_REQUIRE(coeffs->n_hist >= 0 && coeffs->n_hist <= 4 && (coeffs->n_hist == 0 || hist),
+                   "b200sd_cfg_scheduler_step_blend: bad history arguments");
+    B200SD_REQUIRE(coeffs->push_eps_slot < 4 && coeffs->push_x0_slot < 4 && coeffs->push_x_slot < 4 &&
+                       (hist || (coeffs->push_eps_slot < 0 && coeffs->push_x0_slot < 0 && coeffs->push_x_slot < 0)),
+                   "b200sd_cfg_scheduler_step_blend: bad history ring slot");
+    B200SD_REQUIRE(!unet_in || c_pad >= c, "b200sd_cfg_scheduler_step_blend: c_pad < c");
+    const int numel = n * c * h * w;
+    const dim3 grid((numel + 255) / 256);
+    if (philox_key)
+        B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<true, true>, grid, dim3(256), 0, stream, noise_pred, latents,
+                                        hist, denoised, reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
+                                        *coeffs, noise_scale, philox_key, philox_offset, *blend));
+    else
+        B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<false, true>, grid, dim3(256), 0, stream, noise_pred, latents,
+                                        hist, denoised, reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
+                                        *coeffs, 0.f, static_cast<const uint32_t*>(nullptr), 0u, *blend));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;

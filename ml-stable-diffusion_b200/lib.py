@@ -49,6 +49,11 @@ class StepCoeffs(C.Structure):
     ]
 
 
+class BlendArgs(C.Structure):
+    _fields_ = [("mask", C.c_void_p), ("image_latents", C.c_void_p), ("noise", C.c_void_p), ("a", C.c_float),
+                ("b", C.c_float)]
+
+
 _SIGNATURES = {
     "b200sd_last_error": (C.c_char_p, []),
     "b200sd_version": (C.c_int, []),
@@ -110,7 +115,11 @@ _SIGNATURES = {
                                                    C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                    C.POINTER(StepCoeffs), C.c_float, C.c_void_p, C.c_uint32,
                                                    C.c_void_p]),
-    "b200sd_image_postprocess": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+    "b200sd_cfg_scheduler_step_blend": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                  C.POINTER(StepCoeffs), C.c_float, C.c_void_p, C.c_uint32,
+                                                  C.POINTER(BlendArgs), C.c_void_p]),
+    "b200sd_image_postprocess":(C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
 }
 # bf16 twins (include/b200sd.h): same signatures, every fp16 pointer is bf16
@@ -732,6 +741,33 @@ def cfg_scheduler_step_noised(noise_pred, latents, coeffs: StepCoeffs, noise_sca
                                                    _ptr(unet_in), c_pad, n, c, h, w, C.byref(coeffs), float(noise_scale),
                                                    _ptr(key), int(offset) & 0xFFFFFFFF, _stream()),
            "b200sd_cfg_scheduler_step_noised")
+    return latents
+
+
+def cfg_scheduler_step_blend(noise_pred, latents, coeffs: StepCoeffs, mask, image_latents, noise, a, b,
+                             noise_scale=0.0, key=None, offset=0, hist=None, denoised=None, unet_in=None):
+    """``cfg_scheduler_step`` (``_noised`` when ``key`` is given), then the inpainting blend
+    ``x' = m x' + (1 - m)(a image_latents + b noise)``: ``mask`` fp32 [n, h*w] (or [n, 1, h, w]), ``image_latents`` /
+    ``noise`` fp32 like ``latents``."""
+    _req(noise_pred, torch.float32, "cfg_scheduler_step_blend noise_pred")
+    _req(latents, torch.float32, "cfg_scheduler_step_blend latents")
+    n, c, h, w = latents.shape
+    _req(mask, torch.float32, "cfg_scheduler_step_blend mask")
+    if mask.numel() != n * h * w:
+        raise B200SDError(f"cfg_scheduler_step_blend: mask has {mask.numel()} elements, expected {n * h * w}")
+    for name, t in (("image_latents", image_latents), ("noise", noise)):
+        _req(t, torch.float32, f"cfg_scheduler_step_blend {name}")
+        if tuple(t.shape) != (n, c, h, w):
+            raise B200SDError(f"cfg_scheduler_step_blend: {name} has shape {tuple(t.shape)}, expected {(n, c, h, w)}")
+    if key is not None and not (key.is_cuda and key.numel() == 1 and key.element_size() == 4):
+        raise B200SDError("cfg_scheduler_step_blend: key must be a one-element 4-byte CUDA tensor")
+    c_pad = 0 if unet_in is None else unet_in.shape[-1]
+    args = BlendArgs(_ptr(mask), _ptr(image_latents), _ptr(noise), float(a), float(b))
+    _check(load().b200sd_cfg_scheduler_step_blend(_ptr(noise_pred), _ptr(latents), _ptr(hist), _ptr(denoised),
+                                                  _ptr(unet_in), c_pad, n, c, h, w, C.byref(coeffs),
+                                                  float(noise_scale), _ptr(key), int(offset) & 0xFFFFFFFF,
+                                                  C.byref(args), _stream()),
+           "b200sd_cfg_scheduler_step_blend")
     return latents
 
 

@@ -40,6 +40,50 @@ def vae_dtype(unet_cfg: dict, vae_cfg: dict):
     return torch.bfloat16 if xl and vae_cfg.get("force_upcast") is True else torch.float16
 
 
+#: the schedulers whose truncated schedule (inpainting at strength < 1) diffusers 0.30.2 runs as ``plan(start)``
+INPAINT_STRENGTH_SCHEDULERS = ("DDIM", "DPMSolverMultistep")
+
+
+def prepare_mask_and_masked_image(image, mask):
+    """diffusers 0.30.2 ``StableDiffusionInpaintPipeline``'s mask processing (``VaeImageProcessor(do_binarize=True,
+    do_convert_grayscale=True)``): ``image`` (B, 3, H, W) in [-1, 1]; ``mask`` (B | 1, 1, H, W) or (H, W) in [0, 1],
+    1 = repaint.  The mask is binarised at 0.5 (0.5 repaints) and broadcast to B; the masked image is
+    ``image * (mask < 0.5)``.  -> (mask (B, 1, H, W) float32 in {0, 1}, masked image (B, 3, H, W) float32)."""
+    image = np.asarray(image, dtype=np.float32)
+    if image.ndim != 4 or image.shape[1] != 3:
+        raise ValueError(f"starting_image must be (B, 3, H, W), got shape {image.shape}")
+    m = np.asarray(mask, dtype=np.float32)
+    if m.ndim == 2:
+        m = m[None, None]
+    if m.ndim != 4 or m.shape[1] != 1:
+        raise ValueError(f"mask_image must be (B, 1, H, W), (1, 1, H, W) or (H, W), got shape {np.shape(mask)}")
+    if m.shape[2:] != image.shape[2:]:
+        raise ValueError(f"mask_image is {m.shape[2]}x{m.shape[3]}, the starting image {image.shape[2]}x{image.shape[3]}")
+    if m.shape[0] not in (1, image.shape[0]):
+        raise ValueError(f"mask_image has batch {m.shape[0]}, the starting image {image.shape[0]}")
+    if not (np.isfinite(m).all() and m.min() >= 0.0 and m.max() <= 1.0):
+        raise ValueError("mask_image values must lie in [0, 1]")
+    m = np.broadcast_to((m >= 0.5).astype(np.float32), (image.shape[0], 1) + image.shape[2:])
+    return np.ascontiguousarray(m), image * (m < 0.5)
+
+
+def latent_mask(mask, factor=8):
+    """``F.interpolate(mask, size=(H // factor, W // factor))`` (nearest, the inpaint pipeline's default): latent
+    pixel (i, j) takes image pixel (factor i, factor j)."""
+    return np.ascontiguousarray(np.asarray(mask, dtype=np.float32)[:, :, ::factor, ::factor])
+
+
+@dataclasses.dataclass
+class InpaintInputs:
+    """One inpainting call's inputs to ``denoise`` (numpy or torch, float32): ``mask`` the latent mask (n, 1, h, w) in
+    {0, 1}, 1 = repaint; for a 4-channel UNet ``image_latents`` (the encoded image x0_img, x-space) and ``noise`` (the
+    initial noise z, unscaled), which the blend reads; for a 9-channel UNet ``masked_image_latents``."""
+    mask: object
+    image_latents: object = None
+    noise: object = None
+    masked_image_latents: object = None
+
+
 @dataclasses.dataclass
 class StableDiffusionPipelineOutput:
     images: Union[List, np.ndarray]
@@ -110,7 +154,9 @@ class B200StableDiffusionPipeline:
         self.height = unet.h * self.vae_scale_factor
         self.width = unet.w * self.vae_scale_factor
         self.images_per_call = unet.batch // 2
-        n, c, h, w = self.images_per_call, unet.in_channels, unet.h, unet.w
+        # the latents have the UNet's OUTPUT channels: an inpainting UNet reads 9 (latents, mask, masked image latents)
+        self.latent_channels = unet.engine.out_ch
+        n, c, h, w = self.images_per_call, self.latent_channels, unet.h, unet.w
         dev = self.device
         self._latents = torch.zeros(n, c, h, w, dtype=torch.float32, device=dev)
         self._hist = torch.zeros(4, n, c, h, w, dtype=torch.float32, device=dev)
@@ -121,6 +167,9 @@ class B200StableDiffusionPipeline:
         # seed) and the draw number of step 0 (part of the graph key: offsets are baked into the graph)
         self._noise_key = torch.zeros(1, dtype=torch.int32, device=dev)
         self._noise_base = 0
+        # inpainting: static device buffers (allocated on first use), filled before each loop so that one loop graph
+        # serves every mask, image and seed
+        self._inpaint_bufs = None
 
     # ---------------------------------------------------------------- factory
     @classmethod
@@ -431,14 +480,17 @@ class B200StableDiffusionPipeline:
                                                                     st.push_x0_slot, st.push_x_slot)
         return k
 
-    def _loop_on_static_buffers(self, plan, guidance_scale, ts_rows, use_controlnet=False, refiner_start_step=None):
+    def _loop_on_static_buffers(self, plan, guidance_scale, ts_rows, use_controlnet=False, refiner_start_step=None,
+                                inpaint=None, blend=None):
         """The whole N-step loop on static device buffers (no host-side tensor arguments): what the loop graph
         captures.  Prologue, once per prompt: cross-attention K/V of all blocks from the text states, the
         time-embedding biases of all ResNet blocks for ALL timesteps (`ts_rows`: each step's timestep repeated per
         batch row, a device tensor made outside the capture), the first UNet input.  Per step: the UNet launch
         sequence and ONE fused kernel for guidance + scheduler update, which also writes the next step's UNet
         input (fp16 NHWC, both CFG halves: pipeline.py:502 np.concatenate([latents] * 2)) -- no fill / copy /
-        layout kernels in between."""
+        layout kernels in between.  ``inpaint`` ("blend" / "unet9", see ``_inpaint_kind``): "blend" runs the step
+        kernel's blend with ``blend[i]`` = (a, b) of step i; "unet9" writes the five conditioning channels (mask,
+        masked image latents) into both halves of the first UNet input, which the step kernel never overwrites."""
         n = self.images_per_call
         rs = len(plan) if refiner_start_step is None else max(0, min(len(plan), refiner_start_step))
         # which UNet runs each step: the SDXL refiner takes over at refiner_start_step with its own conditioning
@@ -452,8 +504,12 @@ class B200StableDiffusionPipeline:
                 m.prepare_prompt()
                 tables[id(m)] = (m.time_table(ts_rows[lo * b: hi * b]), lo)
         first = models[0]
-        L.nchw_to_nhwc(self._latents, c_pad=first.engine.in_pad, out=first._x_nhwc[:n])
-        L.nchw_to_nhwc(self._latents, c_pad=first.engine.in_pad, out=first._x_nhwc[n:])
+        x_in = self._latents
+        if inpaint == "unet9":
+            x_in = self._inpaint_bufs["unet_in"]
+            x_in[:, :self.latent_channels].copy_(self._latents)
+        L.nchw_to_nhwc(x_in, c_pad=first.engine.in_pad, out=first._x_nhwc[:n])
+        L.nchw_to_nhwc(x_in, c_pad=first.engine.in_pad, out=first._x_nhwc[n:])
         if use_controlnet:
             self.prepare_controlnets(ts_rows)
         for i, st in enumerate(plan):
@@ -463,17 +519,66 @@ class B200StableDiffusionPipeline:
             k = self._coeffs(st, guidance_scale)
             k.noise_pred_nhwc = 1
             nxt = models[i + 1] if i + 1 < len(plan) else u
-            self._step(st, k, u._out_nhwc, unet_in=nxt._x_nhwc)
+            self._step(st, k, u._out_nhwc, unet_in=nxt._x_nhwc, blend=blend[i] if blend else None)
 
-    def _step(self, st, k, noise_pred, unet_in=None):
-        """One fused guidance + scheduler update of the loop state, with the step's noise when the plan has some."""
-        if st.noise_offset >= 0:
+    def _step(self, st, k, noise_pred, unet_in=None, blend=None):
+        """One fused guidance + scheduler update of the loop state, with the step's noise when the plan has some and
+        the inpainting blend with ``blend`` = (a, b) when given."""
+        if blend is not None:
+            b = self._inpaint_bufs
+            noised = st.noise_offset >= 0
+            L.cfg_scheduler_step_blend(noise_pred, self._latents, k, b["mask"], b["image_latents"], b["noise"],
+                                       blend[0], blend[1], st.noise_scale if noised else 0.0,
+                                       self._noise_key if noised else None,
+                                       self._noise_base + st.noise_offset if noised else 0, hist=self._hist,
+                                       denoised=self._denoised, unet_in=unet_in)
+        elif st.noise_offset >= 0:
             L.cfg_scheduler_step_noised(noise_pred, self._latents, k, st.noise_scale, self._noise_key,
                                         self._noise_base + st.noise_offset, hist=self._hist, denoised=self._denoised,
                                         unet_in=unet_in)
         else:
             L.cfg_scheduler_step(noise_pred, self._latents, k, hist=self._hist, denoised=self._denoised,
                                  unet_in=unet_in)
+
+    def _inpaint_kind(self, inpainting, start_step=0, controlnet=False, refiner=False):
+        """None (no inpainting), "blend" (a 4-channel UNet: the step kernel blends the noised image back in) or
+        "unet9" (a 9-channel inpainting UNet: mask and masked image latents are UNet input channels).  Raises a
+        ValueError naming any combination the inpainting loop does not support."""
+        cin = self.unet.in_channels
+        if not inpainting:
+            if cin == 9:
+                raise ValueError("the UNet is an inpainting UNet (in_channels=9): pass mask_image and starting_image")
+            return None
+        if cin not in (4, 9):
+            raise ValueError(f"inpainting runs UNets with in_channels 4 or 9, this one has in_channels={cin}")
+        if self.unet.engine.xl:
+            raise ValueError("inpainting is not supported for SDXL (text_time) UNets")
+        if refiner or self.unet_refiner is not None:
+            raise ValueError("inpainting is not supported with the SDXL refiner")
+        if controlnet or self.controlnet:
+            raise ValueError("inpainting is not supported with ControlNet")
+        if start_step and self.scheduler_name not in INPAINT_STRENGTH_SCHEDULERS:
+            raise ValueError(f"inpainting at strength < 1 is not supported for the {self.scheduler_name} scheduler "
+                             f"(only {INPAINT_STRENGTH_SCHEDULERS})")
+        return "unet9" if cin == 9 else "blend"
+
+    def _set_inpaint_buffers(self, kind, inp):
+        """Copy one call's mask and image latents into the static buffers the loop (graph) reads."""
+        n, c, h, w = self._latents.shape
+        if self._inpaint_bufs is None:
+            zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
+            self._inpaint_bufs = {"mask": zeros(n, 1, h, w), "image_latents": zeros(n, c, h, w),
+                                  "noise": zeros(n, c, h, w), "unet_in": zeros(n, self.unet.in_channels, h, w)}
+        b = self._inpaint_bufs
+        as_dev = lambda v, shape: torch.as_tensor(v, dtype=torch.float32).to(self.device).reshape(shape)  # noqa: E731
+        mask = as_dev(inp.mask, (n, 1, h, w))
+        b["mask"].copy_(mask)
+        if kind == "blend":
+            b["image_latents"].copy_(as_dev(inp.image_latents, (n, c, h, w)))
+            b["noise"].copy_(as_dev(inp.noise, (n, c, h, w)))
+        else:
+            b["unet_in"][:, c:c + 1].copy_(mask)
+            b["unet_in"][:, c + 1:].copy_(as_dev(inp.masked_image_latents, (n, self.unet.in_channels - c - 1, h, w)))
 
     def set_control_conditions(self, controlnet_cond):
         """Copy the conditioning images (each (2B, 3, H, W)) into the ControlNets' static input buffers."""
@@ -502,7 +607,8 @@ class B200StableDiffusionPipeline:
         return torch.tensor([float(st.timestep) for st in plan for _ in range(self.unet.batch)], dtype=torch.float32,
                             device=self.device)
 
-    def _loop_graph_for(self, key, plan, guidance_scale, use_controlnet=False, refiner_start_step=None):
+    def _loop_graph_for(self, key, plan, guidance_scale, use_controlnet=False, refiner_start_step=None, inpaint=None,
+                        blend=None):
         g = self._loop_graphs.get(key)
         if g is None:
             keep = self._latents.clone()
@@ -510,7 +616,8 @@ class B200StableDiffusionPipeline:
             s = torch.cuda.Stream(device=self.device)  # eager warm-up off the capture: workspaces, weight tiling
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._loop_on_static_buffers(plan[:1], guidance_scale, ts_rows[: self.unet.batch], use_controlnet)
+                self._loop_on_static_buffers(plan[:1], guidance_scale, ts_rows[: self.unet.batch], use_controlnet,
+                                             inpaint=inpaint, blend=blend[:1] if blend else None)
                 if refiner_start_step is not None and refiner_start_step < len(plan):  # warm the refiner's kernels too
                     self._loop_on_static_buffers(plan[-1:], guidance_scale, ts_rows[-self.unet.batch:], use_controlnet, 0)
             torch.cuda.current_stream().wait_stream(s)
@@ -518,7 +625,8 @@ class B200StableDiffusionPipeline:
             self._latents.copy_(keep)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._loop_on_static_buffers(plan, guidance_scale, ts_rows, use_controlnet, refiner_start_step)
+                self._loop_on_static_buffers(plan, guidance_scale, ts_rows, use_controlnet, refiner_start_step,
+                                             inpaint, blend)
             g._b200sd_keep = ts_rows
             self._latents.copy_(keep)  # capture does not execute, but keep the contract obvious
             if len(self._loop_graphs) >= 4:
@@ -528,7 +636,8 @@ class B200StableDiffusionPipeline:
 
     def denoise(self, text_embeddings, latents, num_inference_steps, guidance_scale, callback=None,
                 callback_steps=1, time_ids=None, text_embeds=None, return_denoised=False, record=None,
-                controlnet_cond=None, start_step=0, refiner=None, refiner_start=0.8, noise_key=None, noise_offset=0):
+                controlnet_cond=None, start_step=0, refiner=None, refiner_start=0.8, noise_key=None, noise_offset=0,
+                inpaint=None):
         """Runs the N-step loop (from ``start_step``: image-to-image) entirely on the device.  ``text_embeddings`` (2B, D, 1, S) and ``latents``
         (B, C, h, w) may be numpy (copied once, before the loop) or CUDA tensors.  ``record`` (a list) receives
         (timestep, noise_pred, latents_after_step) clones per step -- a debugging / testing aid.  Without
@@ -538,10 +647,19 @@ class B200StableDiffusionPipeline:
         x / sqrt(sigma^2 + 1), so their latents are divided once before the loop and multiplied back off the hot path.
         ``noise_key`` / ``noise_offset`` (ancestral samplers): step j adds the Philox normals of
         ``NvRandomSource(noise_key)``'s draw number ``noise_offset + j``; without a key one ``np.random.randint(2**32)``
-        is drawn."""
+        is drawn.
+        ``inpaint`` (``InpaintInputs``): the latent mask and image latents of an inpainting call (``__call__`` with
+        ``mask_image``); required for a 9-channel UNet.  They are copied into static buffers before the loop, so the
+        loop graph depends on the inpainting kind only, never on the mask or the images."""
         sched = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs)
         plan = list(sched.plan(start=start_step)) if start_step else list(sched.plan())
         n = self.images_per_call
+        kind = self._inpaint_kind(inpaint is not None, start_step, bool(controlnet_cond), refiner is not None)
+        blend = None
+        if kind is not None:
+            self._set_inpaint_buffers(kind, inpaint)
+            if kind == "blend":
+                blend = sched.blend_coeffs(start_step)
         self._ctx.copy_(torch.as_tensor(text_embeddings), non_blocking=True)
         self._latents.copy_(torch.as_tensor(latents), non_blocking=True)
         if sched.input_scale(0) != 1.0:
@@ -579,8 +697,8 @@ class B200StableDiffusionPipeline:
                 r._text_embeds.copy_(torch.as_tensor(refiner["text_embeds"]))
                 rstep = int(np.float32(len(plan)) * np.float32(refiner_start))  # Int(Float(timeSteps.count) * refinerStart)
             key = (self.scheduler_name, int(num_inference_steps), float(guidance_scale), int(start_step),
-                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base)
-            self._loop_graph_for(key, plan, guidance_scale, bool(controlnet_cond), rstep).replay()
+                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base, kind)
+            self._loop_graph_for(key, plan, guidance_scale, bool(controlnet_cond), rstep, kind, blend).replay()
             return self._denoised if return_denoised else self._latents
         if refiner is not None:
             raise ValueError("the refiner hand-off runs in the device loop only (no callback / record)")
@@ -588,7 +706,11 @@ class B200StableDiffusionPipeline:
         k = L.StepCoeffs()
         for i, st in enumerate(plan):
             self._t.fill_(float(st.timestep))
-            sample = torch.cat([self._latents, self._latents], 0)  # pipeline.py:502
+            x_in = self._latents
+            if kind == "unet9":  # cat([latents, mask, masked_image_latents], 1), the same conditioning every step
+                x_in = self._inpaint_bufs["unet_in"]
+                x_in[:, :self.latent_channels].copy_(self._latents)
+            sample = torch.cat([x_in, x_in], 0)  # pipeline.py:502
             residuals = None
             if controlnet_cond:  # pipeline.py:515-529
                 residuals = self.run_controlnet(sample, self._t, self._ctx, controlnet_cond)
@@ -596,7 +718,7 @@ class B200StableDiffusionPipeline:
             self._coeffs(st, guidance_scale, k)
             if record is not None:
                 eps_copy = noise_pred.clone()
-            self._step(st, k, noise_pred)
+            self._step(st, k, noise_pred, blend=blend[i] if blend else None)
             if record is not None:
                 record.append((st.timestep, eps_copy, x_space(i + 1).clone()))
             if callback is not None and i % callback_steps == 0:
@@ -617,11 +739,19 @@ class B200StableDiffusionPipeline:
                  return_dict=True, callback=None, callback_steps=1, controlnet_cond=None,
                  original_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
                  target_size: Optional[Tuple[int, int]] = None, unet_batch_one=False, prompt_embeds=None,
-                 starting_image=None, strength=0.5, seed=None, rng="numpy", refiner_start=0.8, aesthetic_score=6.0,
-                 negative_aesthetic_score=2.5, **kwargs):
-        """``starting_image`` ((B, 3, H, W) in [-1, 1], the vae_encoder input) + ``strength`` select the Swift
-        pipeline's image-to-image mode (StableDiffusionPipeline.swift:250-262, 361-378): the encoded image is noised
-        to timestep ``timeSteps[startStep]`` and only the remaining steps run."""
+                 starting_image=None, strength=None, seed=None, rng="numpy", refiner_start=0.8, aesthetic_score=6.0,
+                 negative_aesthetic_score=2.5, mask_image=None, **kwargs):
+        """``starting_image`` ((B, 3, H, W) in [-1, 1], the vae_encoder input) + ``strength`` (default 0.5) select the
+        Swift pipeline's image-to-image mode (StableDiffusionPipeline.swift:250-262, 361-378): the encoded image is
+        noised to timestep ``timeSteps[startStep]`` and only the remaining steps run.
+
+        ``mask_image`` ((B | 1, 1, H, W) or (H, W) in [0, 1], 1 = repaint) with ``starting_image`` inpaints, as diffusers
+        0.30.2's ``StableDiffusionInpaintPipeline`` (``strength`` default 1.0; < 1 for DDIM and DPM-Solver++ only, start
+        step ``get_timesteps``'s).  A 9-channel inpainting UNet reads cat([latents, mask, masked image latents]); a
+        4-channel UNet keeps the unmasked region by blending the noised image latents back in after every step, so
+        the unmasked latents end exactly on the image latents.  Draws from the global numpy stream, after the latent
+        noise: the encoder noise of the full image (4-channel UNet, or strength < 1), then that of the masked image
+        (9-channel UNet)."""
         self.check_inputs(prompt, height, width, callback_steps)
         height = height or self.height
         width = width or self.width
@@ -656,19 +786,55 @@ class B200StableDiffusionPipeline:
                 text_embeds = torch.as_tensor(xl_pooled, dtype=torch.float32, device=self.device)
             if text_embeds is None:
                 text_embeds = torch.zeros(2 * self.images_per_call, 1280, device=self.device)
-        if starting_image is not None and self.scheduler_name in S.SIGMA_SCHEDULERS:
+        sched = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs)
+        inpaint_kind, start_step = None, 0
+        if mask_image is not None or self.unet.in_channels == 9:
+            if mask_image is not None and starting_image is None:
+                raise ValueError("mask_image needs a starting_image (the image to inpaint)")
+            strength = 1.0 if strength is None else float(strength)
+            if not 0.0 < strength <= 1.0:
+                raise ValueError(f"inpainting strength must be in (0, 1], got {strength}")
+            start_step = sched.inpaint_start_step(strength)
+            if start_step >= num_inference_steps:
+                raise ValueError(f"strength {strength} leaves no denoising steps")
+            inpaint_kind = self._inpaint_kind(mask_image is not None, start_step, bool(controlnet_cond))
+            if self.vae_encoder is None:
+                raise ValueError("inpainting needs a vae_encoder (with_vae_encoder=True)")
+        elif starting_image is not None and self.scheduler_name in S.SIGMA_SCHEDULERS:
             raise ValueError(f"image-to-image is not implemented for the {self.scheduler_name} scheduler")
-        init_sigma = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs).init_noise_sigma
-        lat = self.prepare_latents(len(prompts), self.unet.in_channels, height, width, latents, seed=seed, rng=rng,
-                                   init_noise_sigma=init_sigma)
+        init_sigma = sched.init_noise_sigma
+        if inpaint_kind is None:
+            lat = self.prepare_latents(len(prompts), self.latent_channels, height, width, latents, seed=seed, rng=rng,
+                                       init_noise_sigma=init_sigma)
+        else:
+            # diffusers keeps the unscaled noise z: the blend and the strength < 1 start noise both read it
+            noise = self.prepare_latents(len(prompts), self.latent_channels, height, width, latents, seed=seed, rng=rng)
+            lat = noise * init_sigma
         # ancestral step noise: keyed by the seed, continuing the latents' Philox stream with the nvidia source; without
         # a seed, denoise() draws the key from the global numpy stream right after the latents
         noise_key, noise_offset = None, 0
         if seed is not None:
             noise_key = seed
             noise_offset = len(prompts) if rng in ("nvidia", "nvidiaRNG") else 0
-        start_step = 0
-        if starting_image is not None:
+        inpaint = None
+        if inpaint_kind is not None:
+            mask_img, masked = prepare_mask_and_masked_image(starting_image, mask_image)
+            enc_dtype = self.vae_encoder.expected_inputs["x"]["dtype"]
+            scaling = self.vae_decoder.engine.scaling
+            x0 = masked_lat = None
+            if inpaint_kind == "blend" or start_step:
+                enc_noise = np.random.randn(*lat.shape).astype(np.float32)
+                x0 = self.vae_encoder.encode(np.asarray(starting_image, dtype=enc_dtype), enc_noise,
+                                             scaling).numpy().astype(np.float32)
+            if inpaint_kind == "unet9":
+                enc_noise = np.random.randn(*lat.shape).astype(np.float32)
+                masked_lat = self.vae_encoder.encode(masked.astype(enc_dtype), enc_noise, scaling).numpy().astype(np.float32)
+            if start_step:
+                a, b = sched.noise_coeffs(start_step)  # add_noise(image_latents, noise, timesteps[t_start])
+                lat = np.float32(a) * x0 + np.float32(b) * noise
+            inpaint = InpaintInputs(latent_mask(mask_img, self.vae_scale_factor), x0, noise, masked_lat)
+        elif starting_image is not None:
+            strength = 0.5 if strength is None else strength
             if self.vae_encoder is None:
                 raise ValueError("a starting image was provided but the pipeline has no vae_encoder")
             sched = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs)
@@ -701,7 +867,7 @@ class B200StableDiffusionPipeline:
         final = self.denoise(text_embeddings, lat, num_inference_steps, guidance_scale, callback, callback_steps,
                              time_ids, text_embeds, controlnet_cond=controlnet_cond or None, start_step=start_step,
                              refiner=refiner, refiner_start=refiner_start, noise_key=noise_key,
-                             noise_offset=noise_offset)
+                             noise_offset=noise_offset, inpaint=inpaint)
         image = self.decode_latents(final).cpu().numpy()  # single device->host copy of the result
         has_nsfw = None  # the safety checker is out of scope (SURVEY section 2, row 19)
         if output_type == "pil":

@@ -82,6 +82,7 @@ class _Base:
         self.n = int(num_inference_steps)
         self.n_train = int(num_train_timesteps)
         self.abar = alphas_cumprod(beta_start, beta_end, num_train_timesteps, beta_schedule).astype(np.float64)
+        self._beta_args = (beta_start, beta_end, num_train_timesteps, beta_schedule)
 
     def scale_model_input(self, x, t):  # identity for DDIM / PNDM / DPM (pipeline.py:504)
         return x
@@ -114,6 +115,29 @@ class _Base:
         t = self.timesteps[self.start_step(strength)]
         a = np.float32(self.abar[t])
         return np.float32(np.sqrt(a)) * original_sample + np.float32(np.sqrt(np.float32(1.0) - a)) * noise
+
+    # ---- inpainting (diffusers 0.30.2 StableDiffusionInpaintPipeline) ----
+    def inpaint_start_step(self, strength: float) -> int:
+        """``get_timesteps``: n - min(int(n * strength), n) in float64 (the image-to-image rule, ``start_step``, rounds
+        in float32 and can differ by one, e.g. n = 100, strength = 0.29)."""
+        return max(self.n - min(int(self.n * float(strength)), self.n), 0)
+
+    def noise_coeffs(self, j: int):
+        """(a, b) of diffusers' ``add_noise(x0, z, timesteps[j])`` = a x0 + b z, in the loop's state space; ``j``
+        indexes the full plan (PNDM's repeated timestep is an entry of its own).  DDIM / PNDM: sqrt(abar_t),
+        sqrt(1 - abar_t) from diffusers' fp32 alpha-bar table."""
+        t = self.plan()[j].timestep
+        a = float(alphas_cumprod_diffusers(*self._beta_args)[t])
+        return math.sqrt(a), math.sqrt(1.0 - a)
+
+    def blend_coeffs(self, start: int = 0):
+        """Per step of ``plan(start)``: the (a, b) of the inpainting blend after that step, x' = m x' + (1 - m)(a x0_img +
+        b z): ``add_noise`` at the next timestep (``timesteps[k + 1]``, what the inpaint pipeline calls after step k),
+        and on the last step (1 / s_N, 0) -- the image latents themselves, divided by the final input scale."""
+        n_plan = len(self.plan(start))
+        out = [self.noise_coeffs(start + k + 1) for k in range(n_plan - 1)]
+        out.append((1.0 / self.input_scale(start + n_plan), 0.0))
+        return out
 
 
 PREDICTION_TYPES = ("epsilon", "v_prediction")
@@ -220,6 +244,16 @@ class DPMSolverMultistepScheduler(_Base):
             if lower_order_stepped < 2:
                 lower_order_stepped += 1
         return out
+
+    def noise_coeffs(self, j):
+        """diffusers' ``add_noise`` with a begin index set (the inpaint pipeline always sets one) reads the sigma table
+        at the STEP index j, not by timestep value: alpha_t = 1 / sqrt(sigma_j^2 + 1), sigma_t = sigma_j alpha_t, sigma_j
+        evaluated in float64 from diffusers' fp32 alpha-bar table."""
+        t = self.plan()[j].timestep
+        a = float(alphas_cumprod_diffusers(*self._beta_args)[t])
+        sig = math.sqrt((1.0 - a) / a)
+        alpha_t = 1.0 / math.sqrt(sig * sig + 1.0)
+        return alpha_t, sig * alpha_t
 
 
 class PNDMScheduler(_Base):
@@ -361,6 +395,12 @@ class _SigmaScheduler(_Base):
     def _update(self, st, i, sig, sig_next, s_next):
         """Fill ce / ch / history / noise of step i (cx = s / s', x0 = s y - sigma eps are common)."""
         raise NotImplementedError
+
+    def noise_coeffs(self, j):
+        """``add_noise`` = x0 + sigma_j z (sigma table at step index j), divided by s_j = sqrt(sigma_j^2 + 1): the loop
+        state is y = x / s."""
+        sig, s = float(self.sigmas[j]), self.input_scale(j)
+        return 1.0 / s, sig / s
 
 
 class EulerDiscreteScheduler(_SigmaScheduler):

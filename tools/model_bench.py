@@ -1,6 +1,7 @@
 """Iter/s of the device denoising loop for one model, with the attention kernels' share of a step.
 
     python tools/model_bench.py --model sd15|sd21-base|sd21 [--reps 3]
+    python tools/model_bench.py --inpaint [--rounds 5] [--reps 3]
 
 The workload is bench.py's: random-init weights, txt2img 512x512 at UNet batch 2 (uncond, cond), 20 DDIM steps, CFG
 7.5, the 20 steps (with the per-prompt prologue) captured as one CUDA graph by bench.LoopBench and timed with
@@ -31,11 +32,60 @@ def power_limit_w(index):
         return None
 
 
+def inpaint_modes(args, dev):
+    """SD-1.5 512x512, UNet batch 2, 20 DDIM steps, CFG 7.5: the pipeline's own loop graph for text-to-image, for
+    inpainting with the 4-channel blend, and for a 9-channel inpainting UNet, timed alternately ``--rounds`` times."""
+    import numpy as np
+
+    from b200sd import config as C
+    from b200sd.pipeline import B200StableDiffusionPipeline as P
+    from b200sd.pipeline import InpaintInputs
+
+    n = bench.N_STEPS_IMG
+    p4 = P.from_random_init("sd15", images_per_call=1, device=dev, seed=1, scheduler="DDIM")
+    p9 = P.from_random_init("sd15", images_per_call=1, device=dev, seed=1, scheduler="DDIM",
+                            unet_cfg=dict(C.SD15_UNET, in_channels=9))
+    g = torch.Generator().manual_seed(93)
+    emb = torch.cat([torch.zeros(1, 768, 1, 77), torch.randn(1, 768, 1, 77, generator=g)]).half()
+    lat = torch.randn(1, 4, 64, 64, generator=g).half().float()
+    mask = (torch.rand(1, 1, 64, 64, generator=g) > 0.5).float()
+    inp = InpaintInputs(mask, torch.randn(1, 4, 64, 64, generator=g), lat, torch.randn(1, 4, 64, 64, generator=g))
+    graphs = {}
+    for mode, pipe, extra in (("txt2img", p4, None), ("inpaint-blend", p4, inp), ("inpaint-9ch", p9, inp)):
+        before = set(pipe._loop_graphs)
+        pipe.denoise(emb, lat, n, 7.5, inpaint=extra)
+        key, = set(pipe._loop_graphs) - before
+        graphs[mode] = pipe._loop_graphs[key]
+    sync = torch.cuda.synchronize
+    times = {m: [] for m in graphs}
+    sampler = bench.ClockSampler(0)
+    sampler.start()
+    for _ in range(args.rounds):
+        for mode, graph in graphs.items():
+            times[mode].append(bench.timed_replays(graph, args.reps, sync) / n)
+    clocks = sampler.stop()
+    for mode, ms in times.items():
+        med = float(np.median(ms))
+        print(json.dumps({"model": "sd15", "mode": mode,
+                          "workload": "512x512, UNet batch 2, 20 DDIM steps, CFG 7.5, fp16, pipeline loop graph",
+                          "iter_per_s": round(1e3 / med, 2), "ms_per_step": round(med, 4),
+                          "ms_per_step_rounds": [round(v, 4) for v in ms],
+                          "card": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0),
+                          "sm_mhz": clocks.get("sm_mhz"), "clock_events": clocks.get("reasons")}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--model", choices=("sd15", "sd21-base", "sd21"), default="sd15")
     ap.add_argument("--reps", type=int, default=3, help="replays of the 20-step graph per measurement")
+    ap.add_argument("--inpaint", action="store_true", help="SD-1.5: text-to-image vs the two inpainting loops")
+    ap.add_argument("--rounds", type=int, default=5, help="--inpaint: alternated measurements per mode")
     args = ap.parse_args()
+    if args.inpaint:
+        dev = torch.device("cuda", 0)
+        torch.cuda.set_device(dev)
+        inpaint_modes(args, dev)
+        return
 
     from b200sd import lib as L
     from b200sd import scheduler as S
