@@ -658,7 +658,14 @@ def nchw_to_nhwc(x, c_pad=None, out=None, out_dtype=torch.float16):
     return out
 
 
+def _f16_or_f32(x, what):
+    """Kernels with one fp16 / fp32 input flag: any other type would be read as fp16 bits."""
+    if x.dtype not in (torch.float16, torch.float32):
+        raise B200SDError(f"{what}: expected fp16 or fp32 input, got {x.dtype}")
+
+
 def nhwc_to_nchw_f32(x, c=None, out=None):
+    _f16_or_f32(x, "nhwc_to_nchw_f32")
     n, h, w, c_pad = x.shape
     c = c_pad if c is None else c
     if out is None:
@@ -706,6 +713,7 @@ def embed_tokens(ids, token_embedding, position_embedding, out=None):
 
 def ctx_to_tokens(ctx, out=None):
     """(B, D, 1, S) fp16/fp32 -> [B*S, D] fp16."""
+    _f16_or_f32(ctx, "ctx_to_tokens")
     b, d, _, s = ctx.shape
     if not ctx.is_contiguous():
         raise B200SDError("ctx_to_tokens: expected contiguous input")
@@ -772,6 +780,7 @@ def cfg_scheduler_step_blend(noise_pred, latents, coeffs: StepCoeffs, mask, imag
 
 
 def image_postprocess(x, c=3, want_u8=False):
+    _f16_or_f32(x, "image_postprocess")
     n, h, w, c_pad = x.shape
     of = torch.empty(n, h, w, c, dtype=torch.float32, device=x.device)
     ou = torch.empty(n, h, w, c, dtype=torch.uint8, device=x.device) if want_u8 else None

@@ -35,6 +35,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import gemm_plan_cases as G  # noqa: E402
+import model_cases as MC  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -375,53 +376,6 @@ class _Replay:
         return "\n".join(lines)
 
 
-def _model_inputs(m, seed):
-    """Random inputs of a model's declared input spec (timesteps mid-schedule, token ids of a short prompt)."""
-    import numpy as np
-
-    g = torch.Generator().manual_seed(seed)
-    kw = {}
-    for k, spec in m.expected_inputs.items():
-        shp = tuple(spec["shape"])
-        if k == "timestep":
-            v = torch.full(shp, 501.0)
-        elif k == "input_ids":
-            v = torch.randint(0, 49406, shp, generator=g).float()
-            v[:, 0], v[:, 20:] = 49406, 49407
-        elif k == "time_ids":
-            v = torch.tensor([768.0, 768.0, 0.0, 0.0, 768.0, 768.0])[: shp[1]].expand(shp).contiguous()
-        elif k == "controlnet_cond":
-            v = torch.rand(shp, generator=g)
-        else:
-            v = torch.randn(shp, generator=g)
-        kw[k] = v.numpy().astype(np.dtype(spec["dtype"]))
-    return kw
-
-
-def _build(name):
-    from b200sd import config as C
-
-    if name.startswith(("sd21", "sd15", "sdxl")):
-        from b200sd.model import UNetModel
-        cfg = {"sd21": C.SD21_BASE_UNET, "sd15": C.SD15_UNET, "sdxl": C.SDXL_BASE_UNET}[name[:4]]
-        batch = 16 if "b16" in name else 2
-        hw = 96 if name.startswith("sdxl") else 64
-        sd = C.random_state_dict(C.unet_param_shapes(cfg), seed=5, dtype=torch.float16)
-        return UNetModel(cfg, sd, batch=batch, height=hw, width=hw, use_cuda_graph=False)
-    if name == "controlnet_sd21":
-        from b200sd.controlnet import ControlNetModel
-        cfg = C.SD21_CONTROLNET
-        sd = C.random_state_dict(C.controlnet_param_shapes(cfg), seed=6, dtype=torch.float16)
-        return ControlNetModel(cfg, sd, batch=2, height=64, width=64, use_cuda_graph=False)
-    if name == "vae_decoder":
-        from b200sd.vae import VAEDecoderModel
-        sd = C.random_state_dict(C.vae_decoder_param_shapes(C.SD_VAE), seed=7, dtype=torch.float16)
-        return VAEDecoderModel(C.SD_VAE, sd, batch=1, height=64, width=64)
-    from b200sd.text_encoder import TextEncoderModel
-    cfg = {"openclip_h": C.OPENCLIP_H_TEXT, "clip_l": C.CLIP_L_TEXT}[name]
-    return TextEncoderModel(cfg, C.random_clip_text_state_dict(cfg, seed=8, dtype=torch.float16), batch=2)
-
-
 @pytest.mark.parametrize("name", ["sd21_b2", "sd21_b16", "sd15_b2", "sdxl_768_b2", "controlnet_sd21", "vae_decoder",
                                   "openclip_h", "clip_l", "sd21_b2_fused", "sd21_b2_halo_tma"])
 def test_model_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
@@ -440,11 +394,11 @@ def test_model_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
         monkeypatch.setenv("B200SD_HALO_TMA", "1024")
     if name.endswith("_halo_tma"):
         monkeypatch.setenv("B200SD_HALO_TMA", "1024")
-    m = _build(name)
+    m = MC.build(name)
     rep = _Replay(lib, name)
     monkeypatch.setattr(lib, "linear", rep.linear)
     monkeypatch.setattr(lib, "conv3x3", rep.conv3x3)
-    m(**_model_inputs(m, seed=9))
+    m(**MC.model_inputs(m, seed=9))
     torch.cuda.synchronize()
     print("\n" + rep.report())
     assert rep.plans, f"{name}: no GEMM / convolution launch was seen"

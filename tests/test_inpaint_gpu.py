@@ -14,7 +14,8 @@ from b200sd import config
 from b200sd import scheduler as S
 from b200sd.rng import NvRandomSource
 from oracle import restated as R
-from test_gemm_plans_gpu import _model_inputs, _Replay
+from model_cases import model_inputs as _model_inputs
+from test_gemm_plans_gpu import _Replay
 from test_unet_gpu import _check
 
 pytestmark = pytest.mark.gpu

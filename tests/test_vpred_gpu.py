@@ -13,7 +13,8 @@ import vpred_oracle as V
 from b200sd import config
 from b200sd import scheduler as S
 from oracle import restated as R
-from test_gemm_plans_gpu import _Replay, _model_inputs
+from model_cases import model_inputs as _model_inputs
+from test_gemm_plans_gpu import _Replay
 from test_unet_gpu import _check
 
 pytestmark = pytest.mark.gpu
