@@ -337,6 +337,34 @@ int b200sd_latent_prep_bf16(const float* z, const float* w, const float* b, floa
 int b200sd_image_postprocess(const void* in, int32_t in_f32, int32_t c_pad, float* out_f32, uint8_t* out_u8,
                              int32_t n, int32_t h, int32_t w, int32_t c, void* stream);
 
+/* ---- safety checker (csrc/vision.cu) ----
+ * CLIP image preprocessing, bit-exact to Pillow's BICUBIC resize + CLIPImageProcessor's centre crop, rescale and
+ * normalise: u8 NHWC images [n, h, w, 3] -> fp32 NCHW pixel_values [n, 3, crop_h, crop_w].  The resize runs in
+ * Pillow's two 8-bit fixed-point passes (horizontal, then vertical; 22 fractional bits).  The host builds the tables
+ * for the output rows / columns the crop keeps: *_bounds [crop][2] = (first input index, taps), *_coeffs
+ * [crop][ksize] int32.  tmp: u8 scratch of n * h * crop_w * 3 bytes.  mean / std: three host floats each. */
+int b200sd_clip_preprocess(const uint8_t* images, int32_t n, int32_t h, int32_t w, uint8_t* tmp,
+                           const int32_t* h_bounds, const int32_t* h_coeffs, int32_t h_ksize,
+                           const int32_t* v_bounds, const int32_t* v_coeffs, int32_t v_ksize, int32_t crop_h,
+                           int32_t crop_w, const float* mean, const float* std, float* out, void* stream);
+/* Patch-embedding GEMM operand: fp32 NCHW [n, c, S, S] -> fp16 [n * (1 + g*g), k_pad] (g = S / patch).  Per image,
+ * row 0 (the class token) is zero and row 1 + py*g + px holds patch (py, px) in (channel, ky, kx) order; columns
+ * c*patch*patch .. k_pad-1 are zero. */
+int b200sd_patchify(const float* pixel_values, int32_t n, int32_t c, int32_t image_size, int32_t patch, int32_t k_pad,
+                    void* out, void* stream);
+/* Safety-checker head (the graph the reference converts, forward_coreml): image_embeds fp32 [n, dim] against the
+ * L2-normalised concept rows fp32 [n_concepts, dim] / [n_special, dim] and their thresholds; adjustment: one fp32
+ * on the device, or null for 0.  -> concept_scores fp32 [n, n_concepts], has_nsfw fp32 [n] (1 or 0).
+ * n_concepts + n_special <= 32. */
+int b200sd_safety_concepts(const float* image_embeds, int32_t n, int32_t dim, const float* concepts,
+                           const float* concept_weights, int32_t n_concepts, const float* special,
+                           const float* special_weights, int32_t n_special, const float* adjustment,
+                           float* concept_scores, float* has_nsfw, void* stream);
+/* Zero every image whose has_nsfw entry is non-zero, in place, in the fp32 NHWC images and / or their u8 copy
+ * (either may be null); other images are not written. */
+int b200sd_filter_images(const float* has_nsfw, float* images, uint8_t* images_u8, int32_t n, int32_t h, int32_t w,
+                         int32_t c, void* stream);
+
 /* ================================================================================================================
  * Model-level handles: one "predict" per model, like the reference's device boundary.
  *

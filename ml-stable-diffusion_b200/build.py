@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200sd.so")
 STAMP = os.path.join(HERE, ".libb200sd.stamp")
-SOURCES = ["runtime.cu", "gemm_conv.cu", "attention.cu", "norm.cu", "elementwise.cu", "model.cu"]
+SOURCES = ["runtime.cu", "gemm_conv.cu", "attention.cu", "norm.cu", "elementwise.cu", "model.cu", "vision.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math_placeholder",

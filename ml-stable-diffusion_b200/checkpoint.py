@@ -21,6 +21,7 @@ _SCHEMAS = {
     "vae_decoder": C.vae_decoder_param_shapes,
     "vae_encoder": C.vae_encoder_param_shapes,
     "text_encoder": C.clip_text_param_shapes,
+    "safety_checker": C.safety_checker_param_shapes,
 }
 # AutoencoderKL checkpoints written before diffusers 0.18 name the mid-block attention projections query / key / value /
 # proj_attn (diffusers remaps them when it loads the file); the engines use the current names
@@ -105,3 +106,66 @@ def read_config(model_dir: str, component: str) -> dict:
     with open(os.path.join(model_dir, component, name)) as f:
         cfg = json.load(f)
     return {k: (tuple(v) if isinstance(v, list) else v) for k, v in cfg.items() if not k.startswith("_")}
+
+
+# CLIPImageProcessor's defaults (transformers 4.44.2, the release the reference pins)
+OPENAI_CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
+OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
+PREPROCESS_DEFAULTS = dict(size=224, crop_h=224, crop_w=224, mean=OPENAI_CLIP_MEAN, std=OPENAI_CLIP_STD)
+
+
+def _edge(raw, key, default):
+    """``size`` / ``crop_size``: an int, or a dict (``shortest_edge`` for size; ``height`` / ``width`` for crop_size)."""
+    v = raw.get(key, default)
+    if isinstance(v, bool) or not isinstance(v, (int, dict)):
+        raise ValueError(f"preprocessor_config.json: {key}={v!r} is neither an int nor a dict")
+    return v
+
+
+def preprocessor_config(raw: dict) -> dict:
+    """A ``feature_extractor/preprocessor_config.json`` (CLIPFeatureExtractor / CLIPImageProcessor) -> dict(size,
+    crop_h, crop_w, mean, std).  Only the pipeline the safety checker was trained with runs on the device: BICUBIC
+    (resample = 3) resize of the shortest edge, centre crop, rescale by 1/255 and normalise.  Anything else raises a
+    ValueError that names the key."""
+    for key in ("do_resize", "do_center_crop", "do_rescale", "do_normalize"):
+        if raw.get(key, True) is not True:
+            raise ValueError(f"preprocessor_config.json: {key}={raw[key]!r}; the safety checker's preprocessing "
+                             "needs resize, centre crop, rescale and normalise")
+    if raw.get("resample", 3) != 3:
+        raise ValueError(f"preprocessor_config.json: resample={raw['resample']!r}; only 3 (BICUBIC) is implemented")
+    if abs(float(raw.get("rescale_factor", 1 / 255)) - 1 / 255) > 1e-12:
+        raise ValueError(f"preprocessor_config.json: rescale_factor={raw['rescale_factor']!r}; only 1/255 is "
+                         "implemented")
+    size = _edge(raw, "size", 224)
+    if isinstance(size, dict):
+        if "shortest_edge" not in size:
+            raise ValueError(f"preprocessor_config.json: size={size!r}; only a shortest_edge resize is implemented")
+        size = size["shortest_edge"]
+    crop = _edge(raw, "crop_size", 224)
+    if isinstance(crop, dict):
+        if "height" not in crop or "width" not in crop:
+            raise ValueError(f"preprocessor_config.json: crop_size={crop!r} needs height and width")
+        crop_h, crop_w = crop["height"], crop["width"]
+    else:
+        crop_h = crop_w = crop
+    if crop_h > size or crop_w > size:
+        raise ValueError(f"preprocessor_config.json: crop_size {crop_h}x{crop_w} is larger than size {size}")
+    mean = tuple(float(v) for v in raw.get("image_mean", OPENAI_CLIP_MEAN))
+    std = tuple(float(v) for v in raw.get("image_std", OPENAI_CLIP_STD))
+    for key, v in (("image_mean", mean), ("image_std", std)):
+        if len(v) != 3:
+            raise ValueError(f"preprocessor_config.json: {key} has {len(v)} entries, expected 3")
+    return dict(size=int(size), crop_h=int(crop_h), crop_w=int(crop_w), mean=mean, std=std)
+
+
+def load_safety_checker(model_dir: str):
+    """``<model_dir>/safety_checker/`` and ``<model_dir>/feature_extractor/`` -> (config, state dict, preprocessing
+    config).  A checker without a feature extractor raises."""
+    fe = os.path.join(model_dir, "feature_extractor", "preprocessor_config.json")
+    if not os.path.exists(fe):
+        raise FileNotFoundError(f"{model_dir} has a safety_checker/ but no feature_extractor/preprocessor_config.json")
+    with open(os.path.join(model_dir, "safety_checker", "config.json")) as f:
+        cfg = C.safety_checker_config(json.load(f))
+    with open(fe) as f:
+        pre = preprocessor_config(json.load(f))
+    return cfg, load_component(model_dir, "safety_checker", cfg), pre

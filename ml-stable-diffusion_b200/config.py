@@ -378,3 +378,94 @@ def random_clip_text_state_dict(cfg, seed=0, dtype=torch.float32):
             t = 0.1 * torch.randn(shp, generator=g)
         sd[name] = t.to(dtype)
     return sd
+
+
+# ---------------------------------------------------------------------------------------------------
+# Stable Diffusion safety checker (diffusers' StableDiffusionSafetyChecker: a transformers.CLIPVisionModel, a bias-free
+# visual projection and 17 + 3 concept embeddings with thresholds; the reference converts it with forward_coreml,
+# torch2coreml.py:1177-1209, and runs it after the VAE decode, pipeline.py:286-311)
+# ---------------------------------------------------------------------------------------------------
+# transformers.CLIPVisionConfig() defaults: they fill the keys a checkpoint's `vision_config` leaves out
+CLIP_VISION_DEFAULTS = dict(hidden_size=768, intermediate_size=3072, num_hidden_layers=12, num_attention_heads=12,
+                            num_channels=3, image_size=224, patch_size=32, hidden_act="quick_gelu", layer_norm_eps=1e-5)
+# CLIPConfig's default projection_dim (the checkpoint's top-level "projection_dim" overrides it)
+CLIP_PROJECTION_DIM_DEFAULT = 512
+# CompVis/stable-diffusion-safety-checker, shipped as `safety_checker/` with SD 1.4 / 1.5: ViT-L/14 at 224
+SD_SAFETY_CHECKER = dict(CLIP_VISION_DEFAULTS, hidden_size=1024, intermediate_size=4096, num_hidden_layers=24,
+                         num_attention_heads=16, patch_size=14, projection_dim=768, num_concepts=17,
+                         num_special_concepts=3)
+TINY_SAFETY_CHECKER = dict(CLIP_VISION_DEFAULTS, hidden_size=128, intermediate_size=512, num_hidden_layers=2,
+                           num_attention_heads=2, patch_size=14, projection_dim=64, num_concepts=17,
+                           num_special_concepts=3)
+
+
+def safety_checker_config(raw: dict) -> dict:
+    """A ``safety_checker/config.json`` (a CLIPConfig) -> the flat config the engine reads: the ``vision_config`` keys
+    over CLIP_VISION_DEFAULTS, the top-level ``projection_dim``, and StableDiffusionSafetyChecker's fixed 17 + 3
+    concept rows."""
+    vis = raw.get("vision_config") or {}
+    cfg = dict(CLIP_VISION_DEFAULTS)
+    cfg.update({k: vis[k] for k in CLIP_VISION_DEFAULTS if k in vis})
+    cfg["projection_dim"] = raw.get("projection_dim", CLIP_PROJECTION_DIM_DEFAULT)
+    cfg["num_concepts"], cfg["num_special_concepts"] = 17, 3
+    return cfg
+
+
+def safety_checker_param_shapes(cfg):
+    """State-dict schema of StableDiffusionSafetyChecker (its CLIPVisionModel sits under ``vision_model.``)."""
+    d, f, p, c = cfg["hidden_size"], cfg["intermediate_size"], cfg["patch_size"], cfg["num_channels"]
+    g = cfg["image_size"] // p
+    proj = cfg["projection_dim"]
+    v = "vision_model.vision_model."
+    s = OrderedDict()
+    s[v + "embeddings.class_embedding"] = (d,)
+    s[v + "embeddings.patch_embedding.weight"] = (d, c, p, p)
+    s[v + "embeddings.position_embedding.weight"] = (g * g + 1, d)
+    s[v + "pre_layrnorm.weight"], s[v + "pre_layrnorm.bias"] = (d,), (d,)
+    for i in range(cfg["num_hidden_layers"]):
+        q = f"{v}encoder.layers.{i}."
+        for nm in ("q_proj", "k_proj", "v_proj", "out_proj"):
+            s[q + f"self_attn.{nm}.weight"] = (d, d)
+            s[q + f"self_attn.{nm}.bias"] = (d,)
+        for ln in ("layer_norm1", "layer_norm2"):
+            s[q + ln + ".weight"] = (d,)
+            s[q + ln + ".bias"] = (d,)
+        s[q + "mlp.fc1.weight"], s[q + "mlp.fc1.bias"] = (f, d), (f,)
+        s[q + "mlp.fc2.weight"], s[q + "mlp.fc2.bias"] = (d, f), (d,)
+    s[v + "post_layernorm.weight"], s[v + "post_layernorm.bias"] = (d,), (d,)
+    s["visual_projection.weight"] = (proj, d)
+    s["concept_embeds"] = (cfg["num_concepts"], proj)
+    s["special_care_embeds"] = (cfg["num_special_concepts"], proj)
+    s["concept_embeds_weights"] = (cfg["num_concepts"],)
+    s["special_care_embeds_weights"] = (cfg["num_special_concepts"],)
+    return s
+
+
+SAFETY_CONCEPT_KEYS = ("concept_embeds", "special_care_embeds", "concept_embeds_weights", "special_care_embeds_weights")
+
+
+def random_safety_checker_state_dict(cfg, seed=0, dtype=torch.float32):
+    """Random-init safety-checker weights (conventions of random_clip_text_state_dict; the patch embedding is a conv,
+    U(+-1/sqrt(fan_in))).  The concept tables are fp32 whatever ``dtype`` is: N(0, 1) embeddings and thresholds of
+    4 to 5 / sqrt(projection_dim), four standard deviations or more above the cosine of a random direction with them,
+    so random images are not flagged."""
+    g = torch.Generator().manual_seed(seed)
+    sd = OrderedDict()
+    for name, shp in safety_checker_param_shapes(cfg).items():
+        if name in SAFETY_CONCEPT_KEYS:
+            t = torch.randn(shp, generator=g) if len(shp) == 2 else \
+                (4 + torch.rand(shp, generator=g)) * cfg["projection_dim"] ** -0.5
+            sd[name] = t.float()
+            continue
+        if "embedding" in name and len(shp) != 4:
+            t = 0.5 * torch.randn(shp, generator=g)
+        elif any(k in name for k in ("layer_norm", "layrnorm", "layernorm")):
+            t = (1.0 + 0.1 * torch.randn(shp, generator=g)) if name.endswith("weight") else 0.1 * torch.randn(shp, generator=g)
+        elif len(shp) == 4:
+            t = (torch.rand(shp, generator=g) * 2 - 1) * (shp[1] * shp[2] * shp[3]) ** -0.5
+        elif len(shp) == 2:
+            t = (torch.rand(shp, generator=g) * 2 - 1) * shp[1] ** -0.5
+        else:
+            t = 0.1 * torch.randn(shp, generator=g)
+        sd[name] = t.to(dtype)
+    return sd

@@ -121,6 +121,18 @@ _SIGNATURES = {
                                                   C.POINTER(BlendArgs), C.c_void_p]),
     "b200sd_image_postprocess":(C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    # safety checker (csrc/vision.cu)
+    "b200sd_clip_preprocess": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p,
+                                         C.c_void_p]),
+    "b200sd_patchify": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                  C.c_void_p]),
+    "b200sd_safety_concepts": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                         C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
+    "b200sd_filter_images": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_void_p]),
 }
 # bf16 twins (include/b200sd.h): same signatures, every fp16 pointer is bf16
 for _name in ("b200sd_gemm", "b200sd_gemm_plan_ex", "b200sd_gemm_describe_plan", "b200sd_group_norm",
@@ -787,6 +799,88 @@ def image_postprocess(x, c=3, want_u8=False):
     _check(load().b200sd_image_postprocess(_ptr(x), int(x.dtype == torch.float32), c_pad, _ptr(of), _ptr(ou), n, h,
                                            w, c, _stream()), "b200sd_image_postprocess")
     return (of, ou) if want_u8 else of
+
+
+def clip_preprocess(images_u8, h_table, v_table, mean, std, out=None, tmp=None):
+    """u8 NHWC [n, h, w, 3] -> fp32 NCHW pixel_values [n, 3, crop_h, crop_w]: Pillow BICUBIC resize (horizontal then
+    vertical fixed-point pass), centre crop, rescale, normalise.  h_table / v_table: (bounds int32 [crop, 2], coeffs
+    int32 [crop, ksize]) CUDA tensors from ``safety_checker.resample_table`` restricted to the crop window."""
+    _req(images_u8, torch.uint8, "clip_preprocess images")
+    n, h, w, c = images_u8.shape
+    if c != 3:
+        raise B200SDError(f"clip_preprocess: expected 3 channels, got {c}")
+    (hb, hc), (vb, vc) = h_table, v_table
+    for t, nm in ((hb, "h bounds"), (hc, "h coeffs"), (vb, "v bounds"), (vc, "v coeffs")):
+        _req(t, torch.int32, f"clip_preprocess {nm}")
+    crop_w, crop_h = hb.shape[0], vb.shape[0]
+    if out is None:
+        out = torch.empty(n, 3, crop_h, crop_w, dtype=torch.float32, device=images_u8.device)
+    _req(out, torch.float32, "clip_preprocess out")
+    if tmp is None or tmp.numel() < n * h * crop_w * 3:
+        tmp = torch.empty(n * h * crop_w * 3, dtype=torch.uint8, device=images_u8.device)
+    fm, fs = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    _check(load().b200sd_clip_preprocess(_ptr(images_u8), n, h, w, _ptr(tmp), _ptr(hb), _ptr(hc), hc.shape[1],
+                                         _ptr(vb), _ptr(vc), vc.shape[1], crop_h, crop_w, fm, fs, _ptr(out),
+                                         _stream()), "b200sd_clip_preprocess")
+    return out
+
+
+def patchify(pixel_values, patch, k_pad, out=None):
+    """fp32 NCHW [n, c, S, S] -> fp16 [n * (1 + (S/patch)^2), k_pad]: per image a zero class-token row, then the
+    patches in row-major order, each flattened in (channel, ky, kx) order and zero padded to k_pad columns."""
+    _req(pixel_values, torch.float32, "patchify pixel_values")
+    n, c, s, s2 = pixel_values.shape
+    if s != s2 or s % patch:
+        raise B200SDError(f"patchify: {s}x{s2} images do not tile into {patch}x{patch} patches")
+    rows = n * (1 + (s // patch) ** 2)
+    if out is None:
+        out = torch.empty(rows, k_pad, dtype=torch.float16, device=pixel_values.device)
+    _req(out, torch.float16, "patchify out")
+    if tuple(out.shape) != (rows, k_pad):
+        raise B200SDError(f"patchify: out has shape {tuple(out.shape)}, expected {(rows, k_pad)}")
+    _check(load().b200sd_patchify(_ptr(pixel_values), n, c, s, patch, k_pad, _ptr(out), _stream()), "b200sd_patchify")
+    return out
+
+
+def safety_concepts(image_embeds, concepts, concept_weights, special, special_weights, adjustment=None):
+    """fp32 image_embeds [n, dim] -> (concept_scores fp32 [n, n_concepts], has_nsfw fp32 [n]) against the
+    L2-normalised concept tables; ``adjustment``: a one-element fp32 CUDA tensor (None: 0)."""
+    for t, nm in ((image_embeds, "image_embeds"), (concepts, "concepts"), (concept_weights, "concept_weights"),
+                  (special, "special"), (special_weights, "special_weights")):
+        _req(t, torch.float32, f"safety_concepts {nm}")
+    if adjustment is not None:
+        _req(adjustment, torch.float32, "safety_concepts adjustment")
+    n, dim = image_embeds.shape
+    nc, ns = concepts.shape[0], special.shape[0]
+    if concepts.shape[1] != dim or special.shape[1] != dim:
+        raise B200SDError(f"safety_concepts: concept tables of width {concepts.shape[1]} / {special.shape[1]}, "
+                          f"embeddings of width {dim}")
+    scores = torch.empty(n, nc, dtype=torch.float32, device=image_embeds.device)
+    flags = torch.empty(n, dtype=torch.float32, device=image_embeds.device)
+    _check(load().b200sd_safety_concepts(_ptr(image_embeds), n, dim, _ptr(concepts), _ptr(concept_weights), nc,
+                                         _ptr(special), _ptr(special_weights), ns, _ptr(adjustment), _ptr(scores),
+                                         _ptr(flags), _stream()), "b200sd_safety_concepts")
+    return scores, flags
+
+
+def filter_images(has_nsfw, images=None, images_u8=None):
+    """Zero, in place, every image whose ``has_nsfw`` entry (fp32 [n]) is non-zero: fp32 and / or u8 NHWC images."""
+    _req(has_nsfw, torch.float32, "filter_images has_nsfw")
+    ref = images if images is not None else images_u8
+    if ref is None:
+        raise B200SDError("filter_images: no images given")
+    if images is not None:
+        _req(images, torch.float32, "filter_images images")
+    if images_u8 is not None:
+        _req(images_u8, torch.uint8, "filter_images images_u8")
+        if images is not None and images_u8.shape != images.shape:
+            raise B200SDError("filter_images: the fp32 and u8 images differ in shape")
+    n, h, w, c = ref.shape
+    if has_nsfw.numel() != n:
+        raise B200SDError(f"filter_images: {has_nsfw.numel()} flags for {n} images")
+    _check(load().b200sd_filter_images(_ptr(has_nsfw), _ptr(images), _ptr(images_u8), n, h, w, c, _stream()),
+           "b200sd_filter_images")
+    return images, images_u8
 
 
 def softmax_rows(scores, scale, out=None, out_dtype=torch.float16):

@@ -124,8 +124,11 @@ class B200StableDiffusionPipeline:
 
     def __init__(self, unet: UNetModel, vae_decoder: VAEDecoderModel, scheduler="DDIM", text_encoder=None,
                  tokenizer=None, force_zeros_for_empty_prompt=True, xl=False, controlnet=None, loop_graph=True,
-                 vae_encoder=None, text_encoder_2=None, tokenizer_2=None, scheduler_kwargs=None, unet_refiner=None):
+                 vae_encoder=None, text_encoder_2=None, tokenizer_2=None, scheduler_kwargs=None, unet_refiner=None,
+                 safety_checker=None):
         self.unet = unet
+        # safety_checker.SafetyCheckerEngine or None: runs after the VAE decode, on the device (pipeline.py:286-311)
+        self.safety_checker = safety_checker
         # SDXL refiner UNet (StableDiffusionXLPipeline.swift:205-225): takes over the loop at step
         # int(len(timesteps) * refiner_start) with its own conditioning (set_refiner_inputs)
         self.unet_refiner = unet_refiner
@@ -175,7 +178,8 @@ class B200StableDiffusionPipeline:
     @classmethod
     def from_random_init(cls, model_version="sd21-base", images_per_call=1, device="cuda", seed=0,
                          scheduler="DDIM", height=None, width=None, unet_cfg=None, vae_cfg=None, controlnet_cfgs=None,
-                         text_encoder_cfg=None, tokenizer=None, with_vae_encoder=False, scheduler_kwargs=None):
+                         text_encoder_cfg=None, tokenizer=None, with_vae_encoder=False, scheduler_kwargs=None,
+                         safety_checker_cfg=None):
         """Random-init weights of the named architecture (no checkpoints exist offline).  ``controlnet_cfgs``:
         list of ControlNet configs (seeded seed+2, seed+3, ...); switches the UNet to its control variant.
         ``model_version``: "sd21-base", "sd21" (SD 2.0 / 2.1 768-v: 768x768 by default, v-prediction), "sd15"
@@ -184,7 +188,9 @@ class B200StableDiffusionPipeline:
         text encoder runs on the
         device (random-init, seed+100) instead of the synthetic embedding table; ``tokenizer``: e.g. a
         ``tokenizer.BPETokenizer`` built from the checkpoint's vocab.json / merges.txt.  ``scheduler_kwargs``: extra
-        scheduler arguments (e.g. ``{"prediction_type": "v_prediction"}``, the default for "sd21")."""
+        scheduler arguments (e.g. ``{"prediction_type": "v_prediction"}``, the default for "sd21").
+        ``safety_checker_cfg``: e.g. config.SD_SAFETY_CHECKER -> a random-init safety checker (seed+200) with
+        CLIPImageProcessor's default preprocessing."""
         native = 768 if model_version == "sd21" else 512
         height, width = height or native, width or native
         scheduler_kwargs = dict(scheduler_kwargs or {})
@@ -225,22 +231,29 @@ class B200StableDiffusionPipeline:
             from .vae import VAEEncoderModel
             esd = C.random_state_dict(C.vae_encoder_param_shapes(vae_cfg), seed=seed + 50, dtype=torch.float16)
             venc = VAEEncoderModel(vae_cfg, esd, batch=images_per_call, height=height, width=width, device=device)
+        checker = None
+        if safety_checker_cfg is not None:
+            from .safety_checker import SafetyCheckerEngine
+            checker = SafetyCheckerEngine(safety_checker_cfg, C.random_safety_checker_state_dict(
+                safety_checker_cfg, seed=seed + 200, dtype=torch.float16), device=device)
         return cls(unet, vae, scheduler=scheduler, xl=unet.engine.xl, controlnet=nets, text_encoder=enc,
                    tokenizer=tokenizer, vae_encoder=venc, force_zeros_for_empty_prompt=unet.engine.xl,
-                   scheduler_kwargs=scheduler_kwargs)
+                   scheduler_kwargs=scheduler_kwargs, safety_checker=checker)
 
     _SCHEDULER_CLASS = {"PNDMScheduler": "PNDM", "DDIMScheduler": "DDIM", "DPMSolverMultistepScheduler": "DPMSolverMultistep"}
 
     @classmethod
     def from_pretrained(cls, model_dir, images_per_call=1, device="cuda", height=None, width=None,
                         scheduler_override=None, controlnet_dirs=None, force_zeros_for_empty_prompt=None,
-                        with_vae_encoder=False, refiner_dir=None):
+                        with_vae_encoder=False, refiner_dir=None, load_safety_checker=True):
         """Build the pipeline from a diffusers-layout model directory (``unet/``, ``vae/``, ``text_encoder[_2]/``,
         ``tokenizer[_2]/``, ``scheduler/``): the counterpart of ``get_coreml_pipe(pytorch_pipe, mlpackages_dir,
         model_version, compute_unit, scheduler_override, controlnet_models, force_zeros_for_empty_prompt)``
         (pipeline.py:607-697), which wires converted .mlpackage files to the same slots.  Weights are read with
         ``checkpoint.load_component`` (schema-checked), configs with ``checkpoint.read_config``.
-        ``refiner_dir``: an SDXL refiner directory whose UNet takes over at ``refiner_start`` (``__call__``)."""
+        ``refiner_dir``: an SDXL refiner directory whose UNet takes over at ``refiner_start`` (``__call__``).
+        ``load_safety_checker``: load ``safety_checker/`` with ``feature_extractor/`` when the directory has them (SD 1.4
+        / 1.5; get_coreml_pipe loads it whenever the diffusers pipeline has one, pipeline.py:650-656); False skips it."""
         import json
         import os
         from . import checkpoint as K
@@ -327,9 +340,13 @@ class B200StableDiffusionPipeline:
                                 width=w, device=device)
         if force_zeros_for_empty_prompt is None:
             force_zeros_for_empty_prompt = xl   # the reference's CLI sets it for SDXL only (pipeline.py:744-755)
+        checker = None
+        if load_safety_checker and os.path.isdir(os.path.join(model_dir, "safety_checker")):
+            from .safety_checker import SafetyCheckerEngine
+            checker = SafetyCheckerEngine(*K.load_safety_checker(model_dir), device=device)
         return cls(unet, vae, scheduler=sched, text_encoder=enc1, tokenizer=tok1, text_encoder_2=enc2, tokenizer_2=tok2,
                    xl=xl, controlnet=nets, vae_encoder=venc, force_zeros_for_empty_prompt=force_zeros_for_empty_prompt,
-                   unet_refiner=refiner, scheduler_kwargs=sched_kw)
+                   unet_refiner=refiner, scheduler_kwargs=sched_kw, safety_checker=checker)
 
     # ---------------------------------------------------------------- reference-named helpers
     def check_inputs(self, prompt, height, width, callback_steps):
@@ -725,13 +742,28 @@ class B200StableDiffusionPipeline:
                 callback(i, st.timestep, x_space(i + 1))
         return self._denoised if return_denoised else self._latents
 
-    def decode_latents(self, latents):
-        """pipeline.py:313-320 on the device: z / scaling -> decoder -> clip(x/2+0.5, 0, 1) -> NHWC fp32."""
+    def decode_latents(self, latents, want_u8=False):
+        """pipeline.py:313-320 on the device: z / scaling -> decoder -> clip(x/2+0.5, 0, 1) -> NHWC fp32 (and, with
+        ``want_u8``, numpy_to_pil's u8 pixels round(255 x))."""
         eng = self.vae_decoder.engine
         self.vae_decoder._z.copy_(latents)
         self.vae_decoder._z.mul_(1.0 / eng.scaling)
         img = eng.forward(self.vae_decoder._z)
-        return L.image_postprocess(img, c=eng.out_ch)
+        return L.image_postprocess(img, c=eng.out_ch, want_u8=want_u8)
+
+    def decode_and_check(self, latents):
+        """Decode, then pipeline.py:286-311 on the device: CLIP preprocessing of the u8 pixels, the vision tower,
+        concept scoring, flagged images zeroed -- and one copy of images and flags to the host at the end.  Differs
+        from the reference by design in two ways: the returned images keep the pipeline's fp32 values (the reference
+        casts them to fp16 for the Core ML call and returns that cast), and the flags are a List[bool], the type
+        StableDiffusionPipelineOutput declares (the reference passes its raw (B, 1, 1, 1) array through).
+        -> (images float32 NHWC numpy, nsfw_content_detected or None without a checker)."""
+        if self.safety_checker is None:
+            return self.decode_latents(latents).cpu().numpy(), None
+        image, image_u8 = self.decode_latents(latents, want_u8=True)
+        flags, _ = self.safety_checker.check(image, image_u8)
+        image, flags = image.cpu().numpy(), flags.cpu().numpy()
+        return image, [bool(f) for f in flags]
 
     # ---------------------------------------------------------------- public API
     def __call__(self, prompt, height=512, width=512, num_inference_steps=50, guidance_scale=7.5,
@@ -868,8 +900,7 @@ class B200StableDiffusionPipeline:
                              time_ids, text_embeds, controlnet_cond=controlnet_cond or None, start_step=start_step,
                              refiner=refiner, refiner_start=refiner_start, noise_key=noise_key,
                              noise_offset=noise_offset, inpaint=inpaint)
-        image = self.decode_latents(final).cpu().numpy()  # single device->host copy of the result
-        has_nsfw = None  # the safety checker is out of scope (SURVEY section 2, row 19)
+        image, has_nsfw = self.decode_and_check(final)  # the only device->host copies of the result
         if output_type == "pil":
             image = self.numpy_to_pil(image)
         if not return_dict:

@@ -11,10 +11,11 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from . import clip_encoder as E
 from . import lib as L
 from .model import B200Model
 
-_ACT = {"gelu": 2, "quick_gelu": 3}
+_ACT = E.ACT
 
 
 class TextEncoderEngine:
@@ -49,19 +50,7 @@ class TextEncoderEngine:
         w = {"tok": f16("text_model.embeddings.token_embedding.weight"),
              "pos": f16("text_model.embeddings.position_embedding.weight"),
              "lnf_g": f32("text_model.final_layer_norm.weight"), "lnf_b": f32("text_model.final_layer_norm.bias"),
-             "layers": []}
-        for i in range(self.layers):
-            p = f"text_model.encoder.layers.{i}."
-            qkv = torch.cat([sd[p + f"self_attn.{n}.weight"].detach().float() for n in ("q_proj", "k_proj", "v_proj")], 0)
-            qkv_b = torch.cat([sd[p + f"self_attn.{n}.bias"].detach().float() for n in ("q_proj", "k_proj", "v_proj")], 0)
-            w["layers"].append({
-                "ln1_g": f32(p + "layer_norm1.weight"), "ln1_b": f32(p + "layer_norm1.bias"),
-                "qkv": qkv.to(device=dev, dtype=torch.float16).contiguous(), "qkv_b": qkv_b.to(dev).contiguous(),
-                "o": f16(p + "self_attn.out_proj.weight"), "o_b": f32(p + "self_attn.out_proj.bias"),
-                "ln2_g": f32(p + "layer_norm2.weight"), "ln2_b": f32(p + "layer_norm2.bias"),
-                "fc1": f16(p + "mlp.fc1.weight"), "fc1_b": f32(p + "mlp.fc1.bias"),
-                "fc2": f16(p + "mlp.fc2.weight"), "fc2_b": f32(p + "mlp.fc2.bias"),
-            })
+             "layers": E.pack_layers(sd, "text_model.encoder.layers.", self.layers, dev)}
         self.w = w
 
     def forward(self, ids, hidden_layer=None):
@@ -73,18 +62,13 @@ class TextEncoderEngine:
         b, s = ids.shape
         want = None if hidden_layer is None else hidden_layer % (self.layers + 1)
         x = L.embed_tokens(ids, w["tok"], w["pos"])
-        picked = x if want == 0 else None
-        for i, ly in enumerate(w["layers"]):
-            n1 = L.layer_norm(x, ly["ln1_g"], ly["ln1_b"], eps=self.eps)
-            qkv = L.linear(n1, ly["qkv"], ly["qkv_b"], static_w=True)
-            a = L.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], b, self.heads, s, s, causal=True)
-            x = L.linear(a, ly["o"], ly["o_b"], x, static_w=True)
-            n2 = L.layer_norm(x, ly["ln2_g"], ly["ln2_b"], eps=self.eps)
-            hdn = L.linear(n2, ly["fc1"], ly["fc1_b"], act=self.act, static_w=True)
-            x = L.linear(hdn, ly["fc2"], ly["fc2_b"], x, static_w=True)
+        picked = [x if want == 0 else None]
+
+        def keep(i, h):
             if want == i + 1:
-                picked = x
-        return L.layer_norm(x, w["lnf_g"], w["lnf_b"], eps=self.eps), picked
+                picked[0] = h
+        x = E.run_layers(x, w["layers"], b, s, d, self.heads, self.act, self.eps, causal=True, on_layer=keep)
+        return L.layer_norm(x, w["lnf_g"], w["lnf_b"], eps=self.eps), picked[0]
 
     def pooled(self, last_hidden, eos_rows):
         """last_hidden fp16 [B*S, D]; eos_rows: LongTensor of the flattened end-of-text row per batch element ->
