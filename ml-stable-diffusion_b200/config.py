@@ -46,6 +46,41 @@ SDXL_BASE_UNET = dict(
     projection_class_embeddings_input_dim=2816,
 )
 
+# SDXL refiner (stabilityai/stable-diffusion-xl-refiner-1.0 unet/config.json): four levels of 384 / 768 / 1536 / 1536
+# channels, 6 / 12 / 24 / 24 heads of 64, depth-4 transformers, conditioned on OpenCLIP bigG alone (1280-wide states).
+# Its time ids are five (original size, crop, aesthetic score): 5 x 256 sinusoids + the 1280-wide pooled embedding =
+# 2560 inputs of add_embedding.  The published file does not name that count; num_time_ids() derives it.
+SDXL_REFINER_UNET = dict(
+    sample_size=128, in_channels=4, out_channels=4,
+    down_block_types=("DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D", "DownBlock2D"),
+    up_block_types=("UpBlock2D", "CrossAttnUpBlock2D", "CrossAttnUpBlock2D", "UpBlock2D"),
+    block_out_channels=(384, 768, 1536, 1536), layers_per_block=2,
+    attention_head_dim=(6, 12, 24, 24), cross_attention_dim=1280,
+    norm_num_groups=32, norm_eps=1e-5, flip_sin_to_cos=True, freq_shift=0,
+    transformer_layers_per_block=4,
+    addition_embed_type="text_time", addition_time_embed_dim=256,
+    projection_class_embeddings_input_dim=2560, num_time_ids=5,
+)
+
+# width of the pooled text embedding an SDXL UNet's add_embedding reads next to the time ids (OpenCLIP bigG's
+# projection_dim, the second text encoder of SDXL-base and the refiner's only one)
+SDXL_POOLED_DIM = 1280
+
+
+def num_time_ids(cfg, pooled_dim=SDXL_POOLED_DIM) -> int:
+    """How many time ids a `text_time` UNet takes: cfg["num_time_ids"] when given, else what the pooled embedding
+    leaves of add_embedding's input, (projection_class_embeddings_input_dim - pooled_dim) / addition_time_embed_dim:
+    6 for SDXL-base (2816), 5 for the refiner (2560).  A diffusers config.json names only the total."""
+    if cfg.get("num_time_ids"):
+        return int(cfg["num_time_ids"])
+    rest = cfg["projection_class_embeddings_input_dim"] - pooled_dim
+    ate = cfg["addition_time_embed_dim"]
+    if rest <= 0 or rest % ate:
+        raise ValueError(f"projection_class_embeddings_input_dim {cfg['projection_class_embeddings_input_dim']} is not "
+                         f"a {pooled_dim}-wide pooled embedding plus a whole number of {ate}-wide time ids")
+    return rest // ate
+
+
 # small config for fast CPU/GPU parity tests (same topology, d_head = 64)
 TINY_UNET = dict(
     sample_size=16, in_channels=4, out_channels=4,

@@ -9,6 +9,7 @@
 #include "../../include/b200sd.h"
 
 #include <algorithm>
+#include <cstdint>
 #include <cooperative_groups.h>
 #include <stdlib.h>
 
@@ -670,8 +671,15 @@ static int group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, in
     float* partial = stats_ws;
     float* final_stats = stats_ws + static_cast<size_t>(n_img) * chunks * groups * 2;
     const size_t smem1 = (static_cast<size_t>(rows) * C * 2 + static_cast<size_t>(C) * 2) * sizeof(float);
-    static size_t smem1_max = 48 * 1024;
-    if (smem1 > smem1_max) {
+    // the 48 KB a launch gets without opting in holds the kernel's static shared memory (s_ticket) too: at C = 3072
+    // (384 vectors, one row) the dynamic part alone is exactly 48 KB, and the launch is refused unless opted in
+    static size_t smem1_static = SIZE_MAX, smem1_max = 0;
+    if (smem1_static == SIZE_MAX) {
+        cudaFuncAttributes fa;
+        B200SD_CHECK_CUDA(cudaFuncGetAttributes(&fa, gn_stats_kernel<T>));
+        smem1_static = fa.sharedSizeBytes;
+    }
+    if (smem1 + smem1_static > 48 * 1024 && smem1 > smem1_max) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(gn_stats_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                static_cast<int>(smem1)));
         smem1_max = smem1;

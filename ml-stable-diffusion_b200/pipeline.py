@@ -336,6 +336,14 @@ class B200StableDiffusionPipeline:
         refiner = None
         if refiner_dir:
             rcfg = K.read_config(refiner_dir, "unet")
+            # the refiner's config.json names add_embedding's input width (2560) but not its five time ids; the rows
+            # __call__ builds for it are five wide, so the count comes from the width its pooled embedding leaves
+            pooled = C.SDXL_POOLED_DIM
+            enc2 = os.path.join(refiner_dir, "text_encoder_2", "config.json")
+            if os.path.exists(enc2):
+                with open(enc2) as fh:
+                    pooled = json.load(fh).get("projection_dim", pooled)
+            rcfg = dict(rcfg, num_time_ids=C.num_time_ids(rcfg, pooled))
             refiner = UNetModel(rcfg, K.load_component(refiner_dir, "unet", rcfg), batch=2 * images_per_call, height=h,
                                 width=w, device=device)
         if force_zeros_for_empty_prompt is None:

@@ -9,7 +9,8 @@ normalisation statistics taken from the operand itself (never from the sums hand
 Tolerance.  Per output element, |got - ref| <= r_out * |ref| + tau * B, with B the same computation on magnitudes:
 B = |A| . |W|^T + |bias| + |residual|.
   * r_out = 2^-10 for fp16 output (round to nearest is within 2^-11 relative; a factor 2 of headroom); 0 for fp32
-    output.  The staged epilogue rounds acc + bias to fp16
+    output.  bf16 output (the bf16 VAEs): r_out = 2^-7 and tau * B charged (1 + r_out) times, the rounded fp32 value
+    being itself tau * B off (test_vae_bf16_gpu.py derives both).  The staged epilogue rounds acc + bias to fp16
     before it adds the residual, so there the rounding of that intermediate is charged too: r_out * (|ref| + |pre|).
   * tau = 2^-14 for fp16 operands: products are exact in fp32 and the wgmma accumulation and the split-K / cluster
     reductions add fp32 rounding of ~2^-24 per addition; over K <= 11520 that is far below 2^-14 * sum |a w| for
@@ -29,6 +30,7 @@ Statistics outputs (rowstats, column stats) are checked against fp64 sums of the
 bit-identical (split-K reductions, cluster reductions, statistics tickets)."""
 import os
 import sys
+import time
 
 import pytest
 import torch
@@ -40,6 +42,7 @@ import model_cases as MC  # noqa: E402
 pytestmark = pytest.mark.gpu
 
 R_OUT_F16 = 2.0 ** -10
+R_OUT_BF16 = 2.0 ** -7
 TAU = 2.0 ** -14
 TAU_NORM = 2.0 ** -11
 ACT_LIP = 1.13
@@ -138,15 +141,27 @@ def _group_norm(x, groups, gamma, beta, eps):  # NHWC fp64, from the definition
     return y * gamma.double() + beta.double()
 
 
-def _taps(x, stride, pad_lo, pad_hi):
-    """NHWC [n, h, w, c] -> [n * ho * wo, 9 * c]: the input window of each of the nine taps, tap-major (OHWI order)."""
+def _pad(x, pad_lo, pad_hi):
     n, h, w, ch = x.shape
     xp = torch.zeros(n, h + pad_lo + pad_hi, w + pad_lo + pad_hi, ch, dtype=x.dtype, device=x.device)
     xp[:, pad_lo:pad_lo + h, pad_lo:pad_lo + w] = x
-    ho, wo = h // stride, w // stride
-    cols = [xp[:, ty:ty + stride * (ho - 1) + 1:stride, tx:tx + stride * (wo - 1) + 1:stride]
+    return xp
+
+
+def _taps_band(xp, stride, y0, y1, wo):
+    """Padded NHWC image [h', w', c] -> the operand rows of output rows y0 <= y < y1, [(y1 - y0) * wo, 9 * c]: the
+    input window of each of the nine taps, tap-major (OHWI order)."""
+    cols = [xp[ty + stride * y0:ty + stride * (y1 - 1) + 1:stride, tx:tx + stride * (wo - 1) + 1:stride]
             for ty in range(3) for tx in range(3)]
-    return torch.cat(cols, -1).reshape(n * ho * wo, 9 * ch)
+    return torch.cat(cols, -1).reshape((y1 - y0) * wo, 9 * xp.shape[-1])
+
+
+def _row_chunks(m, k, unit, per_image, elems=1 << 26):
+    """[r0, r1) ranges covering m operand rows, each a multiple of `unit` rows inside one block of `per_image` rows,
+    with at most ~elems operand elements (fp64: 512 MB) so that the 1024^2 maps' references fit beside the model."""
+    step = max(unit, elems // max(1, k) // unit * unit)
+    return [(r0, min(i0 + per_image, r0 + step)) for i0 in range(0, m, per_image)
+            for r0 in range(i0, i0 + per_image, step)]
 
 
 def _chunks(lo, ch):
@@ -154,8 +169,9 @@ def _chunks(lo, ch):
 
 
 def _operands(c, t):
-    """(A, |A| for the bound, W, k-blocks): fp64 operand [M, K], weights [N, K] and the column range of each 64-channel
-    k-block of the kernel's main loop."""
+    """(rows, W, k-blocks, chunks): rows(r0, r1) -> (A, |A| for the bound), rows [r0, r1) of the fp64 operand [M, K];
+    the weights [N, K]; the column range of each 64-channel k-block of the kernel's main loop; the row ranges
+    (_row_chunks) to evaluate the reference in."""
     c0, c1 = c["c0"], c["c1"]
     cin = c0 + c1
     x = t["x"].double() if t["x1"] is None else torch.cat([t["x"], t["x1"]], -1).double()
@@ -173,33 +189,45 @@ def _operands(c, t):
         x = x.repeat_interleave(2, 1).repeat_interleave(2, 2)
         mag = mag.repeat_interleave(2, 1).repeat_interleave(2, 2)
     per_tap = _chunks(0, c0) + _chunks(c0, c1)
+    w = t["w"].double()
     if c["op"] == "linear" or c["taps"] == 1:
         a, am = x.reshape(-1, cin), mag.reshape(-1, cin)
-        blocks = per_tap
-    else:
-        pad = (0, 1) if c["pad_after"] else (1, 1)
-        a, am = _taps(x, c["stride"], *pad), _taps(mag, c["stride"], *pad)
-        blocks = [(tap * cin + lo, tap * cin + hi) for tap in range(9) for lo, hi in per_tap]
-        if c["c2"]:
-            s = t["s0"].double() if t["s1"] is None else torch.cat([t["s0"], t["s1"]], -1).double()
-            s = s.reshape(a.shape[0], -1)
-            a, am = torch.cat([a, s], 1), torch.cat([am, s.abs()], 1)
-            blocks += _chunks(9 * cin, c["c2"]) + _chunks(9 * cin + c["c2"], c["c3"])
-    return a, am, t["w"].double(), blocks
+        m = a.shape[0]
+        return (lambda r0, r1: (a[r0:r1], am[r0:r1])), w, per_tap, _row_chunks(m, cin, 1, m)
+    pad = (0, 1) if c["pad_after"] else (1, 1)
+    xp, mp = _pad(x, *pad), _pad(mag, *pad)
+    stride = c["stride"]
+    ho, wo = x.shape[1] // stride, x.shape[2] // stride
+    blocks = [(tap * cin + lo, tap * cin + hi) for tap in range(9) for lo, hi in per_tap]
+    s = None
+    if c["c2"]:
+        s = t["s0"].double() if t["s1"] is None else torch.cat([t["s0"], t["s1"]], -1).double()
+        s = s.reshape(x.shape[0] * ho * wo, -1)
+        blocks += _chunks(9 * cin, c["c2"]) + _chunks(9 * cin + c["c2"], c["c3"])
+
+    def rows(r0, r1):  # whole output rows of one image (_row_chunks with unit wo, per_image ho * wo)
+        img, y0 = divmod(r0 // wo, ho)
+        y1 = y0 + (r1 - r0) // wo
+        a, am = _taps_band(xp[img], stride, y0, y1, wo), _taps_band(mp[img], stride, y0, y1, wo)
+        if s is not None:
+            a, am = torch.cat([a, s[r0:r1]], 1), torch.cat([am, s[r0:r1].abs()], 1)
+        return a, am
+
+    return rows, w, blocks, _row_chunks(x.shape[0] * ho * wo, w.shape[1], wo, ho * wo)
 
 
 def _gelu(x):
     return 0.5 * x * (1.0 + torch.special.erf(x * 2.0 ** -0.5))
 
 
-def _epilogue(c, t, acc, bound):
-    """fp64 epilogue of the launch: (ref, B, the value before the residual)."""
+def _epilogue(c, t, acc, bound, r0=0):
+    """fp64 epilogue of the launch's rows r0 <= r < r0 + len(acc): (ref, B, the value before the residual)."""
     m = acc.shape[0]
     y, b = acc, bound
     if t["bias"] is not None:
         bias = t["bias"].double()
         if t["bias_rows"]:
-            bias = bias[torch.arange(m, device=acc.device) // t["bias_rows"], : c["n"]]
+            bias = bias[torch.arange(r0, r0 + m, device=acc.device) // t["bias_rows"], : c["n"]]
         y, b = y + bias, b + bias.abs()
     if c["act"]:
         y = {1: lambda v: v * torch.sigmoid(v), 2: _gelu, 3: lambda v: v * torch.sigmoid(1.702 * v)}[c["act"]](y)
@@ -209,17 +237,19 @@ def _epilogue(c, t, acc, bound):
         y, b = va * _gelu(gate), _gelu(gate).abs() * b[:, 0::2] + ACT_LIP * va.abs() * b[:, 1::2]
     pre = y
     if t["res"] is not None:
-        r = t["res"].double().reshape(m, -1)
+        r = t["res"].reshape(-1, y.shape[1])[r0:r0 + m].double()
         y, b = y + r, b + r.abs()
     return y, b, pre
 
 
-def _tolerance(c, plan, ref, bound, pre):
+def _tolerance(c, plan, ref, bound, pre, bf16=False):
     tau = TAU_NORM if (c["gn"] or c["ln"]) else TAU
     if c["f32"]:
         return tau * bound
     staged = plan["variant"] == 5 or plan.get("halo_kind") == 0
     scale = ref.abs() + (pre.abs() if staged and c["residual"] else 0.0)
+    if bf16:
+        return R_OUT_BF16 * scale + (1.0 + R_OUT_BF16) * tau * bound
     return R_OUT_F16 * scale + tau * bound
 
 
@@ -228,31 +258,41 @@ def _plan(lib, c):
 
 
 def _check(what, c, t, plan, out, chan, rows):
-    """Compare one launch's outputs with the fp64 reference; returns the worst err / tol."""
-    a, am, w, blocks = _operands(c, t)
-    acc = a @ w.t()
-    bound0 = am @ w.abs().t()
-    ref, bound, pre = _epilogue(c, t, acc, bound0)
-    tol = _tolerance(c, plan, ref, bound, pre)
-    got = out.double().reshape(ref.shape)
-    err = (got - ref).abs()
-    bad = err > tol
-    worst = (err / tol).max().item()
-    if bad.any():
-        idx = torch.nonzero(bad)
-        r, col = idx[0].tolist()
-        raise AssertionError(f"{what} ({plan}): {int(bad.sum())}/{bad.numel()} elements out of tolerance, worst err/tol "
-                             f"{worst:.3g}; rows {sorted(set(idx[:, 0].tolist()))[:8]}, columns "
-                             f"{sorted(set(idx[:, 1].tolist()))[:8]}; first at ({r}, {col}): got {got[r, col].item():.6g} "
-                             f"ref {ref[r, col].item():.6g} tol {tol[r, col].item():.3g}")
-
-    # the bound must see one missing 64-channel k-block: the first one and the last (ragged) one
+    """Compare one launch's outputs with the fp64 reference, a band of rows at a time; returns the worst err / tol."""
+    a_rows, w, blocks, chunks = _operands(c, t)
+    bf16 = t.get("bf16", False)
+    wt, wabs = w.t(), w.abs().t()
+    got_all = out.double().reshape(chunks[-1][1], -1)
+    worst = 0.0
+    seen = {"first": False, "last": False}
+    for r0, r1 in chunks:
+        a, am = a_rows(r0, r1)
+        acc = a @ wt
+        bound0 = am @ wabs
+        ref, bound, pre = _epilogue(c, t, acc, bound0, r0)
+        tol = _tolerance(c, plan, ref, bound, pre, bf16)
+        got = got_all[r0:r1]
+        err = (got - ref).abs()
+        bad = err > tol
+        worst = max(worst, (err / tol).max().item())
+        if bad.any():
+            idx = torch.nonzero(bad)
+            r, col = idx[0].tolist()
+            raise AssertionError(f"{what} ({plan}): {int(bad.sum())}/{bad.numel()} elements of rows [{r0}, {r1}) out of "
+                                 f"tolerance, worst err/tol {(err / tol).max().item():.3g}; rows "
+                                 f"{sorted(set((idx[:, 0] + r0).tolist()))[:8]}, columns "
+                                 f"{sorted(set(idx[:, 1].tolist()))[:8]}; first at ({r0 + r}, {col}): got "
+                                 f"{got[r, col].item():.6g} ref {ref[r, col].item():.6g} tol {tol[r, col].item():.3g}")
+        # the bound must see one missing 64-channel k-block: the first one and the last (ragged) one
+        for which, (lo, hi) in (("first", blocks[0]), ("last", blocks[-1])):
+            if not seen[which]:
+                miss = _epilogue(c, t, acc - a[:, lo:hi] @ w[:, lo:hi].t(), bound0, r0)[0]
+                seen[which] = bool(((miss - ref).abs() > tol).any())
     for which, (lo, hi) in (("first", blocks[0]), ("last", blocks[-1])):
-        miss = _epilogue(c, t, acc - a[:, lo:hi] @ w[:, lo:hi].t(), bound0)[0]
-        assert ((miss - ref).abs() > tol).any(), f"{what}: tolerance cannot see the {which} k-block [{lo}, {hi}) missing"
+        assert seen[which], f"{what}: tolerance cannot see the {which} k-block [{lo}, {hi}) missing"
 
     if rows is not None:
-        o = out.double().reshape(ref.shape[0], -1)
+        o = got_all
         s = rows.double().sum(0)
         assert ((s[:, 0] - o.sum(1)).abs() <= STAT_REL * o.abs().sum(1) + 1e-6).all(), f"{what}: row sums"
         assert ((s[:, 1] - (o * o).sum(1)).abs() <= STAT_REL * (o * o).sum(1) + 1e-6).all(), f"{what}: row sums of squares"
@@ -313,7 +353,8 @@ class _Replay:
 
     def _record(self, c, t, out, st, rs):
         c["stats"] = st is not None and "chan" in st
-        plan = G.parse_plan(self.lib.describe_plan(**G.describe_kwargs(c)))
+        t["bf16"] = t["x"].dtype == torch.bfloat16
+        plan = G.parse_plan(self.lib.describe_plan(**G.describe_kwargs(c), bf16=t["bf16"]))
         torch.cuda.synchronize()
         kind = "linear" if c["op"] == "linear" else ("conv1x1" if c["taps"] == 1 else "conv3x3")
         k = c["c0"] + c["c1"]
@@ -326,7 +367,7 @@ class _Replay:
         calls, w0 = self.plans.get(key, (0, 0.0))
         self.plans[key] = (calls + 1, max(w0, worst))
 
-    def linear(self, x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=torch.float16, split_k=0,
+    def linear(self, x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=None, split_k=0,
                block_n=0, bias_rows=0, bias_stride=0, out=None, static_w=False, act=0, ln=None, stats=None, cs_hw=0,
                rowstats=None):
         m, n = x.shape[0], wgt.shape[0]
@@ -343,7 +384,7 @@ class _Replay:
         self._record(c, t, y, stats, rowstats)
         return y
 
-    def conv3x3(self, x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=torch.float16, split_k=0,
+    def conv3x3(self, x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=None, split_k=0,
                 block_n=0, bias_rows=0, bias_stride=0, out=None, act=0, static_w=True, pad_after_only=False,
                 halo=False, gn=None, upsample=False, stats=None, rowstats=None, taps=9, shortcut=None):
         nimg, h, w, c0 = x.shape
@@ -376,16 +417,17 @@ class _Replay:
         return "\n".join(lines)
 
 
-@pytest.mark.parametrize("name", ["sd21_b2", "sd21_b16", "sd15_b2", "sdxl_768_b2", "controlnet_sd21", "vae_decoder",
-                                  "openclip_h", "clip_l", "sd21_b2_fused", "sd21_b2_halo_tma"])
+MODELS = MC.SHIPPED + ["sd21_b2_fused", "sd21_b2_halo_tma"]
+
+
+@pytest.mark.parametrize("name", MODELS)
 def test_model_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
-    """SD-2.1-base UNet at batch 2 and 16 (the benchmark's 8 prompts per GPU), SD-1.5, SDXL-base at 768^2, the SD-2.1
-    ControlNet, the VAE decoder 64 -> 512 and both CLIP text encoders from random-init weights; SD-2.1 twice more with
-    the opt-in halo convolutions: B200SD_FUSED=1 (GroupNorm + SiLU in the halo kernel's operand path, kinds 0 / 1) and
-    B200SD_HALO_TMA=1024 (plain convolutions on maps of >= 1024 pixels with TMA patches, kind 2).  Under B200SD_FUSED=1
-    every convolution behind a GroupNorm takes the GroupNorm-fused kernel, so B200SD_HALO_TMA has nothing left to take
-    there: kind 2 needs the run of its own.  Prints one line per distinct plan (run with -s); GEMM_PLANS.md holds
-    these tables as measured on an H100."""
+    """Every model of model_cases.SHIPPED from random-init weights (the bf16 VAEs against the bf16 output bound); SD-2.1
+    twice more with the opt-in halo convolutions: B200SD_FUSED=1 (GroupNorm + SiLU in the halo kernel's operand path,
+    kinds 0 / 1) and B200SD_HALO_TMA=1024 (plain convolutions on maps of >= 1024 pixels with TMA patches, kind 2).
+    Under B200SD_FUSED=1 every convolution behind a GroupNorm takes the GroupNorm-fused kernel, so B200SD_HALO_TMA has
+    nothing left to take there: kind 2 needs the run of its own.  Prints one line per distinct plan and the wall time
+    of the build, forward and checks (run with -s); GEMM_PLANS.md holds these tables as measured on an H100."""
     lib = cuda_lib
     for k in ("B200SD_CLUSTER_SPLITK", "B200SD_STAGED", "B200SD_FUSED", "B200SD_HALO_TMA"):
         monkeypatch.delenv(k, raising=False)
@@ -394,13 +436,14 @@ def test_model_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
         monkeypatch.setenv("B200SD_HALO_TMA", "1024")
     if name.endswith("_halo_tma"):
         monkeypatch.setenv("B200SD_HALO_TMA", "1024")
+    t0 = time.perf_counter()
     m = MC.build(name)
     rep = _Replay(lib, name)
     monkeypatch.setattr(lib, "linear", rep.linear)
     monkeypatch.setattr(lib, "conv3x3", rep.conv3x3)
     m(**MC.model_inputs(m, seed=9))
     torch.cuda.synchronize()
-    print("\n" + rep.report())
+    print(f"\n{rep.report()}\n  wall time {time.perf_counter() - t0:.1f} s")
     assert rep.plans, f"{name}: no GEMM / convolution launch was seen"
     halo = {(key[8], key[9]) for key in rep.plans}  # (halo_kind, GroupNorm fused)
     if name.endswith("_fused"):  # the opt-in paths this run exists for were taken

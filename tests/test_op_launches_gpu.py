@@ -37,6 +37,7 @@ embedding with its frequency table shifted by one; latent_prep without its last 
 Run with -s for one line per distinct (op, shape, dtype, path) with its launch count and worst err / tol."""
 import os
 import sys
+import time
 
 import pytest
 import torch
@@ -207,25 +208,31 @@ class _Replay:
         return "\n".join(lines)
 
 
-MODELS = ["sd21_b2", "sd21_b16", "sd15_b2", "sdxl_768_b2", "controlnet_sd21", "vae_decoder", "openclip_h", "clip_l",
-          "sd21_768_b2", "vae_decoder_bf16", "vae_encoder_bf16", "openclip_bigg", "sd21_b2_fused2"]
+MODELS = MC.SHIPPED + ["sd21_b2_fused2"]
+
+
+def _gn_channels(rows):
+    """Total channels of every GroupNorm row of a report (shape key (n, h, w, C0 or "C0+C1", groups))."""
+    return {sum(int(c) for c in str(key[1][3]).split("+")) for key in rows if key[0].startswith("group_norm")}
 
 
 @pytest.mark.parametrize("name", MODELS)
 def test_model_op_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
-    """One eager forward of each model of model_cases.py (sd21_b2_fused2: SD-2.1 under B200SD_FUSED=2, where
-    group_norm_apply normalises from the producers' channel sums), every wrapped launch checked."""
+    """One eager forward of each model of model_cases.SHIPPED (sd21_b2_fused2: SD-2.1 under B200SD_FUSED=2, where
+    group_norm_apply normalises from the producers' channel sums), every wrapped launch checked.  Prints the table and
+    the wall time of the build, forward and checks (run with -s)."""
     lib = cuda_lib
     for k in ("B200SD_CLUSTER_SPLITK", "B200SD_STAGED", "B200SD_FUSED", "B200SD_HALO_TMA"):
         monkeypatch.delenv(k, raising=False)
     if name.endswith("_fused2"):
         monkeypatch.setenv("B200SD_FUSED", "2")
+    t0 = time.perf_counter()
     m = MC.build(name[: -len("_fused2")] if name.endswith("_fused2") else name)
     rep = _Replay(lib, name)
     rep.install(monkeypatch)
     m(**MC.model_inputs(m, seed=9))
     torch.cuda.synchronize()
-    print("\n" + rep.report())
+    print(f"\n{rep.report()}\n  wall time {time.perf_counter() - t0:.1f} s")
     ops = {key[0] for key in rep.rows}
     assert rep.rows, f"{name}: no launch was seen"
     if name.startswith(("sd", "controlnet")):
@@ -233,16 +240,30 @@ def test_model_op_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
         assert {"attention", gn, "linear_small", "timestep_embedding"} <= ops, sorted(ops)
     if name.startswith("vae_decoder"):
         assert {"group_norm", "softmax_rows", "latent_prep", "upsample2x"} <= ops, sorted(ops)
+    if name.startswith("vae_encoder"):
+        assert {"group_norm", "softmax_rows"} <= ops, sorted(ops)
     if name.startswith(("openclip", "clip")):
         assert {"attention", "layer_norm", "embed_tokens"} <= ops, sorted(ops)
+    # the shapes each new case exists for
+    if name.startswith("sdxl_refiner"):  # groups of 12, 36 and 96 channels: none a whole number of 8-channel vectors
+        assert {384, 1152, 3072} <= _gn_channels(rep.rows), sorted(_gn_channels(rep.rows))
+        assert {key[1][4] for key in rep.rows if key[0] == "attention"} == {64}
+    if name == "controlnet_sd15":
+        assert {key[1][4] for key in rep.rows if key[0] == "attention"} == {40, 80, 160}
+    if name.endswith("_768") and name.startswith("vae_decoder"):
+        assert any(key[0] == "softmax_rows" and key[1][1] == 96 * 96 for key in rep.rows)
+        assert any(key[0] == "group_norm" and key[1][1:3] == (768, 768) for key in rep.rows)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # Synthetic edge cases the models do not reach.
 # ---------------------------------------------------------------------------------------------------------------------
 def _gn_input(g, n, hw, c, groups, rho, dt, dev="cuda"):
-    """randn + a per-group offset of +-rho (so |mu| / sigma ~ rho) + a spatial ramp (pixel range errors show)."""
-    off = rho * torch.randn(groups, generator=g, device=dev).sign().repeat_interleave(c // groups)
+    """randn + a per-group offset of +-rho (so |mu| / sigma ~ rho), alternating in sign so that every group boundary
+    separates offsets 2 rho apart (a boundary moved by 8 channels shows at any group width) + a spatial ramp (pixel
+    range errors show)."""
+    sign = 1.0 - 2.0 * (torch.arange(groups, device=dev) % 2)
+    off = (rho * sign).repeat_interleave(c // groups)
     ramp = torch.linspace(-1.0, 1.0, hw, device=dev)[None, :, None]
     return (torch.randn(n, hw, c, generator=g, device=dev) + off + ramp).to(dt)
 
@@ -266,11 +287,12 @@ def _gn_run(lib, x, c0, h, w, groups, silu, dt, rho, drop_px, expect_launches, g
     ref, tol = OR.group_norm(xd, gamma, beta, groups, 1e-5, silu, dt)
     w_ = OR.worst(y.reshape(n, hw, c), ref, tol)
     assert w_ <= 1.0, f"GroupNorm n={n} hw={hw} C={c0}+{c - c0} groups={groups} rho={rho} {dt}: err/tol {w_:.3g}"
-    probes = [OR.gn_stats(xd, groups, px=slice(0, hw - drop_px))] if drop_px else []
+    probes = [("last pixels missing", OR.gn_stats(xd, groups, px=slice(0, hw - drop_px)))] if drop_px else []
     if groups > 1:
-        probes.append(OR.gn_stats(xd, groups, shift=8))
-    for st in probes:
-        assert OR.rejects(OR.group_norm(xd, gamma, beta, groups, 1e-5, silu, dt, stats=st)[0], ref, tol)
+        probes.append(("groups shifted by 8 channels", OR.gn_stats(xd, groups, shift=8)))
+    for what, st in probes:
+        assert OR.rejects(OR.group_norm(xd, gamma, beta, groups, 1e-5, silu, dt, stats=st)[0], ref, tol), \
+            f"GroupNorm n={n} hw={hw} C={c} groups={groups}: the bound cannot see {what}"
     return w_
 
 
@@ -284,11 +306,15 @@ def _fallback_last_chunk(hw):
 
 @pytest.mark.parametrize("dt", [F16, BF16])
 @pytest.mark.parametrize("groups,c,hw", [(1, 520, 1039), (1, 520, 2049), (1, 520, 2048), (2, 1040, 1039),
-                                         (2, 1040, 2049), (2, 1040, 2048)])
+                                         (2, 1040, 2049), (2, 1040, 2048), (2, 3072, 1039), (2, 3072, 2049),
+                                         (32, 3072, 8193)])
 def test_group_norm_fallback_empty_chunks(cuda_lib, dt, groups, c, hw):
     """A chunk of > 512 channels is refused by the cluster planner, so these run the two-kernel fallback.  hw = 1039:
     64 chunks of 17 pixels, the last two empty; hw = 2049: 128 chunks of 17, the last seven empty; hw = 2048: 128 full
-    chunks (the control).  2 images, then 5: the ticket counters reset themselves between launches."""
+    chunks (the control).  C = 3072 is the SDXL refiner's widest concatenation (1536 + 1536), 384 vectors per pixel:
+    the most the fallback takes.  At 32 groups of 96 channels and hw = 8193 the cluster path is refused for its slab
+    (1025 rows x 192 B > 200 KB at cluster size 8, 2 at 5 images) and the fallback runs 128 chunks of 65 pixels, the
+    last one empty.  2 images, then 5: the ticket counters reset themselves between launches."""
     lib = cuda_lib
     g = torch.Generator(device="cuda").manual_seed(hw + groups)
     for n in (2, 5):
@@ -308,18 +334,33 @@ CLUSTER_CASES = [
     (1280, 0, 15, 17, 6),      # cs 2, deep; ragged (128 + 127 rows)
     (1280, 0, 16, 16, 16),     # cs 1, deep; batch 16
     (320, 0, 6, 6, 2),         # cs 1, 2 rows in flight
+    # the SDXL refiner's geometries: groups of 12, 36, 96 and 72 channels, none a whole number of 8-channel vectors
+    (384, 0, 128, 128, 2),     # chunk 48 (lcm(12, 8) = 24, doubled to >= 32), 6 vectors: 2048 rows per CTA at cs 8 make
+                               # a 213 KB slab > 200 KB, so the planner refuses it: the fallback (cs 0, two launches)
+    (768, 384, 64, 64, 2),     # cs 8, deep; chunk 72 = lcm(36, 8), 9 vectors, 28 rows x 9 = 252 of 256 threads
+    (1536, 1536, 32, 32, 2),   # cs 8, deep; C = 3072, chunk 96, 12 vectors, 21 rows x 12 = 252 threads
+    (1536, 768, 16, 16, 2),    # cs 8, 2 rows in flight; C = 2304, chunk 72, 32 rows per CTA
+    (1536, 1536, 12, 12, 2),   # cs 4, 2 rows in flight; the refiner's lowest level at 768^2 (hw / 8 = 18 < 32)
+    (1536, 1536, 32, 32, 16),  # 512 clusters: cs 1, whose 1024-row slab (209 KB) is refused: the fallback at C = 3072,
+                               # 384 vectors, one row: 48 KB of dynamic shared memory beside the kernel's static ticket
+                               # (the refiner at 1024^2, 8 images per call)
 ]
-CLUSTER_SIZE = [8, 8, 8, 4, 4, 2, 1, 1]
+CLUSTER_SIZE = [8, 8, 8, 4, 4, 2, 1, 1, 0, 8, 8, 8, 4, 0]
 
 
 @pytest.mark.parametrize("dt", [F16, BF16])
 @pytest.mark.parametrize("case", range(len(CLUSTER_CASES)))
 def test_group_norm_cluster_shapes(cuda_lib, dt, case):
+    """Cluster size 0: the planner refuses the cluster kernel and the two-kernel fallback runs; its probe drops the last
+    statistics chunk's pixels."""
     lib = cuda_lib
     c0, c1, h, w, n = CLUSTER_CASES[case]
     cs, hw, c = CLUSTER_SIZE[case], h * w, c0 + c1
     g = torch.Generator(device="cuda").manual_seed(case)
     x = _gn_input(g, n, hw, c, 32, 3.0, dt)
+    if cs == 0:
+        _gn_run(lib, x, c0, h, w, 32, case % 2 == 0, dt, 3.0, _fallback_last_chunk(hw), 2)
+        return
     drop = hw - (cs - 1) * (-(-hw // cs)) if cs > 1 else 0  # the last CTA's pixels
     _gn_run(lib, x, c0, h, w, 32, case % 2 == 0, dt, 3.0, drop, 1)
 
