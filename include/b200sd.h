@@ -159,6 +159,18 @@ int b200sd_gemm_describe_plan_bf16(const b200sd_gemm_args* args, char* buf, size
 /* bytes of fp32 scratch b200sd_gemm would need for these args (0 if no split-K) */
 size_t b200sd_gemm_workspace_bytes(const b200sd_gemm_args* args);
 
+/* ---- W8A8 3x3 convolution (int8 wgmma, s32 accumulators) --------------------------------------
+ * a0: int8 NHWC [n_img, h, w, c0] (c0 a multiple of 16); wgt: int8 pre-tiled [n_tiles][k_blocks][block_n][128]
+ * (tap-major, each tap's channels zero padded to a multiple of 128; wgt_tiled = 1 and the planned block_n);
+ * col_scale: fp32 [n], s_a * s_w[col].  out[row, col] = fp16(float(acc) * col_scale[col] + bias + residual) with
+ * bias a vector or per-image rows (bias_rows) and an fp16 residual; split-K as b200sd_gemm.  Supports mode 1, stride 1,
+ * pad 1, one source; rejects mode 0, stride 2, pad_after_only, a1 / a2 / a3, geglu, act, out_f32, halo, upsample2x,
+ * gn_*, cs_*, rs_out and ln_* with an error naming the field. */
+int b200sd_gemm_s8(const b200sd_gemm_args* args, const float* col_scale, void* stream);
+int b200sd_gemm_plan_ex_s8(const b200sd_gemm_args* args, int32_t* out8);
+int b200sd_gemm_describe_plan_s8(const b200sd_gemm_args* args, char* buf, size_t buf_size);
+size_t b200sd_gemm_workspace_bytes_s8(const b200sd_gemm_args* args);
+
 /* small-M linear on CUDA cores (weight-bandwidth bound): out[m, n] = act_in(x[m, :]) . W[n, :] + b[n]
  * for the time-embedding MLPs (unet.py:665-682) and the per-ResNet time_emb_proj(silu(emb))
  * (unet.py:442, 476-478).  x, out fp32; W fp16 [n, k]; act_in: 0 none, 1 SiLU on the input;
@@ -184,6 +196,11 @@ int b200sd_group_norm_bf16(const void* x0, const void* x1, int32_t c0, int32_t c
                            int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
                            void* out, float* stats_ws, size_t stats_ws_bytes, void* stream);
 size_t b200sd_group_norm_workspace_bytes(int32_t n_img, int32_t hw, int32_t c, int32_t groups);
+/* b200sd_group_norm on fp16 sources whose output is the int8 operand of b200sd_gemm_s8: the fp32 normalised (+SiLU)
+ * value y is stored as q = clamp(rint(y * inv_scale), -127, 127) (inv_scale = 1 / s_a > 0). */
+int b200sd_group_norm_s8(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
+                         int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu, float inv_scale,
+                         void* out, float* stats_ws, size_t stats_ws_bytes, void* stream);
 /* GroupNorm (+SiLU, + concat) from PRODUCER-SIDE statistics: chan0 / chan1 are the per-channel (sum, sum of squares)
  * [n_img][c][2] a b200sd_gemm call left behind (cs_chan); no statistics pass, one read + one write of the tensor.  Used
  * where the consumer is not the halo convolution (which applies the normalisation in its own operand path). */
@@ -242,6 +259,12 @@ int b200sd_nhwc_to_nchw_f32(const void* in, int32_t in_f32, float* out, int32_t 
                             int32_t w, int32_t c_pad, void* stream);
 /* nearest x2 upsample NHWC fp16 (F.interpolate, unet.py:499); a byte copy, so bf16 tensors use it as well */
 int b200sd_upsample2x(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c, void* stream);
+/* nearest x2 upsample of fp16 NHWC into int8: q = clamp(rint(x * inv_scale), -127, 127) (b200sd_gemm_s8's operand) */
+int b200sd_upsample2x_s8(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c, float inv_scale,
+                         void* stream);
+/* W8A8 calibration probe: *slot = max(*slot, max |x|) over numel (even) fp16 values; deterministic (atomicMax on the
+ * bit pattern of non-negative floats).  *slot must start >= 0. */
+int b200sd_absmax_f16(const void* x, size_t numel, float* slot, void* stream);
 /* out = a + b (fp16; ControlNet residual injection unet.py:1009-1022) */
 int b200sd_add(const void* a, const void* b, void* out, size_t numel, void* stream);
 /* BC1S fp16/fp32 context (B, D, 1, S) -> token-major fp16 [B*S, D] */

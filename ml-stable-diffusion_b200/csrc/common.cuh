@@ -40,6 +40,9 @@ void set_error(const char* fmt, ...);
 // types are two bytes wide and the out-of-bounds zero fill (0x0000) is +0 in both.
 int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                     const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides);
+// The same encoding for any element type (UINT8 for the int8 convolution: its zero fill is 0 as well).
+int encode_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides);
 
 int num_sms();
 
@@ -260,6 +263,59 @@ B200SD_WGMMA_SS_BOTH(256,
 #undef B200SD_WGMMA_SS_BOTH
 #undef B200SD_WGMMA_SS
 
+// D[64 x N] (+)= A[64 x 32] * B[N x 32]^T with signed int8 operands (K-major, smem) and int32 accumulators: the same
+// 32-byte k step and the same accumulator layout as wgmma_ss<N> (IGMMA in SASS).
+template <int N>
+__device__ __forceinline__ void wgmma_ss_s8(int32_t* d, uint64_t da, uint64_t db, uint32_t acc);
+#define B200SD_I8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
+#define B200SD_WGMMA_S8(N, REGS, IP, IA, IB, ...)                                                                    \
+    template <>                                                                                                      \
+    __device__ __forceinline__ void wgmma_ss_s8<N>(int32_t* d, uint64_t da, uint64_t db, uint32_t acc) {             \
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IP ", 0;\n\t"                                          \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.s8.s8 {" REGS "}, %" #IA ", %" #IB ", p;\n\t}\n"  \
+                     : __VA_ARGS__                                                                                   \
+                     : "l"(da), "l"(db), "r"(acc)                                                                    \
+                     : "memory");                                                                                    \
+    }
+#define B200SD_R16 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define B200SD_R32 B200SD_R16 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define B200SD_R64 B200SD_R32 ", %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define B200SD_R96 B200SD_R64 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define B200SD_R128 B200SD_R96 ", %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define B200SD_R160 B200SD_R128 ", %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define B200SD_R192 B200SD_R160 ", %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define B200SD_R256 B200SD_R192 ", %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, " \
+    "%111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+B200SD_WGMMA_S8(16, B200SD_R16, 10, 8, 9, B200SD_I8(0))
+B200SD_WGMMA_S8(32, B200SD_R32, 18, 16, 17, B200SD_I8(0), B200SD_I8(8))
+B200SD_WGMMA_S8(64, B200SD_R64, 34, 32, 33, B200SD_I8(0), B200SD_I8(8), B200SD_I8(16), B200SD_I8(24))
+B200SD_WGMMA_S8(96, B200SD_R96, 50, 48, 49, B200SD_I8(0), B200SD_I8(8), B200SD_I8(16), B200SD_I8(24), B200SD_I8(32),
+                B200SD_I8(40))
+B200SD_WGMMA_S8(128, B200SD_R128, 66, 64, 65, B200SD_I8(0), B200SD_I8(8), B200SD_I8(16), B200SD_I8(24), B200SD_I8(32),
+                B200SD_I8(40), B200SD_I8(48), B200SD_I8(56))
+B200SD_WGMMA_S8(160, B200SD_R160, 82, 80, 81, B200SD_I8(0), B200SD_I8(8), B200SD_I8(16), B200SD_I8(24), B200SD_I8(32),
+                B200SD_I8(40), B200SD_I8(48), B200SD_I8(56), B200SD_I8(64), B200SD_I8(72))
+B200SD_WGMMA_S8(192, B200SD_R192, 98, 96, 97, B200SD_I8(0), B200SD_I8(8), B200SD_I8(16), B200SD_I8(24), B200SD_I8(32),
+                B200SD_I8(40), B200SD_I8(48), B200SD_I8(56), B200SD_I8(64), B200SD_I8(72), B200SD_I8(80), B200SD_I8(88))
+B200SD_WGMMA_S8(256, B200SD_R256, 130, 128, 129, B200SD_I8(0), B200SD_I8(8), B200SD_I8(16), B200SD_I8(24), B200SD_I8(32),
+                B200SD_I8(40), B200SD_I8(48), B200SD_I8(56), B200SD_I8(64), B200SD_I8(72), B200SD_I8(80), B200SD_I8(88),
+                B200SD_I8(96), B200SD_I8(104), B200SD_I8(112), B200SD_I8(120))
+#undef B200SD_R256
+#undef B200SD_R192
+#undef B200SD_R160
+#undef B200SD_R128
+#undef B200SD_R96
+#undef B200SD_R64
+#undef B200SD_R32
+#undef B200SD_R16
+#undef B200SD_WGMMA_S8
+#undef B200SD_I8
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs_s32(int32_t* d) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
 // A from registers (fp16 pairs in the accumulator layout of a 64 x 16 tile), B [16 x 64] from smem, MN-major
 __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
     asm volatile(
@@ -379,6 +435,17 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 
 // The 16-bit activation types: fp16 everywhere, bf16 (fp32's exponent range) for the VAEs whose activations exceed
 // fp16's 65504.  Conversions in the form the fp16 kernels were written in, so their fp16 code is unchanged.
+// W8A8 activation quantization of eight fp32 values: q = clamp(rint(y * inv_scale), -127, 127), packed little-endian
+__device__ __forceinline__ uint2 quantize8_s8(const float (&f)[8], float inv_scale) {
+    uint32_t w[2] = {0u, 0u};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const int q = min(127, max(-127, __float2int_rn(f[e] * inv_scale)));
+        w[e >> 2] |= (static_cast<uint32_t>(q) & 0xffu) << (8 * (e & 3));
+    }
+    return make_uint2(w[0], w[1]);
+}
+
 template <typename T>
 struct Elem16;
 template <>

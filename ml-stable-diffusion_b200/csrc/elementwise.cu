@@ -4,6 +4,7 @@
 #include "../../include/b200sd.h"
 
 #include <algorithm>
+#include <cmath>
 
 namespace b200sd {
 
@@ -105,6 +106,55 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ in, uint4* __restric
         const int b = static_cast<int>(r / (2 * h));
         out[i] = in[((static_cast<size_t>(b) * h + (oy >> 1)) * w + (ox >> 1)) * vecs + v];
     }
+}
+
+// nearest x2 upsample of an fp16 NHWC tensor into the int8 operand of the W8A8 convolution: each source vector of eight
+// channels is quantized once (q = clamp(rint(x * inv_scale), -127, 127)) and written to its four output pixels
+__global__ void upsample2x_s8_kernel(const uint4* __restrict__ in, uint2* __restrict__ out, int n, int h, int w, int vecs,
+                                     float inv_scale) {
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
+    pdl_wait();
+    const size_t total = static_cast<size_t>(n) * h * w * vecs;
+    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const int v = static_cast<int>(i % vecs);
+        size_t r = i / vecs;
+        const int x = static_cast<int>(r % w);
+        r /= w;
+        const int y = static_cast<int>(r % h);
+        const int b = static_cast<int>(r / h);
+        const uint4 raw = in[i];
+        const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
+        float f[8];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const float2 t = __half22float2(h2[q]);
+            f[2 * q] = t.x;
+            f[2 * q + 1] = t.y;
+        }
+        const uint2 pk = quantize8_s8(f, inv_scale);
+        const size_t o = ((static_cast<size_t>(b) * 2 * h + 2 * y) * (2 * w) + 2 * x) * vecs + v;
+        out[o] = pk;
+        out[o + vecs] = pk;
+        out[o + static_cast<size_t>(2 * w) * vecs] = pk;
+        out[o + static_cast<size_t>(2 * w) * vecs + vecs] = pk;
+    }
+}
+
+// max |x| of an fp16 tensor folded into *slot: a non-negative float orders like its bit pattern, so atomicMax on the
+// bits gives the same result in any order (W8A8 calibration)
+__global__ void absmax_f16_kernel(const __half2* __restrict__ x, size_t n2, unsigned int* __restrict__ slot) {
+    pdl_trigger();
+    pdl_wait();
+    float m = 0.f;
+    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n2;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const float2 f = __half22float2(x[i]);
+        m = fmaxf(m, fmaxf(fabsf(f.x), fabsf(f.y)));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(slot, __float_as_uint(m));
 }
 
 __global__ void add_kernel(const __half2* __restrict__ a, const __half2* __restrict__ b, __half2* __restrict__ out,
@@ -428,6 +478,33 @@ extern "C" int b200sd_upsample2x(const void* in, void* out, int32_t n, int32_t h
     const size_t total = static_cast<size_t>(n) * 4 * h * w * (c / 8);
     B200SD_CHECK_CUDA(launch_kernel(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream, reinterpret_cast<const uint4*>(in),
                                                                 reinterpret_cast<uint4*>(out), n, h, w, c / 8));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_upsample2x_s8(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c, float inv_scale,
+                                    void* stream_) {
+    if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(in && out && c % 8 == 0, "b200sd_upsample2x_s8: c=%d must be a multiple of 8", c);
+    B200SD_REQUIRE(std::isfinite(inv_scale) && inv_scale > 0.f, "b200sd_upsample2x_s8: inv_scale=%g must be positive and finite",
+                   static_cast<double>(inv_scale));
+    const size_t total = static_cast<size_t>(n) * h * w * (c / 8);
+    B200SD_CHECK_CUDA(launch_kernel(upsample2x_s8_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream,
+                                    reinterpret_cast<const uint4*>(in), reinterpret_cast<uint2*>(out), n, h, w, c / 8, inv_scale));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_absmax_f16(const void* x, size_t numel, float* slot, void* stream_) {
+    if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(x && slot && numel % 2 == 0, "b200sd_absmax_f16: bad arguments (numel=%zu must be even)", numel);
+    B200SD_CHECK_CUDA(launch_kernel(absmax_f16_kernel, dim3(std::min(grid_for(numel / 2, 256), 1024)), dim3(256), 0,
+                                    stream, reinterpret_cast<const __half2*>(x), numel / 2,
+                                    reinterpret_cast<unsigned int*>(slot)));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;

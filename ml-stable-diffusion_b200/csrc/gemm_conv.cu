@@ -101,6 +101,7 @@ struct __align__(64) GemmParams {
     int staged;                // staged epilogue (fp16 tile in shared memory, coalesced row-wise stores)
     int stage_dedicated;       // the staging tile has its own shared memory (persistent CTAs with several tiles)
     long long* dbg;            // optional timeline of CTA 0 (clock64 at fixed points; tools/halo_timeline.py)
+    const float* col_scale;    // int8 convolution: [N] s_a * s_w[n], applied to the int32 accumulators
 };
 
 struct TileCoord {
@@ -584,6 +585,35 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, float (&acc)[
     if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
 }
 
+// gemm_mainloop for int8 operands: a 128-byte k-block is 128 channels, four m64nkBNk32 steps, int32 accumulators.
+template <int kBN>
+__device__ __forceinline__ void gemm_mainloop_s8(const GemmParams& p, int32_t (&acc)[kBN / 2], const uint8_t* smem_a,
+                                                 const uint8_t* smem_b, uint64_t* full_bar, uint64_t* empty_bar, int kb0,
+                                                 int kb1, int& stage, uint32_t& phase, int wg, bool leader) {
+    constexpr int b_stage = kBN * kBK * 2;
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smem_a + stage * kAStage + wg * (kAStage / 2)), 1024, 0);
+        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + stage * b_stage), 1024, 0);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            wgmma_ss_s8<kBN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == p.stages) {
+            stage = 0;
+            phase ^= 1;
+        }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs_s32<kBN / 2>(acc);
+    if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+}
+
 // Accumulator fragment of a consumer thread -> fp32 tile in shared memory, row-major with row stride `ld` floats
 // (the layout the row-wise epilogue and the cluster split-K reduction read).
 template <int R>
@@ -691,8 +721,11 @@ __device__ __forceinline__ void cluster_splitk_reduce(const GemmParams& p, const
 
 // T: operand / 16-bit output type (__half; __nv_bfloat16 for the generic, plain and fp32-output variants only).
 // kBN: tile width (columns); p.block_n == kBN.  Each consumer thread holds kBN / 2 fp32 accumulators.
-template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN>
-__global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __grid_constant__ GemmParams p) {
+// kS8: int8 operands (k-block = 128 channels, int32 accumulators scaled by p.col_scale into the fp32 ones before the
+// epilogue); T is then the type of the residual and the output.
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN, bool kS8>
+__device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
+    constexpr int kChunk = kS8 ? 2 * kBK : kBK;  // channels per k-block (128 bytes either way)
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
     // integer-rounded pointer -- lets the compiler emit LDS / STS for everything derived from it; rounding through
     // uintptr_t turned every shared access of the loader and the epilogues into generic LD.E / ST.E
@@ -752,7 +785,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
                 const int tap = kb / p.kc;
                 const int j = kb - tap * p.kc;
                 const bool src1 = j >= p.kc0;
-                const int c = (src1 ? (j - p.kc0) : j) * kBK;
+                const int c = (src1 ? (j - p.kc0) : j) * kChunk;
                 const int wk = tap * p.Kpt + (src1 ? p.C0 : 0) + c;
                 void* dst_b = smem_b + st * b_stage;
                 const int brow = p.wgt_tiled ? (t.n_tile * p.kb_total + kb) * p.block_n : t.n_tile * p.block_n;
@@ -771,7 +804,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
                     tap = 4;
                 } else {
                     const bool src1 = j >= p.kc0;
-                    c = (src1 ? (j - p.kc0) : j) * kBK;
+                    c = (src1 ? (j - p.kc0) : j) * kChunk;
                     tmA = src1 ? &p.tmA1 : &p.tmA0;
                 }
                 void* dst_a = smem_a + st * kAStage;
@@ -859,8 +892,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
                 }
                 if (p.bias_rows > 0 && valid) bias_sel = min(1, max(0, out_row / p.bias_rows - img0));
             }
-            if (p.ln_parts != 0)
+            if constexpr (kS8) {  // the int8 convolution has no LayerNorm fold: its column scales take that vector
+                for (int c = tid_e; c < p.block_n; c += kEpiThreads) wg_s[c] = (ncol0 + c < p.N) ? p.col_scale[ncol0 + c] : 0.f;
+            } else if (p.ln_parts != 0) {
                 for (int c = tid_e; c < p.block_n; c += kEpiThreads) wg_s[c] = (ncol0 + c < p.N) ? p.ln_wg[ncol0 + c] : 0.f;
+            }
             uint4 res_pre[4];
             if (kStaged) staged_load_residual(p, t, staged_map(p, t, lane), warp, 0, res_pre);
             if (p.res_smem) {
@@ -874,7 +910,22 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
             }
             const int bias_base = (p.bias_mode == 2 && p.bias_rows > 0 && valid) ? (out_row / p.bias_rows) * p.bias_stride : 0;
 
-            gemm_mainloop<T, kBN>(p, acc, smem_a, smem_b, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
+            if constexpr (kS8) {
+                int32_t iacc[kBN / 2];
+                gemm_mainloop_s8<kBN>(p, iacc, smem_a, smem_b, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
+                epi_bar_sync();  // the column scales are in wg_s
+                const int cq = 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < kBN / 8; ++j) {
+                    const float s0 = wg_s[8 * j + cq], s1 = wg_s[8 * j + cq + 1];
+                    acc[4 * j] = static_cast<float>(iacc[4 * j]) * s0;
+                    acc[4 * j + 1] = static_cast<float>(iacc[4 * j + 1]) * s1;
+                    acc[4 * j + 2] = static_cast<float>(iacc[4 * j + 2]) * s0;
+                    acc[4 * j + 3] = static_cast<float>(iacc[4 * j + 3]) * s1;
+                }
+            } else {
+                gemm_mainloop<T, kBN>(p, acc, smem_a, smem_b, full_bar, empty_bar, kb0, kb1, stage, phase, wg, leader);
+            }
 
             if (p.res_smem) cp_async_wait_all();
             epi_bar_sync();  // every wgmma of the tile retired: the stages may be overwritten; staged operands visible
@@ -963,6 +1014,20 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
     }
 }
 
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN>
+__global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __grid_constant__ GemmParams p) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gemm_kernel_body<T, kGeneric, kGeglu, kOutF32, kPartial, kStaged, kBN, false>(p);
+}
+
+// W8A8 3x3 convolution (b200sd_gemm_s8): int8 NHWC activations and pre-tiled int8 weights on IGMMA, fp16 residual and
+// output.  Variants: generic, plain and split-K epilogues.
+template <bool kGeneric, bool kPartial, int kBN>
+__global__ void __launch_bounds__(kGemmThreads, 1) igmma_conv_kernel(const __grid_constant__ GemmParams p) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gemm_kernel_body<__half, kGeneric, false, false, kPartial, false, kBN, true>(p);
+}
+
 
 // Tile widths the GEMM kernel is compiled for; plan_gemm chooses among exactly these (widest first).
 static constexpr int kGemmWidths[] = {256, 192, 160, 128, 96, 64, 32, 16};
@@ -988,6 +1053,20 @@ static KernelFn gemm_kernel(int width_index) {
                                                  B200SD_GEMM_FN(128), B200SD_GEMM_FN(96),  B200SD_GEMM_FN(64),
                                                  B200SD_GEMM_FN(32),  B200SD_GEMM_FN(16)};
 #undef B200SD_GEMM_FN
+    return fns[width_index];
+}
+template <bool kGeneric, bool kPartial, int kBN>
+static constexpr KernelFn s8_fn() {
+    if constexpr (kBN == 16 && !kGeneric) return nullptr;  // the regular variants need block_n % 32 == 0
+    else return igmma_conv_kernel<kGeneric, kPartial, kBN>;
+}
+template <bool kGeneric, bool kPartial>
+static KernelFn s8_kernel(int width_index) {
+#define B200SD_S8_FN(bn) s8_fn<kGeneric, kPartial, bn>()
+    static const KernelFn fns[kNumGemmWidths] = {B200SD_S8_FN(256), B200SD_S8_FN(192), B200SD_S8_FN(160),
+                                                 B200SD_S8_FN(128), B200SD_S8_FN(96),  B200SD_S8_FN(64),
+                                                 B200SD_S8_FN(32),  B200SD_S8_FN(16)};
+#undef B200SD_S8_FN
     return fns[width_index];
 }
 
@@ -1572,7 +1651,28 @@ static int halo_pick_block_n(const b200sd_gemm_args& a) {
 // activations overflow fp16: modes 0 / 1, stride 1 / 2, pad_after_only, bias, residual, fp32 output and tiled weights,
 // on the generic, plain and fp32-output epilogues.  Everything else is rejected by name, and the plan never takes
 // split-K (workspace or cluster) or the staged epilogue, whatever the environment switches say.
-static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false) {
+// s8: the W8A8 convolution (b200sd_gemm_s8): int8 activations and weights, k-blocks of 128 channels.  It serves the
+// stride-1 pad-1 3x3 convolution of one source with a bias vector or per-image bias rows, an fp16 residual, fp16 output
+// and split-K; everything else is rejected by name.
+static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false, bool s8 = false) {
+    if (s8) {
+        B200SD_REQUIRE(a.mode == 1, "b200sd_gemm_s8: mode=%d is not supported (the 3x3 convolution, mode 1)", a.mode);
+        B200SD_REQUIRE(a.stride == 1, "b200sd_gemm_s8: stride=%d is not supported (1)", a.stride);
+        B200SD_REQUIRE(!a.pad_after_only, "b200sd_gemm_s8: pad_after_only is not supported");
+        B200SD_REQUIRE(!a.a1 && a.c1 == 0, "b200sd_gemm_s8: a1 (second source) is not supported");
+        B200SD_REQUIRE(!a.a2 && !a.a3 && a.c2 == 0 && a.c3 == 0, "b200sd_gemm_s8: a2 / a3 (folded shortcut) are not supported");
+        B200SD_REQUIRE(!a.geglu, "b200sd_gemm_s8: geglu is not supported");
+        B200SD_REQUIRE(a.act == 0, "b200sd_gemm_s8: act=%d is not supported", a.act);
+        B200SD_REQUIRE(!a.out_f32, "b200sd_gemm_s8: out_f32 is not supported (fp16 output)");
+        B200SD_REQUIRE(!a.halo, "b200sd_gemm_s8: halo is not supported");
+        B200SD_REQUIRE(!a.upsample2x, "b200sd_gemm_s8: upsample2x is not supported");
+        B200SD_REQUIRE(a.gn_groups == 0 && !a.gn_chan0 && !a.gn_chan1 && !a.gn_gamma && !a.gn_beta,
+                       "b200sd_gemm_s8: gn_* (fused GroupNorm) is not supported");
+        B200SD_REQUIRE(!a.cs_partial && !a.cs_chan && !a.cs_tickets, "b200sd_gemm_s8: cs_* (column statistics) are not supported");
+        B200SD_REQUIRE(!a.rs_out, "b200sd_gemm_s8: rs_out (row statistics) is not supported");
+        B200SD_REQUIRE(a.ln_parts == 0 && !a.ln_stat && !a.ln_wg, "b200sd_gemm_s8: ln_* (LayerNorm fold) is not supported");
+        B200SD_REQUIRE(a.c0 > 0 && a.c0 % 16 == 0, "b200sd_gemm_s8: c0=%d must be a positive multiple of 16 (TMA row stride)", a.c0);
+    }
     B200SD_REQUIRE(a.mode == 0 || a.mode == 1, "b200sd_gemm: bad mode %d", a.mode);
     if (bf16) {
         B200SD_REQUIRE(!a.geglu, "b200sd_gemm_bf16: geglu is not supported in bf16");
@@ -1593,8 +1693,9 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false)
     B200SD_REQUIRE(a.n > 0, "b200sd_gemm: n=%d", a.n);
     pl.N = a.n;
     pl.Kpt = a.c0 + a.c1;
-    pl.kc0 = (a.c0 + kBK - 1) / kBK;
-    pl.kc1 = (a.c1 + kBK - 1) / kBK;
+    const int chunk = s8 ? 2 * kBK : kBK;  // channels per 128-byte k-block
+    pl.kc0 = (a.c0 + chunk - 1) / chunk;
+    pl.kc1 = (a.c1 + chunk - 1) / chunk;
     pl.taps = a.mode == 1 ? 9 : 1;
     pl.kb_total = pl.taps * (pl.kc0 + pl.kc1) + (a.c2 + kBK - 1) / kBK + (a.c3 + kBK - 1) / kBK;
     B200SD_REQUIRE((a.c2 == 0 && a.c3 == 0) || (a.mode == 1 && a.stride == 1 && !a.halo && a.c2 > 0 && a.c2 % 8 == 0 && a.c3 % 8 == 0),
@@ -1727,7 +1828,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false)
     const int per_stage = kAStage + pl.block_n * kBK * 2;
     {
         // staged epilogue: fp16 tile in shared memory, row-contiguous residual reads / stores, statistics outputs
-        const bool eligible = !bf16 && regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
+        const bool eligible = !bf16 && !s8 && regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
         // column statistics need the staged epilogue; row statistics alone ride on the register epilogue (every thread
         // owns a row there), which keeps the residual tile prefetched in shared memory during the main loop
         pl.staged = (eligible && (a.cs_partial != nullptr || (a.residual != nullptr && staged_enabled()))) ? 1 : 0;
@@ -1779,10 +1880,12 @@ static size_t plan_workspace(const GemmPlan& pl) {
 
 extern void count_launch(int n);
 
-static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16) {
+static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16, const float* col_scale = nullptr) {
+    const bool s8 = col_scale != nullptr;
     GemmPlan pl;
-    if (int rc = plan_gemm(a, pl, bf16)) return rc;
+    if (int rc = plan_gemm(a, pl, bf16, s8)) return rc;
     B200SD_REQUIRE(a.a0 && a.wgt && a.out, "b200sd_gemm: null pointer");
+    B200SD_REQUIRE(!s8 || a.wgt_tiled, "b200sd_gemm_s8: the weights must be pre-tiled (wgt_tiled = 1, explicit block_n)");
     B200SD_REQUIRE(a.c1 == 0 || a.a1, "b200sd_gemm: a1 is null but c1 > 0");
     const size_t ws = plan_workspace(pl);
     B200SD_REQUIRE(ws == 0 || (a.workspace && a.workspace_bytes >= ws),
@@ -1826,6 +1929,15 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
         } else {
             p.tmA1 = p.tmA0;
         }
+    } else if (s8) {
+        // int8 NHWC source: a box is 128 channels (128 bytes, one swizzle row), the channel tail is zero filled
+        const uint32_t box[4] = {2 * kBK, static_cast<uint32_t>(pl.bw), static_cast<uint32_t>(pl.bh),
+                                 static_cast<uint32_t>(pl.bn_img)};
+        const uint64_t c = static_cast<uint64_t>(a.c0);
+        const uint64_t dims[4] = {c, static_cast<uint64_t>(a.w), static_cast<uint64_t>(a.h), static_cast<uint64_t>(a.n_img)};
+        const uint64_t str[3] = {c, c * a.w, c * a.w * a.h};
+        if (int rc = encode_tmap(&p.tmA0, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.a0, 4, dims, str, box, es1)) return rc;
+        p.tmA1 = p.tmA2 = p.tmA3 = p.tmA0;
     } else {
         const uint32_t st = static_cast<uint32_t>(a.stride);
         const uint32_t box[4] = {kBK, static_cast<uint32_t>(pl.bw) * st, static_cast<uint32_t>(pl.bh) * st,
@@ -1848,7 +1960,14 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
             if (int rc = encode_tmap_f16(maps[src], ptrs[src], 4, dims, str, box, es)) return rc;
         }
     }
-    if (a.wgt_tiled) {
+    if (s8) {
+        B200SD_REQUIRE(a.block_n == pl.block_n, "b200sd_gemm_s8: tiled weights need an explicit block_n");
+        const uint64_t rows = static_cast<uint64_t>(pl.n_tiles) * pl.kb_total * pl.block_n;
+        const uint64_t dims[2] = {2 * kBK, rows};
+        const uint64_t str[1] = {2 * kBK};
+        const uint32_t box[2] = {2 * kBK, static_cast<uint32_t>(pl.block_n)};
+        if (int rc = encode_tmap(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.wgt, 2, dims, str, box, es1)) return rc;
+    } else if (a.wgt_tiled) {
         B200SD_REQUIRE(a.block_n == pl.block_n, "b200sd_gemm: tiled weights need an explicit block_n");
         const uint64_t rows = static_cast<uint64_t>(pl.n_tiles) * pl.kb_total * pl.block_n;
         const uint64_t dims[2] = {kBK, rows};
@@ -1953,7 +2072,15 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
     const int wi = gemm_width_index(pl.block_n);
     const int variant = pl.variant;
     KernelFn fn = nullptr;
-    if (bf16) {  // plan_gemm gives bf16 only these three variants
+    p.col_scale = col_scale;
+    if (s8) {  // plan_gemm gives int8 only these three variants
+        switch (variant) {
+            case kVariantGeneric: fn = s8_kernel<true, false>(wi); break;
+            case kVariantSplitK: fn = s8_kernel<false, true>(wi); break;
+            case kVariantPlain: fn = s8_kernel<false, false>(wi); break;
+            default: break;
+        }
+    } else if (bf16) {  // plan_gemm gives bf16 only these three variants
         switch (variant) {
             case kVariantGeneric: fn = gemm_kernel<__nv_bfloat16, true, false, false, false, false>(wi); break;
             case kVariantF32: fn = gemm_kernel<__nv_bfloat16, false, false, true, false, false>(wi); break;
@@ -1970,17 +2097,18 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
             default: fn = gemm_kernel<__half, false, false, false, false, false>(wi); break;
         }
     }
-    B200SD_REQUIRE(fn != nullptr, "b200sd_gemm: no %s kernel for variant %d at block_n %d", bf16 ? "bf16" : "fp16", variant,
-                   pl.block_n);
+    B200SD_REQUIRE(fn != nullptr, "b200sd_gemm: no %s kernel for variant %d at block_n %d", s8 ? "int8" : (bf16 ? "bf16" : "fp16"),
+                   variant, pl.block_n);
     if (pl.splits > 1 && !pl.cluster) {
         // the separate reduce kernel applies bias / residual; the partial writer must not
         p.bias = nullptr;
         p.residual = nullptr;
     }
-    static bool attr_set[2][6][kNumGemmWidths] = {};
-    if (!attr_set[bf16][variant][wi]) {
+    static bool attr_set[3][6][kNumGemmWidths] = {};
+    const int dt = s8 ? 2 : (bf16 ? 1 : 0);
+    if (!attr_set[dt][variant][wi]) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set[bf16][variant][wi] = true;
+        attr_set[dt][variant][wi] = true;
     }
     if (pl.cluster) {
         B200SD_REQUIRE(variant == 1, "b200sd_gemm: cluster split-K needs the regular epilogue variant");
@@ -2025,17 +2153,24 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
 
 }  // namespace b200sd
 
-static int gemm_entry(const b200sd_gemm_args* args, void* stream, bool bf16) {
+static int gemm_entry(const b200sd_gemm_args* args, void* stream, bool bf16, const float* col_scale = nullptr) {
     if (!b200sd::launch_class_enabled(1)) return 0;  // bench.py's per-class timing graphs
     if (!args) {
-        b200sd::set_error(bf16 ? "b200sd_gemm_bf16: args is null" : "b200sd_gemm: args is null");
+        b200sd::set_error(col_scale ? "b200sd_gemm_s8: args is null" : (bf16 ? "b200sd_gemm_bf16: args is null" : "b200sd_gemm: args is null"));
         return 2;
     }
-    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream), bf16);
+    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream), bf16, col_scale);
 }
 
 extern "C" int b200sd_gemm(const b200sd_gemm_args* args, void* stream) { return gemm_entry(args, stream, false); }
 extern "C" int b200sd_gemm_bf16(const b200sd_gemm_args* args, void* stream) { return gemm_entry(args, stream, true); }
+extern "C" int b200sd_gemm_s8(const b200sd_gemm_args* args, const float* col_scale, void* stream) {
+    if (!col_scale) {
+        b200sd::set_error("b200sd_gemm_s8: col_scale is null");
+        return 2;
+    }
+    return gemm_entry(args, stream, false, col_scale);
+}
 
 extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {
     if (!args || !out4) return 2;
@@ -2047,19 +2182,19 @@ extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {
 
 // Planning query before the weights are tiled: a halo call plans for chunk-major tiled weights of the requested (or the
 // preferred) width.
-static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl, bool bf16) {
+static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl, bool bf16, bool s8 = false) {
     b200sd_gemm_args a = *args;
-    if (a.halo && !bf16) {
+    if (a.halo && !bf16 && !s8) {
         if (a.block_n == 0) a.block_n = b200sd::halo_pick_block_n(a);
         a.wgt_tiled = 1;
     }
-    return b200sd::plan_gemm(a, pl, bf16);
+    return b200sd::plan_gemm(a, pl, bf16, s8);
 }
 
-static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16) {
+static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16, bool s8 = false) {
     if (!args || !out8) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = plan_query(args, pl, bf16)) return rc;
+    if (int rc = plan_query(args, pl, bf16, s8)) return rc;
     out8[0] = pl.block_n, out8[1] = pl.splits, out8[2] = pl.kb_total, out8[3] = pl.n_tiles;
     out8[4] = pl.cs_slots, out8[5] = pl.staged, out8[6] = pl.stages, out8[7] = pl.m_tiles;
     return 0;
@@ -2067,11 +2202,12 @@ static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16) {
 
 extern "C" int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, false); }
 extern "C" int b200sd_gemm_plan_ex_bf16(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, true); }
+extern "C" int b200sd_gemm_plan_ex_s8(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, false, true); }
 
-static int describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size, bool bf16) {
+static int describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size, bool bf16, bool s8 = false) {
     if (!args || !buf || buf_size == 0) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = plan_query(args, pl, bf16)) return rc;
+    if (int rc = plan_query(args, pl, bf16, s8)) return rc;
     // variant: GemmVariant of the GEMM kernel (-1: halo convolution); halo_kind / halo_wide: which halo_conv_kernel
     // instantiation runs (-1 / 0 for the GEMM kernel); win: the halo walk over th x tw windows instead of image rows
     snprintf(buf, buf_size,
@@ -2089,10 +2225,20 @@ extern "C" int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf
 extern "C" int b200sd_gemm_describe_plan_bf16(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
     return describe_plan(args, buf, buf_size, true);
 }
+extern "C" int b200sd_gemm_describe_plan_s8(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
+    return describe_plan(args, buf, buf_size, false, true);
+}
 
 extern "C" size_t b200sd_gemm_workspace_bytes(const b200sd_gemm_args* args) {
     if (!args) return 0;
     b200sd::GemmPlan pl;
     if (b200sd::plan_gemm(*args, pl)) return 0;
+    return b200sd::plan_workspace(pl);
+}
+
+extern "C" size_t b200sd_gemm_workspace_bytes_s8(const b200sd_gemm_args* args) {
+    if (!args) return 0;
+    b200sd::GemmPlan pl;
+    if (b200sd::plan_gemm(*args, pl, false, true)) return 0;
     return b200sd::plan_workspace(pl);
 }

@@ -9,6 +9,7 @@
 #include "../../include/b200sd.h"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cooperative_groups.h>
 #include <stdlib.h>
@@ -174,13 +175,12 @@ __global__ void __launch_bounds__(416) gn_stats_kernel(const T* __restrict__ x0,
 }
 
 // ---- GroupNorm pass 2: normalise, affine, optional SiLU (and concat of the two sources) ------------
-template <typename T>
-__global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x0, const T* __restrict__ x1,
-                                                       int c0, int c1, int hw, int groups,
-                                                       const float* __restrict__ final_stats,
-                                                       const float* __restrict__ gamma,
-                                                       const float* __restrict__ beta, int silu,
-                                                       T* __restrict__ out, int px_per_block) {
+template <typename T, bool kS8>
+__device__ __forceinline__ void gn_apply_body(const T* __restrict__ x0, const T* __restrict__ x1, int c0, int c1, int hw,
+                                              int groups, const float* __restrict__ final_stats,
+                                              const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                              T* __restrict__ out, int8_t* __restrict__ out_s8, float inv_scale,
+                                              int px_per_block) {
     pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
     pdl_wait();
     const int C = c0 + c1;
@@ -214,13 +214,39 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x0,
             const float y = f[e] * s_scale[ch + e] + s_shift[ch + e];
             f[e] = silu ? silu_f(y) : y;
         }
-        uint4 pk;
-        pk.x = Elem16<T>::pack2(f[0], f[1]);
-        pk.y = Elem16<T>::pack2(f[2], f[3]);
-        pk.z = Elem16<T>::pack2(f[4], f[5]);
-        pk.w = Elem16<T>::pack2(f[6], f[7]);
-        *reinterpret_cast<uint4*>(out + (static_cast<size_t>(n) * hw + px) * C + ch) = pk;
+        if constexpr (kS8) {
+            *reinterpret_cast<uint2*>(out_s8 + (static_cast<size_t>(n) * hw + px) * C + ch) = quantize8_s8(f, inv_scale);
+        } else {
+            uint4 pk;
+            pk.x = Elem16<T>::pack2(f[0], f[1]);
+            pk.y = Elem16<T>::pack2(f[2], f[3]);
+            pk.z = Elem16<T>::pack2(f[4], f[5]);
+            pk.w = Elem16<T>::pack2(f[6], f[7]);
+            *reinterpret_cast<uint4*>(out + (static_cast<size_t>(n) * hw + px) * C + ch) = pk;
+        }
     }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x0, const T* __restrict__ x1,
+                                                       int c0, int c1, int hw, int groups,
+                                                       const float* __restrict__ final_stats,
+                                                       const float* __restrict__ gamma,
+                                                       const float* __restrict__ beta, int silu,
+                                                       T* __restrict__ out, int px_per_block) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gn_apply_body<T, false>(x0, x1, c0, c1, hw, groups, final_stats, gamma, beta, silu, out, nullptr, 0.f, px_per_block);
+}
+
+__global__ void __launch_bounds__(256) gn_apply_s8_kernel(const __half* __restrict__ x0, const __half* __restrict__ x1,
+                                                          int c0, int c1, int hw, int groups,
+                                                          const float* __restrict__ final_stats,
+                                                          const float* __restrict__ gamma,
+                                                          const float* __restrict__ beta, int silu,
+                                                          int8_t* __restrict__ out, float inv_scale, int px_per_block) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gn_apply_body<__half, true>(x0, x1, c0, c1, hw, groups, final_stats, gamma, beta, silu, nullptr, out, inv_scale,
+                                px_per_block);
 }
 
 // ---- GroupNorm apply from producer-side statistics -----------------------------------------------------------------
@@ -303,11 +329,13 @@ __global__ void __launch_bounds__(256) gn_apply_chan_kernel(const __half* __rest
 // through distributed shared memory in rank order -- no global barrier, no partial buffers, no atomics (bitwise
 // reproducible).  Thread t owns vector column t % vpr for all its pixels, so per-channel
 // partial sums live in registers and fold rows -> channels -> groups in a fixed order.
-template <typename T, int kRowsInFlight>
-__global__ void gn_cluster_kernel(const T* __restrict__ x0, const T* __restrict__ x1, int c0, int c1, int hw,
-                                  int groups, int chunk_ch, int rows_per_cta, float eps,
-                                  const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
-                                  T* __restrict__ out) {
+// kS8: the W8A8 convolution's operand -- the fp32 result y is stored as int8 q = clamp(rint(y * inv_scale), -127, 127)
+// to out_s8 instead of as T to out.
+template <typename T, int kRowsInFlight, bool kS8>
+__device__ __forceinline__ void gn_cluster_body(const T* __restrict__ x0, const T* __restrict__ x1, int c0, int c1, int hw,
+                                                int groups, int chunk_ch, int rows_per_cta, float eps,
+                                                const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                                T* __restrict__ out, int8_t* __restrict__ out_s8, float inv_scale) {
     using E = Elem16<T>;
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
@@ -419,7 +447,8 @@ __global__ void gn_cluster_kernel(const T* __restrict__ x0, const T* __restrict_
             sc8[e] = stat[ng + g] * gamma[ch + e];
             sh8[e] = fmaf(-mean8[e], sc8[e], beta[ch + e]);
         }
-        T* dst = out + static_cast<size_t>(n) * hw * C + ch;
+        T* dst = kS8 ? nullptr : out + static_cast<size_t>(n) * hw * C + ch;
+        int8_t* dst8 = kS8 ? out_s8 + static_cast<size_t>(n) * hw * C + ch : nullptr;
 #pragma unroll 2
         for (int px = px0 + ty; px < px1; px += TY) {
             const uint4 raw = slab[(px - px0) * vpr + cv];
@@ -436,15 +465,39 @@ __global__ void gn_cluster_kernel(const T* __restrict__ x0, const T* __restrict_
                 const float y = fmaf(f[e], sc8[e], sh8[e]);
                 f[e] = silu ? __fdividef(y, 1.0f + __expf(-y)) : y;
             }
-            uint4 pk;
-            pk.x = E::pack2(f[0], f[1]);
-            pk.y = E::pack2(f[2], f[3]);
-            pk.z = E::pack2(f[4], f[5]);
-            pk.w = E::pack2(f[6], f[7]);
-            *reinterpret_cast<uint4*>(dst + static_cast<size_t>(px) * C) = pk;
+            if constexpr (kS8) {
+                *reinterpret_cast<uint2*>(dst8 + static_cast<size_t>(px) * C) = quantize8_s8(f, inv_scale);
+            } else {
+                uint4 pk;
+                pk.x = E::pack2(f[0], f[1]);
+                pk.y = E::pack2(f[2], f[3]);
+                pk.z = E::pack2(f[4], f[5]);
+                pk.w = E::pack2(f[6], f[7]);
+                *reinterpret_cast<uint4*>(dst + static_cast<size_t>(px) * C) = pk;
+            }
         }
     }
     cluster.barrier_wait();
+}
+
+template <typename T, int kRowsInFlight>
+__global__ void gn_cluster_kernel(const T* __restrict__ x0, const T* __restrict__ x1, int c0, int c1, int hw,
+                                  int groups, int chunk_ch, int rows_per_cta, float eps,
+                                  const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                  T* __restrict__ out) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gn_cluster_body<T, kRowsInFlight, false>(x0, x1, c0, c1, hw, groups, chunk_ch, rows_per_cta, eps, gamma, beta, silu, out,
+                                             nullptr, 0.f);
+}
+
+template <int kRowsInFlight>
+__global__ void gn_cluster_s8_kernel(const __half* __restrict__ x0, const __half* __restrict__ x1, int c0, int c1, int hw,
+                                     int groups, int chunk_ch, int rows_per_cta, float eps,
+                                     const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                     int8_t* __restrict__ out, float inv_scale) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gn_cluster_body<__half, kRowsInFlight, true>(x0, x1, c0, c1, hw, groups, chunk_ch, rows_per_cta, eps, gamma, beta, silu,
+                                                 nullptr, out, inv_scale);
 }
 
 static int gn_chunks(int hw, int n_img) {
@@ -583,14 +636,16 @@ extern "C" size_t b200sd_group_norm_workspace_bytes(int32_t n_img, int32_t hw, i
 }
 
 // b200sd_group_norm (T = __half) and b200sd_group_norm_bf16 (T = __nv_bfloat16): same plans, same kernels
+// out_s8 (fp16 input only): b200sd_group_norm_s8 -- the int8 operand of the W8A8 convolution instead of `out`
 template <typename T>
 static int group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
                       int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
-                      void* out, float* stats_ws, size_t stats_ws_bytes, void* stream_) {
+                      void* out, float* stats_ws, size_t stats_ws_bytes, void* stream_, int8_t* out_s8 = nullptr,
+                      float inv_scale = 0.f) {
     if (!b200sd::launch_class_enabled(4)) return 0;  // bench.py's per-class timing graphs
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const int C = c0 + c1;
-    B200SD_REQUIRE(x0 && out && gamma && beta && stats_ws, "b200sd_group_norm: null pointer");
+    B200SD_REQUIRE(x0 && (out || out_s8) && gamma && beta && stats_ws, "b200sd_group_norm: null pointer");
     B200SD_REQUIRE(c0 > 0 && c0 % 8 == 0 && c1 >= 0 && c1 % 8 == 0 && (c1 == 0 || x1),
                    "b200sd_group_norm: channels must be multiples of 8 (c0=%d c1=%d)", c0, c1);
     B200SD_REQUIRE(groups > 0 && C % groups == 0, "b200sd_group_norm: %d channels not divisible by %d groups", C,
@@ -631,10 +686,12 @@ static int group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, in
         if (mode == 1 && vpr <= 64 && C % chunk == 0 && csmem <= 200 * 1024 && n_img <= 65535 && C / chunk <= 65535) {
             const int deep = (rows_per_cta + TY - 1) / TY >= 3 ? 1 : 0;
             auto kern = deep ? gn_cluster_kernel<T, 8> : gn_cluster_kernel<T, 2>;
-            static bool attr[2] = {false, false};
-            if (!attr[deep]) {
-                B200SD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-                attr[deep] = true;
+            auto kern8 = deep ? gn_cluster_s8_kernel<8> : gn_cluster_s8_kernel<2>;
+            static bool attr[2] = {false, false}, attr8[2] = {false, false};
+            if (!(out_s8 ? attr8 : attr)[deep]) {
+                if (out_s8) B200SD_CHECK_CUDA(cudaFuncSetAttribute(kern8, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+                else B200SD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+                (out_s8 ? attr8 : attr)[deep] = true;
             }
             cudaLaunchConfig_t cfg;
             memset(&cfg, 0, sizeof(cfg));
@@ -654,11 +711,17 @@ static int group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, in
                 at[1].val.programmaticStreamSerializationAllowed = 1;
                 cfg.numAttrs = 2;
             }
-            B200SD_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, reinterpret_cast<const T*>(x0),
-                                                 reinterpret_cast<const T*>(x1), static_cast<int>(c0),
-                                                 static_cast<int>(c1), static_cast<int>(hw), static_cast<int>(groups), chunk,
-                                                 rows_per_cta, eps, gamma, beta, static_cast<int>(silu),
-                                                 reinterpret_cast<T*>(out)));
+            if (out_s8)
+                B200SD_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern8, reinterpret_cast<const __half*>(x0),
+                                                     reinterpret_cast<const __half*>(x1), static_cast<int>(c0),
+                                                     static_cast<int>(c1), static_cast<int>(hw), static_cast<int>(groups), chunk,
+                                                     rows_per_cta, eps, gamma, beta, static_cast<int>(silu), out_s8, inv_scale));
+            else
+                B200SD_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, reinterpret_cast<const T*>(x0),
+                                                     reinterpret_cast<const T*>(x1), static_cast<int>(c0),
+                                                     static_cast<int>(c1), static_cast<int>(hw), static_cast<int>(groups), chunk,
+                                                     rows_per_cta, eps, gamma, beta, static_cast<int>(silu),
+                                                     reinterpret_cast<T*>(out)));
             B200SD_CHECK_CUDA(cudaGetLastError());
             count_launch(1);
             return 0;
@@ -692,9 +755,14 @@ static int group_norm(const void* x0, const void* x1, int32_t c0, int32_t c1, in
     const int px_per_block = std::max(1, (hw + want_blocks - 1) / want_blocks);
     const int blocks = (hw + px_per_block - 1) / px_per_block;
     const size_t smem2 = 2 * static_cast<size_t>(C) * sizeof(float);
-    B200SD_CHECK_CUDA(launch_kernel(gn_apply_kernel<T>, dim3(dim3(blocks, n_img)), dim3(256), smem2, stream, 
-        reinterpret_cast<const T*>(x0), reinterpret_cast<const T*>(x1), c0, c1, hw, groups, final_stats,
-        gamma, beta, silu, reinterpret_cast<T*>(out), px_per_block));
+    if (out_s8)
+        B200SD_CHECK_CUDA(launch_kernel(gn_apply_s8_kernel, dim3(dim3(blocks, n_img)), dim3(256), smem2, stream,
+            reinterpret_cast<const __half*>(x0), reinterpret_cast<const __half*>(x1), c0, c1, hw, groups, final_stats,
+            gamma, beta, silu, out_s8, inv_scale, px_per_block));
+    else
+        B200SD_CHECK_CUDA(launch_kernel(gn_apply_kernel<T>, dim3(dim3(blocks, n_img)), dim3(256), smem2, stream, 
+            reinterpret_cast<const T*>(x0), reinterpret_cast<const T*>(x1), c0, c1, hw, groups, final_stats,
+            gamma, beta, silu, reinterpret_cast<T*>(out), px_per_block));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(2);
     return 0;
@@ -704,6 +772,16 @@ extern "C" int b200sd_group_norm(const void* x0, const void* x1, int32_t c0, int
                                  int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
                                  void* out, float* stats_ws, size_t stats_ws_bytes, void* stream) {
     return group_norm<__half>(x0, x1, c0, c1, n_img, hw, groups, eps, gamma, beta, silu, out, stats_ws, stats_ws_bytes, stream);
+}
+
+extern "C" int b200sd_group_norm_s8(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,
+                                    int32_t groups, float eps, const float* gamma, const float* beta, int32_t silu,
+                                    float inv_scale, void* out, float* stats_ws, size_t stats_ws_bytes, void* stream) {
+    B200SD_REQUIRE(out != nullptr, "b200sd_group_norm_s8: null pointer");
+    B200SD_REQUIRE(std::isfinite(inv_scale) && inv_scale > 0.f, "b200sd_group_norm_s8: inv_scale=%g must be positive and finite",
+                   static_cast<double>(inv_scale));
+    return group_norm<__half>(x0, x1, c0, c1, n_img, hw, groups, eps, gamma, beta, silu, nullptr, stats_ws, stats_ws_bytes,
+                              stream, static_cast<int8_t*>(out), inv_scale);
 }
 
 extern "C" int b200sd_group_norm_bf16(const void* x0, const void* x1, int32_t c0, int32_t c1, int32_t n_img, int32_t hw,

@@ -67,6 +67,11 @@ static EncodeTiledFn get_encode_fn() {
 
 int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                     const uint32_t* box, const uint32_t* elem_strides) {
+    return encode_tmap(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, base, rank, dims, strides_bytes, box, elem_strides);
+}
+
+int encode_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides) {
     EncodeTiledFn fn = get_encode_fn();
     B200SD_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
     B200SD_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor map base %p is not 16-byte aligned", base);
@@ -82,7 +87,7 @@ int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t
                            static_cast<unsigned long long>(gs[i]), i + 1);
         }
     }
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gd,
+    CUresult r = fn(map, dtype, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gd,
                     gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B200SD_REQUIRE(r == CUDA_SUCCESS,

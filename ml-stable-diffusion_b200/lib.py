@@ -104,6 +104,17 @@ _SIGNATURES = {
     "b200sd_upsample2x": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p]),
     "b200sd_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    # W8A8 (int8 wgmma) 3x3 convolution and its operand producers
+    "b200sd_gemm_s8": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p, C.c_void_p]),
+    "b200sd_gemm_plan_ex_s8": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(C.c_int32)]),
+    "b200sd_gemm_describe_plan_s8": (C.c_int, [C.POINTER(GemmArgs), C.c_char_p, C.c_size_t]),
+    "b200sd_gemm_workspace_bytes_s8": (C.c_size_t, [C.POINTER(GemmArgs)]),
+    "b200sd_group_norm_s8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_float, C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p,
+                                       C.c_size_t, C.c_void_p]),
+    "b200sd_upsample2x_s8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                       C.c_void_p]),
+    "b200sd_absmax_f16": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "b200sd_ctx_to_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_void_p]),
     "b200sd_embed_tokens": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
@@ -284,27 +295,28 @@ TILED_WEIGHTS = os.environ.get("B200SD_TILED_W", "1") != "0"
 _tiled_cache = {}
 
 
-def pack_tiled(w2d, c0, c1, taps, bn, chunk_major=False, extra=(0, 0)):
+def pack_tiled(w2d, c0, c1, taps, bn, chunk_major=False, extra=(0, 0), chunk=64):
     """[N, taps*(c0+c1) (+ c2 + c3)] -> [n_tiles, k_blocks, bn, 64] fp16 in the exact k-block order of the kernel's main
     loop (tap-major; per tap the 64-channel chunks of source 0, then of source 1; ragged chunks zero padded), so
     that each weight tile is one contiguous bn*128-byte burst in HBM.  chunk_major: k-block = chunk * taps + tap
     (the halo convolution walks all nine taps of one 64-channel chunk before the next chunk).  extra = (c2, c3): the
-    folded shortcut's columns follow the convolution's: their chunks (source 2, then source 3) are the last k-blocks."""
+    folded shortcut's columns follow the convolution's: their chunks (source 2, then source 3) are the last k-blocks.
+    chunk: channels per k-block (128 for the int8 convolution, whose k-block is the same 128 bytes)."""
     n, kpt = w2d.shape[0], c0 + c1
-    kc0, kc1 = (c0 + 63) // 64, (c1 + 63) // 64
+    kc0, kc1 = (c0 + chunk - 1) // chunk, (c1 + chunk - 1) // chunk
     kc = kc0 + kc1
     nt = (n + bn - 1) // bn
     c2, c3 = extra
     wp = torch.zeros(nt * bn, taps, kpt, dtype=w2d.dtype, device=w2d.device)
     wp[:n] = w2d[:, : taps * kpt].reshape(n, taps, kpt)
-    out = torch.zeros(nt, taps, kc, bn, 64, dtype=w2d.dtype, device=w2d.device)
+    out = torch.zeros(nt, taps, kc, bn, chunk, dtype=w2d.dtype, device=w2d.device)
     for j in range(kc):
-        lo = j * 64 if j < kc0 else c0 + (j - kc0) * 64
-        hi = min(lo + 64, c0 if j < kc0 else kpt)
+        lo = j * chunk if j < kc0 else c0 + (j - kc0) * chunk
+        hi = min(lo + chunk, c0 if j < kc0 else kpt)
         out[:, :, j, :, : hi - lo] = wp[:, :, lo:hi].reshape(nt, bn, taps, hi - lo).permute(0, 2, 1, 3)
     if chunk_major:
         out = out.permute(0, 2, 1, 3, 4)
-    out = out.reshape(nt, taps * kc, bn, 64)
+    out = out.reshape(nt, taps * kc, bn, chunk)
     if c2 + c3:
         if chunk_major:
             raise B200SDError("pack_tiled: shortcut columns are not supported in the chunk-major (halo) layout")
@@ -543,6 +555,111 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=No
     else:
         run_gemm(args)
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# W8A8: int8 3x3 convolution (b200sd_gemm_s8) and the kernels that produce its int8 operand
+# ------------------------------------------------------------------------------------------------
+def plan_ex_s8(args):
+    """plan_ex of the int8 convolution (k-blocks of 128 channels)."""
+    plan = (C.c_int32 * 8)()
+    _check(load().b200sd_gemm_plan_ex_s8(C.byref(args), plan), "b200sd_gemm_plan_ex_s8")
+    return tuple(int(v) for v in plan)
+
+
+def describe_plan_s8(n, c0, n_img, h, w, has_bias=True, has_residual=False, bias_rows=0, split_k=0, block_n=0) -> str:
+    """Host-only: the tiling b200sd_gemm_s8 would choose for a stride-1 3x3 convolution (see describe_plan)."""
+    a = GemmArgs()
+    a.mode, a.n, a.c0, a.n_img, a.h, a.w, a.stride = 1, n, c0, n_img, h, w, 1
+    a.bias_rows, a.split_k, a.block_n = bias_rows, split_k, block_n
+    a.bias = 1 if has_bias else None
+    a.residual = 1 if has_residual else None
+    buf = C.create_string_buffer(512)
+    _check(load().b200sd_gemm_describe_plan_s8(C.byref(a), buf, 512), "b200sd_gemm_describe_plan_s8")
+    return buf.value.decode()
+
+
+def _tiled_s8(args, wgt):
+    """int8 [Cout, 9*C0] OHWI weights -> the pre-tiled layout of the planned width (cached per (weight, block_n))."""
+    bn = args.block_n if args.block_n > 0 else plan_ex_s8(args)[0]
+    key = (wgt.data_ptr(), bn, args.c0, "s8")
+    hit = _tiled_cache.get(key)
+    if hit is not None and hit[0]() is wgt and hit[1] == wgt._version:
+        return hit[2], bn
+    if torch.cuda.is_current_stream_capturing():
+        raise B200SDError("conv3x3_s8: weights of this shape were not tiled before CUDA-graph capture; run one eager "
+                          "call with the same shapes first")
+    packed = pack_tiled(wgt, args.c0, 0, 9, bn, chunk=128)
+    _tiled_cache[key] = (weakref.ref(wgt), wgt._version, packed)
+    return packed, bn
+
+
+def conv3x3_s8(x, wgt, col_scale, bias=None, residual=None, *, bias_rows=0, bias_stride=0, split_k=0, block_n=0,
+               out=None):
+    """W8A8 3x3 pad-1 stride-1 convolution on int8 wgmma.  x int8 NHWC [N, H, W, C] (C a multiple of 16); wgt int8
+    [Cout, 9*C] (OHWI, symmetric per-output-channel quantized); col_scale fp32 [Cout] = s_a * s_w; bias fp32 [Cout] or
+    [N, Cout] rows (bias_rows = H*W); residual fp16 NHWC [N, H, W, Cout].  Returns fp16 NHWC
+    fp16(acc * col_scale + bias + residual)."""
+    _req(x, torch.int8, "conv3x3_s8 x")
+    _req(wgt, torch.int8, "conv3x3_s8 wgt")
+    _req(col_scale, torch.float32, "conv3x3_s8 col_scale")
+    if residual is not None:
+        _req(residual, torch.float16, "conv3x3_s8 residual")
+    nimg, h, w, c = x.shape
+    cout = wgt.shape[0]
+    if wgt.shape[1] != 9 * c or col_scale.numel() != cout:
+        raise B200SDError(f"conv3x3_s8: weight {tuple(wgt.shape)} / col_scale {col_scale.numel()} do not match "
+                          f"{c} input and {cout} output channels")
+    if out is None:
+        out = torch.empty(nimg, h, w, cout, dtype=torch.float16, device=x.device)
+    _req(out, torch.float16, "conv3x3_s8 out")
+    args = gemm_args(1, x, wgt, out, bias=bias, residual=residual, n=cout, n_img=nimg, h=h, w=w, bias_rows=bias_rows,
+                     bias_stride=bias_stride, split_k=split_k, block_n=block_n)
+    packed, bn = _tiled_s8(args, wgt)
+    args.wgt, args.block_n, args.wgt_tiled = packed.data_ptr(), bn, 1
+    need = int(load().b200sd_gemm_workspace_bytes_s8(C.byref(args)))
+    if need:
+        ws = _workspace(need, x.device)
+        args.workspace = ws.data_ptr()
+        args.workspace_bytes = ws.numel() * 4
+    _check(load().b200sd_gemm_s8(C.byref(args), _ptr(col_scale), _stream()), "b200sd_gemm_s8")
+    return out
+
+
+def group_norm_s8(x, gamma, beta, groups, eps, inv_scale, silu=True, x1=None, out=None):
+    """group_norm (fp16 sources) whose output is int8: q = clamp(rint(y * inv_scale), -127, 127) of the fp32 y."""
+    _req(x, torch.float16, "group_norm_s8 x")
+    _same16(torch.float16, x1, None, "group_norm_s8 x1")
+    nimg, h, w, c0 = x.shape
+    c1 = 0 if x1 is None else x1.shape[-1]
+    if out is None:
+        out = torch.empty(nimg, h, w, c0 + c1, dtype=torch.int8, device=x.device)
+    _req(out, torch.int8, "group_norm_s8 out")
+    need = int(load().b200sd_group_norm_workspace_bytes(nimg, h * w, c0 + c1, groups))
+    ws = _workspace(need, x.device)
+    _check(load().b200sd_group_norm_s8(_ptr(x), _ptr(x1), c0, c1, nimg, h * w, groups, float(eps), _ptr(gamma), _ptr(beta),
+                                       int(silu), float(inv_scale), _ptr(out), _ptr(ws), ws.numel() * 4, _stream()),
+           "b200sd_group_norm_s8")
+    return out
+
+
+def upsample2x_s8(x, inv_scale, out=None):
+    """Nearest x2 upsample of fp16 NHWC x into int8: q = clamp(rint(x * inv_scale), -127, 127)."""
+    _req(x, torch.float16, "upsample2x_s8 x")
+    n, h, w, c = x.shape
+    if out is None:
+        out = torch.empty(n, 2 * h, 2 * w, c, dtype=torch.int8, device=x.device)
+    _req(out, torch.int8, "upsample2x_s8 out")
+    _check(load().b200sd_upsample2x_s8(_ptr(x), _ptr(out), n, h, w, c, float(inv_scale), _stream()), "b200sd_upsample2x_s8")
+    return out
+
+
+def absmax(x, slot):
+    """slot (fp32 device scalar, >= 0) = max(slot, max |x|) for an fp16 tensor x: the W8A8 calibration probe."""
+    _req(x, torch.float16, "absmax x")
+    _req(slot, torch.float32, "absmax slot")
+    _check(load().b200sd_absmax_f16(_ptr(x), x.numel(), _ptr(slot), _stream()), "b200sd_absmax_f16")
+    return slot
 
 
 def linear_small(x, wgt, bias=None, add=None, act_in=False, act_out=False):

@@ -245,7 +245,7 @@ class B200StableDiffusionPipeline:
     @classmethod
     def from_pretrained(cls, model_dir, images_per_call=1, device="cuda", height=None, width=None,
                         scheduler_override=None, controlnet_dirs=None, force_zeros_for_empty_prompt=None,
-                        with_vae_encoder=False, refiner_dir=None, load_safety_checker=True):
+                        with_vae_encoder=False, refiner_dir=None, load_safety_checker=True, unet_quantization=None):
         """Build the pipeline from a diffusers-layout model directory (``unet/``, ``vae/``, ``text_encoder[_2]/``,
         ``tokenizer[_2]/``, ``scheduler/``): the counterpart of ``get_coreml_pipe(pytorch_pipe, mlpackages_dir,
         model_version, compute_unit, scheduler_override, controlnet_models, force_zeros_for_empty_prompt)``
@@ -253,7 +253,9 @@ class B200StableDiffusionPipeline:
         ``checkpoint.load_component`` (schema-checked), configs with ``checkpoint.read_config``.
         ``refiner_dir``: an SDXL refiner directory whose UNet takes over at ``refiner_start`` (``__call__``).
         ``load_safety_checker``: load ``safety_checker/`` with ``feature_extractor/`` when the directory has them (SD 1.4
-        / 1.5; get_coreml_pipe loads it whenever the diffusers pipeline has one, pipeline.py:650-656); False skips it."""
+        / 1.5; get_coreml_pipe loads it whenever the diffusers pipeline has one, pipeline.py:650-656); False skips it.
+        ``unet_quantization``: a ``quantization.W8A8Recipe`` or the path of a saved one (``calibrate_unet``); the base
+        UNet runs the convolutions it names in W8A8.  The refiner, ControlNets, VAE and text encoders stay fp16."""
         import json
         import os
         from . import checkpoint as K
@@ -270,7 +272,7 @@ class B200StableDiffusionPipeline:
         w = (width // f) if width else size
         xl = ucfg.get("addition_embed_type") == "text_time"
         unet = UNetModel(ucfg, K.load_component(model_dir, "unet", ucfg), batch=2 * images_per_call, height=h, width=w,
-                         device=device)
+                         device=device, quantization=unet_quantization)
         vsd = K.read_state_dict(os.path.join(model_dir, "vae"))
         vdtype = vae_dtype(ucfg, vcfg)
         vae = VAEDecoderModel(vcfg, K.check_state_dict("vae_decoder", vcfg, vsd), batch=images_per_call, height=h,
@@ -749,6 +751,29 @@ class B200StableDiffusionPipeline:
             if callback is not None and i % callback_steps == 0:
                 callback(i, st.timestep, x_space(i + 1))
         return self._denoised if return_denoised else self._latents
+
+    def calibrate_unet(self, prompts, num_inference_steps=50, guidance_scale=7.5, seed=0):
+        """W8A8 calibration: runs the denoising loop eagerly with the fp16 UNet once per prompt (seed, seed + 1, ...)
+        and records max |x| at the input of every convolution the engine can quantize, over every UNet call (all
+        steps, both classifier-free-guidance halves).  Returns the ``quantization.W8A8Recipe`` with s_a = amax / 127 for
+        all of them; ``from_pretrained(..., unet_quantization=recipe)`` (or ``recipe.save(path)``) applies it."""
+        from .quantization import W8A8Recipe
+        if isinstance(prompts, str):
+            prompts = [prompts]
+        u = self.unet
+        eng = u.engine
+        slots = eng.set_calibration(True)
+        graphed, u.use_cuda_graph = u.use_cuda_graph, False  # the probes must not enter a captured graph
+        try:
+            for i, p in enumerate(prompts):
+                # a callback keeps denoise() on the step-by-step path, where every UNet call runs eagerly
+                self(p, height=self.height, width=self.width, num_inference_steps=num_inference_steps,
+                     guidance_scale=guidance_scale, seed=seed + i, output_type="np", callback=lambda *a: None)
+            torch.cuda.synchronize(self.device)
+        finally:
+            u.use_cuda_graph = graphed
+            eng.set_calibration(False)
+        return W8A8Recipe.from_amax({n: float(t.item()) for n, t in slots.items()}, eng.cfg)
 
     def decode_latents(self, latents, want_u8=False):
         """pipeline.py:313-320 on the device: z / scaling -> decoder -> clip(x/2+0.5, 0, 1) -> NHWC fp32 (and, with

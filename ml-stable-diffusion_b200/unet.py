@@ -25,6 +25,7 @@ import os
 import torch
 
 from . import lib as L
+from . import quantization as Q
 
 
 class AttentionImplementations(enum.Enum):
@@ -83,7 +84,9 @@ class _Packer:
 class UNetEngine:
     """Holds device-resident packed weights and issues the forward launch sequence."""
 
-    def __init__(self, cfg: dict, state_dict: dict, device="cuda"):
+    def __init__(self, cfg: dict, state_dict: dict, device="cuda", quantization=None):
+        """quantization: a W8A8Recipe (or the path of a saved one): the ResNet / up-sampler convolutions it names run
+        on the int8 convolution kernel with its activation scales; every other layer is unchanged."""
         L.load()
         self.cfg = dict(cfg)
         self.dev = torch.device(device)
@@ -124,8 +127,22 @@ class UNetEngine:
         for c, h in zip(boc, self.heads):
             if c % h or c // h not in L.ATTENTION_HEAD_DIMS:
                 raise L.B200SDError(f"b200sd attention kernel supports head dims {L.ATTENTION_HEAD_DIMS} (got {c}/{h})")
+        self.fusion_mode = fm
+        self.recipe = Q.as_recipe(quantization)
+        self.calib = None  # layer -> fp32 device slot of max |x| while calibrating (set_calibration)
+        if self.recipe is not None:
+            self._require_default_level("a W8A8 recipe")
+            self.recipe.validate(self.cfg)
         L.reserve_attention_workspace(self.dev, max(c // h for c, h in zip(boc, self.heads)))
         self._pack(state_dict)
+
+    def _require_default_level(self, what):
+        """The W8A8 launches (and the calibration probes) replace the default level's GroupNorm + 9-tap convolution
+        pairs; the opt-in fusion levels and the TMA-patch halo convolution take other paths."""
+        if self.fusion_mode != "ln":
+            raise ValueError(f"{what} needs B200SD_FUSED=ln (the default), got B200SD_FUSED={self.fusion_mode}")
+        if self.halo_tma_min_hw:
+            raise ValueError(f"{what} cannot be combined with B200SD_HALO_TMA")
 
     # ------------------------------------------------------------------ packing
     def _pack(self, sd):
@@ -233,6 +250,20 @@ class UNetEngine:
         self.kv_w = P.f16(torch.cat(kv_w, 0)) if kv_w else None
         self.kv_total = off_kv
         self.w = w
+        # W8A8 layers: int8 OHWI weights, col_scale = s_a * s_w, 1 / s_a for the producer of the int8 operand
+        self.q = {}
+        for name, s_a in (self.recipe.scales.items() if self.recipe is not None else ()):
+            wt = sd[name + ".weight"].detach().float()
+            qw, s_w = Q.quantize_weight(wt.permute(0, 2, 3, 1).reshape(wt.shape[0], -1))
+            self.q[name] = {"w": qw.to(self.dev).contiguous(), "cs": (s_w * s_a).to(self.dev).contiguous(),
+                            "inv": 1.0 / s_a}
+            # the fp16 copies of a quantized convolution are never launched
+            block, conv = name.rsplit(".", 1)
+            if conv == "conv":
+                del w[name]["w"]
+            else:
+                for k in (("c1",) if conv == "conv1" else ("c2", "c2sc")):
+                    w[block].pop(k, None)
         self.weight_bytes = sum(t.numel() * t.element_size() for t in self._tensors())
 
     def _tensors(self):
@@ -250,6 +281,26 @@ class UNetEngine:
         yield self.temb_b
         if self.kv_w is not None:
             yield self.kv_w
+        yield from walk(getattr(self, "q", {}))
+
+    # ------------------------------------------------------------------ W8A8 calibration
+    def set_calibration(self, on: bool):
+        """Calibration mode: every forward folds max |x| at the input of every quantizable layer into a device slot
+        (deterministic).  Returns the slots (layer -> fp32 [1] tensor) when switched on; they accumulate until the
+        mode is switched on again."""
+        if not on:
+            self.calib = None
+            return None
+        if self.recipe is not None:
+            raise ValueError("calibrate the fp16 UNet: this engine already runs a W8A8 recipe")
+        self._require_default_level("W8A8 calibration")
+        layers = [n for n, c in Q.quantizable_layers(self.cfg).items() if c % 16 == 0]
+        self.calib = {n: torch.zeros(1, dtype=torch.float32, device=self.dev) for n in layers}
+        return self.calib
+
+    def _probe(self, name, x):
+        if self.calib is not None and name in self.calib:
+            L.absmax(x, self.calib[name])
 
     # ------------------------------------------------------------------ blocks
     def _resnet(self, p, x, x1, temb_all):
@@ -303,9 +354,15 @@ class UNetEngine:
               and kw.get("stride", 1) == 1 and kw.get("out_dtype", torch.float16) == torch.float16 and not kw.get("act"))
         return 2 if ok else False
 
-    def _gn_conv(self, x, xs, x1, x1s, gamma, beta, eps, silu, wgt, bias, residual=None, stats=None, **kw):
+    def _gn_conv(self, x, xs, x1, x1s, gamma, beta, eps, silu, wgt, bias, residual=None, stats=None, layer=None, **kw):
+        q = self.q.get(layer)
+        if q is not None:  # W8A8: GroupNorm (+SiLU) straight to int8, int8 convolution
+            hq = L.group_norm_s8(x, gamma, beta, self.groups, eps, q["inv"], silu=silu, x1=x1)
+            return L.conv3x3_s8(hq, q["w"], q["cs"], bias, residual, bias_rows=kw.get("bias_rows", 0),
+                                bias_stride=kw.get("bias_stride", 0))
         if not self.fuse_gn:  # standalone GroupNorm launch + plain convolution, no statistics side outputs
             hh = L.group_norm(x, gamma, beta, self.groups, eps, silu=silu, x1=x1)
+            self._probe(layer, hh)
             return L.conv3x3(hh, wgt, bias, residual, halo=False if kw.get("shortcut") else self._halo_tma(hh, wgt, kw), **kw)
         have = xs is not None and (x1 is None or x1s is not None)
         halo = self._use_halo(x)
@@ -323,20 +380,21 @@ class UNetEngine:
         n, h, wd, _ = x.shape
         off, co = self.temb_slices[p]
         st1, st2 = {}, {}
-        hh = self._gn_conv(x, xs, x1, x1s, r["n1g"], r["n1b"], self.eps, True, r["c1"], temb_all[:, off:],
-                           stats=st1 if self.fuse_gn else None, bias_rows=h * wd, bias_stride=self.temb_total)
-        if "c2sc" in r:
+        hh = self._gn_conv(x, xs, x1, x1s, r["n1g"], r["n1b"], self.eps, True, r.get("c1"), temb_all[:, off:],
+                           stats=st1 if self.fuse_gn else None, layer=p + ".conv1", bias_rows=h * wd,
+                           bias_stride=self.temb_total)
+        if "c2sc" in r and (p + ".conv2") not in self.q:
             # out = conv2(h) + conv_shortcut(x ++ x1) as ONE launch (unet.py:483-489)
             out = self._gn_conv(hh, None, None, None, r["n2g"], r["n2b"], self.eps, True, r["c2sc"], r["c2scb"], None,
-                                shortcut=(x, x1))
+                                layer=p + ".conv2", shortcut=(x, x1))
             return out, None
         if "sc" in r:
             res = L.linear(x.reshape(n * h * wd, -1), r["sc"], r["scb"],
                            x1=None if x1 is None else x1.reshape(n * h * wd, -1), static_w=True)
         else:
             res = x
-        out = self._gn_conv(hh, st1.get("chan"), None, None, r["n2g"], r["n2b"], self.eps, True, r["c2"], r["c2b"], res,
-                            stats=st2 if self.fuse_gn else None)
+        out = self._gn_conv(hh, st1.get("chan"), None, None, r["n2g"], r["n2b"], self.eps, True, r.get("c2"), r["c2b"], res,
+                            stats=st2 if self.fuse_gn else None, layer=p + ".conv2")
         return out, st2.get("chan")
 
     def _transformer_f(self, p, x, xs, kv_all, batch, heads, s_ctx):
@@ -407,9 +465,14 @@ class UNetEngine:
                 if typ == "CrossAttnUpBlock2D":
                     x, xs = self._transformer_f(f"up_blocks.{i}.attentions.{j}", x, xs, kv_all, batch, rheads[i], s_ctx)
             if i != self.nb - 1:
-                u = self.w[f"up_blocks.{i}.upsamplers.0.conv"]
+                name = f"up_blocks.{i}.upsamplers.0.conv"
+                u = self.w[name]
                 st = {}
-                if self.fuse_gn and 4 * x.shape[1] * x.shape[2] >= self.halo_min_hw:
+                self._probe(name, x)
+                if name in self.q:
+                    q = self.q[name]
+                    x = L.conv3x3_s8(L.upsample2x_s8(x, q["inv"]), q["w"], q["cs"], u["b"])
+                elif self.fuse_gn and 4 * x.shape[1] * x.shape[2] >= self.halo_min_hw:
                     x = L.conv3x3(x, u["w"], u["b"], halo=True, upsample=True, stats=st)
                 else:
                     up = L.upsample2x(x)
