@@ -171,6 +171,29 @@ int b200sd_gemm_plan_ex_s8(const b200sd_gemm_args* args, int32_t* out8);
 int b200sd_gemm_describe_plan_s8(const b200sd_gemm_args* args, char* buf, size_t buf_size);
 size_t b200sd_gemm_workspace_bytes_s8(const b200sd_gemm_args* args);
 
+/* ---- palettized weights (n-bit lookup-table weights decoded in the GEMM producer) -------------------------------
+ * The B operand of b200sd_gemm given as palette indices: weight[j, k] = fp16_rn(float(lut[seg(j)][idx[j, k]]) *
+ * kscale[k]) (kscale NULL: the palette entry itself), seg(j) = (j >= seg_end0) + (j >= seg_end1).  idx[j, :] is row j
+ * of `packed`, the indices of the weight's columns in the kernel's k order (tap-major, source 0 then source 1) packed
+ * least-significant bit first, nbits per index; columns past the last k-block are ignored.  The launch uses the plan
+ * b200sd_gemm would use for the same args (tile width, split-K, k order), so its output is bit-identical to
+ * b200sd_gemm on the decoded weights; b200sd_gemm_workspace_bytes gives its scratch.  Supports modes 0 / 1, stride 1
+ * / 2, one or two sources with c0, c1 multiples of 64, bias, residual, geglu, act, split-K, rs_out and the LayerNorm
+ * fold; rejects wgt_tiled, halo, upsample2x, gn_*, cs_*, a2 / a3 and out_f32 with an error naming the field. */
+typedef struct {
+    const void* packed;    /* uint8 [n][row_bytes] */
+    const void* lut;       /* fp16 [3][256]: the palettes of the three row segments (entries past 2^bits unused) */
+    const float* kscale;   /* fp32 [k_blocks * 64] per-k scale (LayerNorm gamma of a folded launch), 16-byte aligned, or NULL */
+    int32_t nbits;         /* index width: 1, 2, 4, 6 or 8 */
+    int32_t row_bytes;     /* bytes per packed row: a multiple of 16, >= k_blocks * 8 * nbits */
+    int32_t seg_end0, seg_end1;
+} b200sd_lut_args;
+
+int b200sd_gemm_lut(const b200sd_gemm_args* args, const b200sd_lut_args* lut, void* stream);
+/* host-only: the tiling of b200sd_gemm_lut as "key=value" fields (b200sd_gemm_describe_plan's, plus stages, pk_slots:
+ * packed-index slots in shared memory, pk_box: bytes per row of a slot, smem: dynamic shared memory bytes) */
+int b200sd_gemm_describe_plan_lut(const b200sd_gemm_args* args, const b200sd_lut_args* lut, char* buf, size_t buf_size);
+
 /* small-M linear on CUDA cores (weight-bandwidth bound): out[m, n] = act_in(x[m, :]) . W[n, :] + b[n]
  * for the time-embedding MLPs (unet.py:665-682) and the per-ResNet time_emb_proj(silu(emb))
  * (unet.py:442, 476-478).  x, out fp32; W fp16 [n, k]; act_in: 0 none, 1 SiLU on the input;

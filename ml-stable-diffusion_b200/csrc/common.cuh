@@ -41,8 +41,10 @@ void set_error(const char* fmt, ...);
 int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                     const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides);
 // The same encoding for any element type (UINT8 for the int8 convolution: its zero fill is 0 as well).
+// swizzle: SWIZZLE_NONE for boxes that are not operand tiles (the packed palette indices of b200sd_gemm_lut).
 int encode_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
-                const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides);
+                const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides,
+                CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 
 int num_sms();
 

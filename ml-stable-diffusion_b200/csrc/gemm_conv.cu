@@ -102,6 +102,11 @@ struct __align__(64) GemmParams {
     int stage_dedicated;       // the staging tile has its own shared memory (persistent CTAs with several tiles)
     long long* dbg;            // optional timeline of CTA 0 (clock64 at fixed points; tools/halo_timeline.py)
     const float* col_scale;    // int8 convolution: [N] s_a * s_w[n], applied to the int32 accumulators
+    // ---- palettized B operand (b200sd_gemm_lut): tmB maps the packed n-bit indices [N][kb_total * 8 * nbits bytes];
+    // the producer warpgroup decodes each k-block through the row segment's palette into the fp16 B stage ----
+    const __half* lut;         // [3][256] palettes of output rows [0, seg_end0), [seg_end0, seg_end1), [seg_end1, N)
+    const float* kscale;       // [kb_total * 64] per-k scale (LayerNorm fold) or null
+    int nbits, pk_box, pk_slots, seg_end0, seg_end1;
 };
 
 struct TileCoord {
@@ -723,7 +728,61 @@ __device__ __forceinline__ void cluster_splitk_reduce(const GemmParams& p, const
 // kBN: tile width (columns); p.block_n == kBN.  Each consumer thread holds kBN / 2 fp32 accumulators.
 // kS8: int8 operands (k-block = 128 channels, int32 accumulators scaled by p.col_scale into the fp32 ones before the
 // epilogue); T is then the type of the residual and the output.
-template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN, bool kS8>
+// Palettized B operand: shared memory after the B stages holds `pk_slots` packed-index slots of kBN * pk_box bytes, then
+// the three palettes ([3][256] fp16) and the slots' full / empty barriers.  Narrow slots (1 / 2 bits) may outnumber the
+// pipeline stages: a wide tile parks its accumulators over stages and slots together.
+static constexpr int kMaxPkSlots = 32;
+static constexpr int kLutSmem = 3 * 256 * 2 + 2 * kMaxPkSlots * 8;
+static constexpr int kLutDecodeThreads = 96;  // producer warps 9..11 decode; warp 8 keeps issuing TMA
+
+// Little-endian bit stream of one 8-index chunk (nbits bytes at a 2-byte aligned offset for 6 bits, nbits-aligned
+// otherwise; 1 bit: one byte).
+__device__ __forceinline__ uint64_t lut_chunk_bits(const uint8_t* src, int nbits) {
+    switch (nbits) {
+        case 1: return *src;
+        case 2: return *reinterpret_cast<const uint16_t*>(src);
+        case 4: return *reinterpret_cast<const uint32_t*>(src);
+        case 6: {
+            const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
+            return static_cast<uint64_t>(s[0]) | (static_cast<uint64_t>(s[1]) << 16) | (static_cast<uint64_t>(s[2]) << 32);
+        }
+        default: return *reinterpret_cast<const uint64_t*>(src);
+    }
+}
+
+// Decodes k-block kb of the tile at output row n0 from a packed slot into a B stage, in the SWIZZLE_128B layout a TMA
+// load of the fp16 tile writes (16-byte chunk c of row r at chunk c ^ (r & 7)).  Rows >= N decode to zero.
+template <int kBN>
+__device__ __forceinline__ void lut_decode_stage(const GemmParams& p, const uint8_t* pk, uint8_t* dst, const __half* lut_s,
+                                                 int n0, int kb, int dt) {
+    const int boff = p.nbits == 1 ? (kb & 1) * 8 : 0;  // 1 bit: the 16-byte box holds k-blocks (kb & ~1, kb | 1)
+    const uint32_t mask = (1u << p.nbits) - 1u;
+    for (int u = dt; u < kBN * 8; u += kLutDecodeThreads) {
+        const int r = u >> 3, c = u & 7;
+        const int row = n0 + r;
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+        if (row < p.N) {
+            const uint64_t bits = lut_chunk_bits(pk + r * p.pk_box + boff + c * p.nbits, p.nbits);
+            const __half* lut = lut_s + ((row >= p.seg_end0) + (row >= p.seg_end1)) * 256;
+            __half h[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) h[i] = lut[static_cast<uint32_t>(bits >> (i * p.nbits)) & mask];
+            if (p.kscale != nullptr) {
+                const float4* ks = reinterpret_cast<const float4*>(p.kscale + kb * kBK + c * 8);
+                const float4 s0 = __ldg(ks), s1 = __ldg(ks + 1);
+                const float s[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+#pragma unroll
+                for (int i = 0; i < 8; ++i) h[i] = __float2half_rn(__half2float(h[i]) * s[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                w[i] = static_cast<uint32_t>(__half_as_ushort(h[2 * i])) | (static_cast<uint32_t>(__half_as_ushort(h[2 * i + 1])) << 16);
+        }
+        *reinterpret_cast<uint4*>(dst + r * 128 + ((c ^ (r & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+}
+
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN, bool kS8, bool kLut = false>
 __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
     constexpr int kChunk = kS8 ? 2 * kBK : kBK;  // channels per k-block (128 bytes either way)
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
@@ -735,7 +794,13 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
     constexpr int b_stage = kBN * kBK * 2;
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + p.stages * kAStage;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + p.stages * b_stage);
+    // palettized B: packed slots, palettes and slot barriers between the B stages and the barriers of the pipeline
+    const int pk_stage = kLut ? kBN * p.pk_box : 0;
+    uint8_t* smem_pk = smem_b + p.stages * b_stage;
+    __half* lut_s = reinterpret_cast<__half*>(smem_pk + (kLut ? p.pk_slots * pk_stage : 0));
+    uint64_t* pk_full = reinterpret_cast<uint64_t*>(lut_s + 3 * 256);
+    uint64_t* pk_empty = pk_full + kMaxPkSlots;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(kLut ? reinterpret_cast<uint8_t*>(lut_s) + kLutSmem : smem_pk);
     uint64_t* empty_bar = full_bar + kMaxStages;
     uint64_t* acc_free = empty_bar + kMaxStages;                     // the pipeline memory is free for the next tile
     float* bias_s = reinterpret_cast<float*>(acc_free + 4);           // [2][block_n] (16 B aligned)
@@ -756,8 +821,15 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
         prefetch_tmap(&p.tmA1);
         prefetch_tmap(&p.tmB);
         for (int s = 0; s < p.stages; ++s) {
-            mbar_init(&full_bar[s], 1);
+            // palettized B: the A load's arrival plus one per decoding thread (each fences its stores to the async proxy)
+            mbar_init(&full_bar[s], kLut ? 1 + kLutDecodeThreads : 1);
             mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
+        }
+        if constexpr (kLut) {
+            for (int s = 0; s < p.pk_slots; ++s) {
+                mbar_init(&pk_full[s], 1);
+                mbar_init(&pk_empty[s], kLutDecodeThreads);
+            }
         }
         mbar_init(acc_free, 1);
         fence_barrier_init();
@@ -780,7 +852,18 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
         if (warp == kProducerWarp && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            const uint32_t tx_bytes = kAStage + b_stage;
+            const uint32_t tx_bytes = kAStage + (kLut ? 0 : b_stage);
+            int ps = 0;  // palettized B: packed slot and its phase
+            uint32_t pph = 0;
+            auto load_pk = [&](const TileCoord& t, int kb) {  // the packed indices of k-block kb into slot ps
+                mbar_expect_tx(&pk_full[ps], pk_stage);
+                const int x = p.nbits == 1 ? (kb >> 1) * 16 : kb * 8 * p.nbits;
+                tma_load_2d(smem_pk + ps * pk_stage, &p.tmB, &pk_full[ps], x, t.n_tile * kBN, kEvictLast);
+                if (++ps == p.pk_slots) {
+                    ps = 0;
+                    pph ^= 1;
+                }
+            };
             auto load_b = [&](const TileCoord& t, int kb, int st) {
                 const int tap = kb / p.kc;
                 const int j = kb - tap * p.kc;
@@ -815,14 +898,18 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
             };
             // ---- weight prefetch ahead of the grid dependency (constant weights only: pre-tiled B operands) ----
             int npre = 0;
-            if (p.wgt_tiled && work0 < total_work) {
+            if ((kLut || p.wgt_tiled) && work0 < total_work) {
                 const TileCoord t = decode_work(p, work0);
                 int kb0, kb1;
                 split_range(p, t.split, kb0, kb1);
-                npre = min(p.stages, kb1 - kb0);
+                npre = min(kLut ? min(p.stages, p.pk_slots) : p.stages, kb1 - kb0);
                 for (int i = 0; i < npre; ++i) {
-                    mbar_expect_tx(&full_bar[i], tx_bytes);
-                    load_b(t, kb0 + i, i);
+                    if constexpr (kLut) {
+                        load_pk(t, kb0 + i);  // stages and slots are all free before the first tile
+                    } else {
+                        mbar_expect_tx(&full_bar[i], tx_bytes);
+                        load_b(t, kb0 + i, i);
+                    }
                 }
             }
             pdl_wait();
@@ -834,7 +921,17 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
                 split_range(p, t.split, kb0, kb1);
                 if (iter > 0) mbar_wait(acc_free, (iter - 1) & 1);  // the previous tile's epilogue left the stages
                 for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                    if (it >= npre) {
+                    if constexpr (kLut) {
+                        // the packed slot is loaded only once the B stage it decodes into is free, so a decoder that
+                        // sees the slot full may write the stage
+                        if (it >= npre) mbar_wait(&empty_bar[stage], phase ^ 1);
+                        mbar_expect_tx(&full_bar[stage], tx_bytes);
+                        load_a(t, kb, stage);
+                        if (it >= npre) {
+                            mbar_wait(&pk_empty[ps], pph ^ 1);
+                            load_pk(t, kb);
+                        }
+                    } else if (it >= npre) {
                         mbar_wait(&empty_bar[stage], phase ^ 1);
                         mbar_expect_tx(&full_bar[stage], tx_bytes);
                         load_a(t, kb, stage);
@@ -845,6 +942,31 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
                     if (++stage == p.stages) {
                         stage = 0;
                         phase ^= 1;
+                    }
+                }
+            }
+        } else if (kLut && warp > kProducerWarp) {
+            // ---- palettized B: warps 9..11 decode each packed slot into its B stage (constant operands only: no
+            // griddepcontrol.wait needed) ----
+            const int dt = threadIdx.x - (kProducerWarp + 1) * 32;
+            for (int i = dt; i < 3 * 256; i += kLutDecodeThreads) lut_s[i] = p.lut[i];
+            asm volatile("bar.sync 2, %0;" ::"n"(kLutDecodeThreads) : "memory");
+            int stage = 0, ps = 0;
+            uint32_t pph = 0;
+            for (int work = work0; work < total_work; work += work_step) {
+                const TileCoord t = decode_work(p, work);
+                int kb0, kb1;
+                split_range(p, t.split, kb0, kb1);
+                for (int kb = kb0; kb < kb1; ++kb) {
+                    mbar_wait(&pk_full[ps], pph);
+                    lut_decode_stage<kBN>(p, smem_pk + ps * pk_stage, smem_b + stage * b_stage, lut_s, t.n_tile * kBN, kb, dt);
+                    fence_proxy_async_smem();  // the generic-proxy stores become visible to wgmma
+                    mbar_arrive(&full_bar[stage]);
+                    mbar_arrive(&pk_empty[ps]);
+                    if (++stage == p.stages) stage = 0;
+                    if (++ps == p.pk_slots) {
+                        ps = 0;
+                        pph ^= 1;
                     }
                 }
             }
@@ -1020,6 +1142,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __gri
     gemm_kernel_body<T, kGeneric, kGeglu, kOutF32, kPartial, kStaged, kBN, false>(p);
 }
 
+// Palettized weights (b200sd_gemm_lut): the fp16 kernel with a B operand decoded from n-bit palette indices.  Variants:
+// generic, plain, split-K and GEGLU epilogues (nbits is a runtime switch of the decoder).
+template <bool kGeneric, bool kGeglu, bool kPartial, int kBN>
+__global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_lut_kernel(const __grid_constant__ GemmParams p) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gemm_kernel_body<__half, kGeneric, kGeglu, false, kPartial, false, kBN, false, true>(p);
+}
+
 // W8A8 3x3 convolution (b200sd_gemm_s8): int8 NHWC activations and pre-tiled int8 weights on IGMMA, fp16 residual and
 // output.  Variants: generic, plain and split-K epilogues.
 template <bool kGeneric, bool kPartial, int kBN>
@@ -1067,6 +1197,21 @@ static KernelFn s8_kernel(int width_index) {
                                                  B200SD_S8_FN(128), B200SD_S8_FN(96),  B200SD_S8_FN(64),
                                                  B200SD_S8_FN(32),  B200SD_S8_FN(16)};
 #undef B200SD_S8_FN
+    return fns[width_index];
+}
+
+template <bool kGeneric, bool kGeglu, bool kPartial, int kBN>
+static constexpr KernelFn lut_fn() {
+    if constexpr (kBN == 16 && !kGeneric) return nullptr;  // the regular variants need block_n % 32 == 0
+    else return wgmma_gemm_lut_kernel<kGeneric, kGeglu, kPartial, kBN>;
+}
+template <bool kGeneric, bool kGeglu, bool kPartial>
+static KernelFn lut_kernel(int width_index) {
+#define B200SD_LUT_FN(bn) lut_fn<kGeneric, kGeglu, kPartial, bn>()
+    static const KernelFn fns[kNumGemmWidths] = {B200SD_LUT_FN(256), B200SD_LUT_FN(192), B200SD_LUT_FN(160),
+                                                 B200SD_LUT_FN(128), B200SD_LUT_FN(96),  B200SD_LUT_FN(64),
+                                                 B200SD_LUT_FN(32),  B200SD_LUT_FN(16)};
+#undef B200SD_LUT_FN
     return fns[width_index];
 }
 
@@ -1518,6 +1663,7 @@ struct GemmPlan {
     int cs_slots;  // statistics slots per image this tiling produces (0: column statistics not available)
     int smem_bytes;
     int variant;    // GEMM kernel: one of GemmVariant (-1 for the halo convolution)
+    int pk_box, pk_slots;  // palettized B: bytes per tile row of a packed slot, slots in the ring (0: fp16 B operand)
     int halo_kind;  // halo convolution: 0 loader warps + staged epilogue, 1 fp32 / narrow epilogue, 2 TMA patches (-1: GEMM)
 };
 
@@ -1878,13 +2024,60 @@ static size_t plan_workspace(const GemmPlan& pl) {
     return (pl.splits > 1 && !pl.cluster) ? static_cast<size_t>(pl.splits) * pl.M * pl.N * sizeof(float) : 0;
 }
 
+// Palettized B operand (b200sd_gemm_lut): the fp16 plan of the same arguments -- tile width, split-K and k order, so
+// the launch is bit-identical to b200sd_gemm on the decoded weights -- with a pipeline depth that makes room for the
+// packed-index slots.  The accumulator tile is parked over the A / B stages and the slots (contiguous, all drained
+// at the end of a tile).
+static int plan_lut(const b200sd_gemm_args& a, const b200sd_lut_args& l, GemmPlan& pl) {
+    B200SD_REQUIRE(l.nbits == 1 || l.nbits == 2 || l.nbits == 4 || l.nbits == 6 || l.nbits == 8,
+                   "b200sd_gemm_lut: nbits=%d is not supported (1, 2, 4, 6 or 8)", l.nbits);
+    B200SD_REQUIRE(!a.wgt_tiled, "b200sd_gemm_lut: wgt_tiled is not supported (the packed indices are the B operand)");
+    B200SD_REQUIRE(!a.halo && !a.upsample2x && a.gn_groups == 0, "b200sd_gemm_lut: halo / upsample2x / gn_* are not supported");
+    B200SD_REQUIRE(!a.cs_partial && !a.cs_chan && !a.cs_tickets, "b200sd_gemm_lut: cs_* (column statistics) are not supported");
+    B200SD_REQUIRE(!a.a2 && !a.a3 && a.c2 == 0 && a.c3 == 0, "b200sd_gemm_lut: a2 / a3 (folded shortcut) are not supported");
+    B200SD_REQUIRE(!a.out_f32, "b200sd_gemm_lut: out_f32 is not supported");
+    // whole 64-channel k-blocks per source: k-block kb holds weight columns [64 kb, 64 kb + 64), no padding positions
+    B200SD_REQUIRE(a.c0 % kBK == 0 && a.c1 % kBK == 0, "b200sd_gemm_lut: c0=%d / c1=%d must be multiples of 64", a.c0, a.c1);
+    B200SD_REQUIRE(l.packed && l.lut, "b200sd_gemm_lut: packed / lut is null");
+    B200SD_REQUIRE((reinterpret_cast<uintptr_t>(l.kscale) & 15) == 0, "b200sd_gemm_lut: kscale %p is not 16-byte aligned",
+                   static_cast<const void*>(l.kscale));
+    B200SD_REQUIRE(0 <= l.seg_end0 && l.seg_end0 <= l.seg_end1, "b200sd_gemm_lut: bad row segments (%d, %d)", l.seg_end0, l.seg_end1);
+    if (int rc = plan_gemm(a, pl)) return rc;
+    B200SD_REQUIRE(!pl.staged, "b200sd_gemm_lut: the staged epilogue is not supported");
+    const long row_min = (pl.kb_total * 8L * l.nbits + 15) / 16 * 16;
+    B200SD_REQUIRE(l.row_bytes % 16 == 0 && l.row_bytes >= row_min, "b200sd_gemm_lut: row_bytes=%d (need a multiple of 16 >= %ld)",
+                   l.row_bytes, row_min);
+    pl.pk_box = std::max(16, 8 * l.nbits);  // TMA boxes are at least 16 bytes wide: at 1 bit one box holds two k-blocks
+    const int per_stage = kAStage + pl.block_n * kBK * 2;
+    const int pk_stage = pl.block_n * pl.pk_box;
+    const int fixed = pl.smem_bytes - pl.stages * per_stage + kLutSmem;
+    const int limit = std::min(227 * 1024, std::max(smem_budget(), pl.smem_bytes));
+    const int park = kBM * (pl.block_n + 4) * 4;
+    int best_s = 0, best_k = 0;
+    for (int s = pl.stages; s >= 2; --s) {
+        const int k = std::min(kMaxPkSlots, (limit - fixed - s * per_stage) / pk_stage);
+        if (k < 2 || s * per_stage + k * pk_stage < park) continue;
+        if (std::min(s, k) > std::min(best_s, best_k)) best_s = s, best_k = k;
+    }
+    B200SD_REQUIRE(best_s > 0, "b200sd_gemm_lut: the pipeline does not fit in shared memory (block_n=%d nbits=%d)", pl.block_n, l.nbits);
+    pl.stages = best_s;
+    pl.pk_slots = best_k;
+    pl.smem_bytes = fixed + best_s * per_stage + best_k * pk_stage;
+    return 0;
+}
+
 extern void count_launch(int n);
 
-static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16, const float* col_scale = nullptr) {
+static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16, const float* col_scale = nullptr,
+                       const b200sd_lut_args* lut = nullptr) {
     const bool s8 = col_scale != nullptr;
     GemmPlan pl;
-    if (int rc = plan_gemm(a, pl, bf16, s8)) return rc;
-    B200SD_REQUIRE(a.a0 && a.wgt && a.out, "b200sd_gemm: null pointer");
+    if (lut) {
+        if (int rc = plan_lut(a, *lut, pl)) return rc;
+    } else if (int rc = plan_gemm(a, pl, bf16, s8)) {
+        return rc;
+    }
+    B200SD_REQUIRE(a.a0 && (a.wgt || lut) && a.out, "b200sd_gemm: null pointer");
     B200SD_REQUIRE(!s8 || a.wgt_tiled, "b200sd_gemm_s8: the weights must be pre-tiled (wgt_tiled = 1, explicit block_n)");
     B200SD_REQUIRE(a.c1 == 0 || a.a1, "b200sd_gemm: a1 is null but c1 > 0");
     const size_t ws = plan_workspace(pl);
@@ -1960,7 +2153,19 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
             if (int rc = encode_tmap_f16(maps[src], ptrs[src], 4, dims, str, box, es)) return rc;
         }
     }
-    if (s8) {
+    if (lut) {
+        // packed indices [N][row_bytes], one box = pk_box bytes of block_n rows (rows >= N are zero filled)
+        const uint64_t dims[2] = {static_cast<uint64_t>(lut->row_bytes), static_cast<uint64_t>(a.n)};
+        const uint64_t str[1] = {static_cast<uint64_t>(lut->row_bytes)};
+        const uint32_t box[2] = {static_cast<uint32_t>(pl.pk_box), static_cast<uint32_t>(pl.block_n)};
+        if (int rc = encode_tmap(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, lut->packed, 2, dims, str, box, es1,
+                                 CU_TENSOR_MAP_SWIZZLE_NONE))
+            return rc;
+        p.lut = reinterpret_cast<const __half*>(lut->lut);
+        p.kscale = lut->kscale;
+        p.nbits = lut->nbits, p.pk_box = pl.pk_box, p.pk_slots = pl.pk_slots;
+        p.seg_end0 = lut->seg_end0, p.seg_end1 = lut->seg_end1;
+    } else if (s8) {
         B200SD_REQUIRE(a.block_n == pl.block_n, "b200sd_gemm_s8: tiled weights need an explicit block_n");
         const uint64_t rows = static_cast<uint64_t>(pl.n_tiles) * pl.kb_total * pl.block_n;
         const uint64_t dims[2] = {2 * kBK, rows};
@@ -2073,7 +2278,15 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
     const int variant = pl.variant;
     KernelFn fn = nullptr;
     p.col_scale = col_scale;
-    if (s8) {  // plan_gemm gives int8 only these three variants
+    if (lut) {
+        switch (variant) {
+            case kVariantGeneric: fn = lut_kernel<true, false, false>(wi); break;
+            case kVariantSplitK: fn = lut_kernel<false, false, true>(wi); break;
+            case kVariantGeglu: fn = lut_kernel<false, true, false>(wi); break;
+            case kVariantPlain: fn = lut_kernel<false, false, false>(wi); break;
+            default: break;
+        }
+    } else if (s8) {  // plan_gemm gives int8 only these three variants
         switch (variant) {
             case kVariantGeneric: fn = s8_kernel<true, false>(wi); break;
             case kVariantSplitK: fn = s8_kernel<false, true>(wi); break;
@@ -2097,15 +2310,16 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
             default: fn = gemm_kernel<__half, false, false, false, false, false>(wi); break;
         }
     }
-    B200SD_REQUIRE(fn != nullptr, "b200sd_gemm: no %s kernel for variant %d at block_n %d", s8 ? "int8" : (bf16 ? "bf16" : "fp16"),
+    B200SD_REQUIRE(fn != nullptr, "b200sd_gemm: no %s kernel for variant %d at block_n %d",
+                   lut ? "palettized" : (s8 ? "int8" : (bf16 ? "bf16" : "fp16")),
                    variant, pl.block_n);
     if (pl.splits > 1 && !pl.cluster) {
         // the separate reduce kernel applies bias / residual; the partial writer must not
         p.bias = nullptr;
         p.residual = nullptr;
     }
-    static bool attr_set[3][6][kNumGemmWidths] = {};
-    const int dt = s8 ? 2 : (bf16 ? 1 : 0);
+    static bool attr_set[4][6][kNumGemmWidths] = {};
+    const int dt = lut ? 3 : (s8 ? 2 : (bf16 ? 1 : 0));
     if (!attr_set[dt][variant][wi]) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set[dt][variant][wi] = true;
@@ -2170,6 +2384,26 @@ extern "C" int b200sd_gemm_s8(const b200sd_gemm_args* args, const float* col_sca
         return 2;
     }
     return gemm_entry(args, stream, false, col_scale);
+}
+
+extern "C" int b200sd_gemm_lut(const b200sd_gemm_args* args, const b200sd_lut_args* lut, void* stream) {
+    if (!b200sd::launch_class_enabled(1)) return 0;  // bench.py's per-class timing graphs
+    if (!args || !lut) {
+        b200sd::set_error("b200sd_gemm_lut: args or lut is null");
+        return 2;
+    }
+    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream), false, nullptr, lut);
+}
+
+extern "C" int b200sd_gemm_describe_plan_lut(const b200sd_gemm_args* args, const b200sd_lut_args* lut, char* buf, size_t buf_size) {
+    if (!args || !lut || !buf || buf_size == 0) return 2;
+    b200sd::GemmPlan pl;
+    if (int rc = b200sd::plan_lut(*args, *lut, pl)) return rc;
+    snprintf(buf, buf_size, "M=%d N=%d kb_total=%d m_tiles=%d n_tiles=%d block_n=%d splits=%d kb_per_split=%d stages=%d "
+             "pk_slots=%d pk_box=%d cluster=%d variant=%d smem=%d",
+             pl.M, pl.N, pl.kb_total, pl.m_tiles, pl.n_tiles, pl.block_n, pl.splits, pl.kb_per_split, pl.stages,
+             pl.pk_slots, pl.pk_box, pl.cluster, pl.variant, pl.smem_bytes);
+    return 0;
 }
 
 extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {

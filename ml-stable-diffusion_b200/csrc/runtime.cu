@@ -71,7 +71,7 @@ int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t
 }
 
 int encode_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
-                const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides) {
+                const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides, CUtensorMapSwizzle swizzle) {
     EncodeTiledFn fn = get_encode_fn();
     B200SD_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
     B200SD_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor map base %p is not 16-byte aligned", base);
@@ -88,7 +88,7 @@ int encode_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, i
         }
     }
     CUresult r = fn(map, dtype, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gd,
-                    gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                    gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B200SD_REQUIRE(r == CUDA_SUCCESS,
                    "cuTensorMapEncodeTiled failed (CUresult %d; rank %d dims %llu,%llu,%llu,%llu box %u,%u,%u,%u)",

@@ -40,6 +40,12 @@ class GemmArgs(C.Structure):
     ]
 
 
+class LutArgs(C.Structure):
+    """b200sd_lut_args: the palettized B operand of b200sd_gemm_lut."""
+    _fields_ = [("packed", C.c_void_p), ("lut", C.c_void_p), ("kscale", C.c_void_p), ("nbits", C.c_int32),
+                ("row_bytes", C.c_int32), ("seg_end0", C.c_int32), ("seg_end1", C.c_int32)]
+
+
 class StepCoeffs(C.Structure):
     _fields_ = [
         ("guidance", C.c_float), ("cx", C.c_float), ("ce", C.c_float), ("ch", C.c_float * 4),
@@ -106,6 +112,8 @@ _SIGNATURES = {
     "b200sd_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     # W8A8 (int8 wgmma) 3x3 convolution and its operand producers
     "b200sd_gemm_s8": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p, C.c_void_p]),
+    "b200sd_gemm_lut": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(LutArgs), C.c_void_p]),
+    "b200sd_gemm_describe_plan_lut": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(LutArgs), C.c_char_p, C.c_size_t]),
     "b200sd_gemm_plan_ex_s8": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(C.c_int32)]),
     "b200sd_gemm_describe_plan_s8": (C.c_int, [C.POINTER(GemmArgs), C.c_char_p, C.c_size_t]),
     "b200sd_gemm_workspace_bytes_s8": (C.c_size_t, [C.POINTER(GemmArgs)]),
@@ -361,6 +369,39 @@ def _maybe_tile_weights(args, wgt, taps):
     args.wgt_tiled = 1
 
 
+def lut_args(pw):
+    """LutArgs of a palettization.PalettizedWeight."""
+    la = LutArgs()
+    la.packed, la.lut = pw.packed.data_ptr(), pw.lut.data_ptr()
+    la.kscale = None if pw.kscale is None else pw.kscale.data_ptr()
+    la.nbits, la.row_bytes = pw.nbits, pw.packed.shape[1]
+    la.seg_end0, la.seg_end1 = pw.seg_ends
+    return la
+
+
+def describe_plan_lut(args, pw) -> str:
+    """Host-only: the tiling b200sd_gemm_lut would choose for these args and palettized weight."""
+    buf = C.create_string_buffer(512)
+    _check(load().b200sd_gemm_describe_plan_lut(C.byref(args), C.byref(lut_args(pw)), buf, 512),
+           "b200sd_gemm_describe_plan_lut")
+    return buf.value.decode()
+
+
+def _is_lut(wgt):
+    return hasattr(wgt, "packed") and hasattr(wgt, "lut")
+
+
+def _run_gemm_lut(args, pw, device):
+    """b200sd_gemm_lut: `pw` (a palettization.PalettizedWeight) is the B operand, on the fp16 plan of `args`."""
+    args.wgt, args.wgt_tiled = None, 0
+    need = gemm_workspace_bytes(args)
+    if need:
+        ws = _workspace(need, device)
+        args.workspace = ws.data_ptr()
+        args.workspace_bytes = ws.numel() * 4
+    _check(load().b200sd_gemm_lut(C.byref(args), C.byref(lut_args(pw)), _stream()), "b200sd_gemm_lut")
+
+
 def gemm_workspace_bytes(args) -> int:
     return int(load().b200sd_gemm_workspace_bytes(C.byref(args)))
 
@@ -468,19 +509,27 @@ def linear(x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=
     ln: LayerNorm of x folded into this GEMM (wgt = gamma (.) W, bias = W beta + b; dict(stat, parts, wg, eps));
     stats / rowstats: dicts that receive the per-channel / per-row sums of the output (see _fused_args)."""
     dt = _act_dtype(x, "linear x")
-    _req(wgt, dt, "linear wgt")
+    lut = _is_lut(wgt)
+    if lut:
+        if dt != torch.float16:
+            raise B200SDError("linear: palettized weights need fp16 activations")
+    else:
+        _req(wgt, dt, "linear wgt")
     _same16(dt, x1, residual, "linear x1 / residual")
     m, n = x.shape[0], wgt.shape[0]
     n_out = n // 2 if geglu else n
     if out is None:
         out = torch.empty(m, n_out, dtype=out_dtype or dt, device=x.device)
     _check_out(out, dt, "linear out")
-    args = gemm_args(0, x, wgt, out, a1=x1, bias=bias, residual=residual, m=m, n=n, geglu=geglu,
+    args = gemm_args(0, x, wgt.packed if lut else wgt, out, a1=x1, bias=bias, residual=residual, m=m, n=n, geglu=geglu,
                      bias_rows=bias_rows, bias_stride=bias_stride, split_k=split_k, block_n=block_n, act=act)
     if ln is not None or stats is not None or rowstats is not None:
         args.split_k = 1
         _keep = _fused_args(args, x.device, n_img=(m // cs_hw if cs_hw else 0), cout=n, stats=stats, cs_hw=cs_hw, ln=ln,
                             rowstats=rowstats, m=m)
+    if lut:
+        _run_gemm_lut(args, wgt, x.device)
+        return out
     if static_w and TILED_WEIGHTS:
         _maybe_tile_weights(args, wgt, 1)
     bf16 = dt == torch.bfloat16
@@ -510,7 +559,12 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=No
     x bf16 runs the bf16 kernels (no halo / gn / upsample / stats / shortcut): wgt, x1, residual and a 16-bit output
     are bf16 too (out_dtype None: x's type)."""
     dt = _act_dtype(x, "conv3x3 x")
-    _req(wgt, dt, "conv3x3 wgt")
+    lut = _is_lut(wgt)
+    if lut:
+        if dt != torch.float16 or halo or shortcut is not None:
+            raise B200SDError("conv3x3: palettized weights need fp16 activations and the 9-tap kernel without a folded shortcut")
+    else:
+        _req(wgt, dt, "conv3x3 wgt")
     _same16(dt, x1, residual, "conv3x3 x1 / residual")
     nimg, h, w, _ = x.shape
     if upsample:
@@ -522,7 +576,7 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=No
     _check_out(out, dt, "conv3x3 out")
     if (gn is not None or upsample or taps == 1) and not halo:
         raise B200SDError("conv3x3: gn / upsample / taps=1 need halo=True")
-    args = gemm_args(1 if taps == 9 else 0, x, wgt, out, a1=x1, bias=bias, residual=residual, n=cout, n_img=nimg, h=h, w=w,
+    args = gemm_args(1 if taps == 9 else 0, x, wgt.packed if lut else wgt, out, a1=x1, bias=bias, residual=residual, n=cout, n_img=nimg, h=h, w=w,
                      stride=stride, bias_rows=bias_rows, bias_stride=bias_stride, split_k=split_k, block_n=block_n, act=act,
                      pad_after_only=pad_after_only, m=(nimg * h * w if taps == 1 else 0))
     args.halo, args.upsample2x = int(halo), int(upsample)
@@ -540,6 +594,9 @@ def conv3x3(x, wgt, bias=None, residual=None, *, x1=None, stride=1, out_dtype=No
         args.split_k = 1
         _keep = _fused_args(args, x.device, n_img=nimg, cout=cout, gn=gn, stats=stats, cs_hw=ho * wo, rowstats=rowstats,
                             m=nimg * ho * wo)
+    if lut:
+        _run_gemm_lut(args, wgt, x.device)
+        return out
     if halo and not (static_w and TILED_WEIGHTS):
         raise B200SDError("conv3x3: the halo kernel needs static pre-tiled weights")
     if static_w and TILED_WEIGHTS:

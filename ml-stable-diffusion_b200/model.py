@@ -54,9 +54,9 @@ class UNetModel(B200Model):
     -> {"noise_pred": fp32}`` (pipeline.py:531-536)."""
 
     def __init__(self, cfg, state_dict, batch=2, height=64, width=64, seq_len=77, device="cuda",
-                 use_cuda_graph=True, io_dtype=np.float16, quantization=None):
-        """quantization: a W8A8Recipe or the path of a saved one (UNetEngine)."""
-        self.engine = UNetEngine(cfg, state_dict, device, quantization=quantization)
+                 use_cuda_graph=True, io_dtype=np.float16, quantization=None, palettization=None):
+        """quantization: a W8A8Recipe or the path of a saved one; palettization: n-bit palettized weights (UNetEngine)."""
+        self.engine = UNetEngine(cfg, state_dict, device, quantization=quantization, palettization=palettization)
         e = self.engine
         self.batch, self.h, self.w, self.seq = batch, height, width, seq_len
         self.in_channels = e.in_ch  # the reference pipeline sets/reads this (pipeline.py:104)

@@ -245,7 +245,8 @@ class B200StableDiffusionPipeline:
     @classmethod
     def from_pretrained(cls, model_dir, images_per_call=1, device="cuda", height=None, width=None,
                         scheduler_override=None, controlnet_dirs=None, force_zeros_for_empty_prompt=None,
-                        with_vae_encoder=False, refiner_dir=None, load_safety_checker=True, unet_quantization=None):
+                        with_vae_encoder=False, refiner_dir=None, load_safety_checker=True, unet_quantization=None,
+                        unet_palettization=None):
         """Build the pipeline from a diffusers-layout model directory (``unet/``, ``vae/``, ``text_encoder[_2]/``,
         ``tokenizer[_2]/``, ``scheduler/``): the counterpart of ``get_coreml_pipe(pytorch_pipe, mlpackages_dir,
         model_version, compute_unit, scheduler_override, controlnet_models, force_zeros_for_empty_prompt)``
@@ -255,7 +256,9 @@ class B200StableDiffusionPipeline:
         ``load_safety_checker``: load ``safety_checker/`` with ``feature_extractor/`` when the directory has them (SD 1.4
         / 1.5; get_coreml_pipe loads it whenever the diffusers pipeline has one, pipeline.py:650-656); False skips it.
         ``unet_quantization``: a ``quantization.W8A8Recipe`` or the path of a saved one (``calibrate_unet``); the base
-        UNet runs the convolutions it names in W8A8.  The refiner, ControlNets, VAE and text encoders stay fp16."""
+        UNet runs the convolutions it names in W8A8.  The refiner, ControlNets, VAE and text encoders stay fp16.
+        ``unet_palettization``: n-bit palettized base-UNet weights -- an nbits int, a {layer: nbits} dict or
+        (pre-analysis json path, recipe key) (``palettization.as_recipe``); the same components stay fp16."""
         import json
         import os
         from . import checkpoint as K
@@ -272,7 +275,7 @@ class B200StableDiffusionPipeline:
         w = (width // f) if width else size
         xl = ucfg.get("addition_embed_type") == "text_time"
         unet = UNetModel(ucfg, K.load_component(model_dir, "unet", ucfg), batch=2 * images_per_call, height=h, width=w,
-                         device=device, quantization=unet_quantization)
+                         device=device, quantization=unet_quantization, palettization=unet_palettization)
         vsd = K.read_state_dict(os.path.join(model_dir, "vae"))
         vdtype = vae_dtype(ucfg, vcfg)
         vae = VAEDecoderModel(vcfg, K.check_state_dict("vae_decoder", vcfg, vsd), batch=images_per_call, height=h,

@@ -25,6 +25,7 @@ import os
 import torch
 
 from . import lib as L
+from . import palettization as Pz
 from . import quantization as Q
 
 
@@ -84,9 +85,13 @@ class _Packer:
 class UNetEngine:
     """Holds device-resident packed weights and issues the forward launch sequence."""
 
-    def __init__(self, cfg: dict, state_dict: dict, device="cuda", quantization=None):
+    def __init__(self, cfg: dict, state_dict: dict, device="cuda", quantization=None, palettization=None):
         """quantization: a W8A8Recipe (or the path of a saved one): the ResNet / up-sampler convolutions it names run
-        on the int8 convolution kernel with its activation scales; every other layer is unchanged."""
+        on the int8 convolution kernel with its activation scales; every other layer is unchanged.
+        palettization: n-bit palettized weights (palettization.as_recipe: an nbits int, a {layer: nbits} dict or
+        (json path, recipe key)).  The layers run per step keep only packed indices and palettes on the device and
+        decode them in the GEMM kernel; the once-per-call layers (time / add embeddings, time_emb_proj, cross-attention
+        to_k / to_v) hold their decoded fp16 values.  Either way the numbers are those of palettization.decoded_state_dict."""
         L.load()
         self.cfg = dict(cfg)
         self.dev = torch.device(device)
@@ -133,6 +138,15 @@ class UNetEngine:
         if self.recipe is not None:
             self._require_default_level("a W8A8 recipe")
             self.recipe.validate(self.cfg)
+        self.palettization = Pz.as_recipe(palettization, self.cfg)
+        if self.palettization is not None:
+            if self.recipe is not None:
+                raise ValueError("palettization cannot be combined with a W8A8 recipe")
+            self._require_default_level("palettization")
+            if not L.TILED_WEIGHTS:
+                raise ValueError("palettization needs B200SD_TILED_W=1 (the default)")
+            if os.environ.get("B200SD_STAGED", "0") == "1":
+                raise ValueError("palettization cannot be combined with B200SD_STAGED=1 (the staged epilogue)")
         L.reserve_attention_workspace(self.dev, max(c // h for c, h in zip(boc, self.heads)))
         self._pack(state_dict)
 
@@ -146,6 +160,37 @@ class UNetEngine:
 
     # ------------------------------------------------------------------ packing
     def _pack(self, sd):
+        # palettized layers: one palette per weight; everything below is packed from the decoded values, then the
+        # per-step launches' fp16 operands are replaced by their packed indices (PalettizedWeight)
+        fits = {}  # layer -> (palette, indices on the host, nbits); each launch packs its indices on the device
+        for name, nbits in (self.palettization or {}).items():
+            lut, idx = Pz.fit_palette(sd[name + ".weight"].to(self.dev), nbits)
+            fits[name] = (lut, idx.cpu(), nbits)
+        if fits:
+            sd = dict(sd)
+            for name, (lut, idx, _) in fits.items():
+                sd[name + ".weight"] = Pz.decode(lut, idx).cpu()
+
+        def seg(name, conv3=False):
+            lut, idx, nbits = fits[name]
+            idx = idx.permute(0, 2, 3, 1) if conv3 else idx
+            return lut, idx.reshape(idx.shape[0], -1).to(self.dev), nbits
+
+        def lutw(names, conv3=False, kscale=None, rows=None):
+            """PalettizedWeight of a launch whose weight rows are these layers' (all palettized), else None.  A fused
+            launch with an fp16 member (attn1 to_q | to_k | to_v with a 16-bit entry) stays fp16 as a whole: its
+            palettized members are held decoded (stored_bits() reports them at 16)."""
+            if not names or any(n not in fits for n in names):
+                return None
+            segs = [seg(n, conv3) for n in names]
+            lay = list(names)
+            if rows is not None:
+                lut, idx, nbits = segs[0]
+                segs = [(lut, rows(idx), nbits)]
+            pw = Pz.palettized(segs, kscale)
+            pw.layers = lay
+            return pw
+
         P = _Packer(sd, self.dev)
         w = {}
         self.temb_slices = {}   # resnet prefix -> (offset, cout)
@@ -170,9 +215,14 @@ class UNetEngine:
                 r["scb"] = P.bias(p + ".conv_shortcut")
                 # the shortcut folded into conv2: its [Cout, Cin] matrix appended along K (extra centre-tap k-blocks of
                 # the same convolution launch, lib.conv3x3(shortcut=...)), one bias vector for both
-                if self.fold_shortcut and not self.fuse_gn and self.fused:
+                if (self.fold_shortcut and not self.fuse_gn and self.fused and (p + ".conv2") not in fits
+                        and (p + ".conv_shortcut") not in fits):
                     r["c2sc"] = torch.cat([r["c2"], r["sc"]], 1).contiguous()
                     r["c2scb"] = (r["c2b"] + r["scb"]).contiguous()
+            for k, name, conv3 in (("c1", ".conv1", True), ("c2", ".conv2", True), ("sc", ".conv_shortcut", False)):
+                pw = lutw([p + name], conv3)
+                if pw is not None:
+                    r[k] = pw
             w[p] = r
 
         def transformer(p, c, depth):
@@ -180,6 +230,10 @@ class UNetEngine:
             t = {"ng": P.f32(p + ".norm.weight"), "nb": P.f32(p + ".norm.bias"),
                  "pi": P.lin(p + ".proj_in"), "pib": P.bias(p + ".proj_in"),
                  "po": P.lin(p + ".proj_out"), "pob": P.bias(p + ".proj_out"), "blocks": []}
+            for k, name in (("pi", ".proj_in"), ("po", ".proj_out")):
+                pw = lutw([p + name])
+                if pw is not None:
+                    t[k] = pw
             for d in range(depth):
                 b = f"{p}.transformer_blocks.{d}"
                 blk = {}
@@ -212,6 +266,20 @@ class UNetEngine:
                         if bkey is not None:
                             bias = bias + blk[bkey]
                         blk[name + "_lnb"] = bias.contiguous()
+                names = {"qkv": [f"{b}.attn1.to_{n}" for n in "qkv"], "q2": [f"{b}.attn2.to_q"],
+                         "gg": [f"{b}.ff.net.0.proj"]}
+                for name, ln in (("qkv", 1), ("q2", 2), ("gg", 3)):
+                    rows = (lambda i: torch.stack([i[: i.shape[0] // 2], i[i.shape[0] // 2:]], 1).reshape(i.shape)) \
+                        if name == "gg" else None
+                    pw = lutw(names[name], rows=rows, kscale=blk[f"ln{ln}g"] if self.fused else None)
+                    if pw is not None:
+                        blk[name + ("_ln" if self.fused else "")] = pw
+                        if self.fused:
+                            del blk[name]  # only the folded launch runs
+                for k, name in (("o1", "attn1.to_out.0"), ("o2", "attn2.to_out.0"), ("f2", "ff.net.2")):
+                    pw = lutw([f"{b}.{name}"])
+                    if pw is not None:
+                        blk[k] = pw
                 t["blocks"].append(blk)
             w[p] = t
 
@@ -229,7 +297,7 @@ class UNetEngine:
                     transformer(f"down_blocks.{i}.attentions.{j}", boc[i], self.depth[i])
             if i != nb - 1:
                 p = f"down_blocks.{i}.downsamplers.0.conv"
-                w[p] = {"w": P.conv3(p), "b": P.bias(p)}
+                w[p] = {"w": lutw([p], True) or P.conv3(p), "b": P.bias(p)}
         resnet("mid_block.resnets.0")
         transformer("mid_block.attentions.0", boc[-1], self.mid_depth)
         resnet("mid_block.resnets.1")
@@ -241,7 +309,7 @@ class UNetEngine:
                     transformer(f"up_blocks.{i}.attentions.{j}", rboc[i], rdepth[i])
             if i != nb - 1:
                 p = f"up_blocks.{i}.upsamplers.0.conv"
-                w[p] = {"w": P.conv3(p), "b": P.bias(p)}
+                w[p] = {"w": lutw([p], True) or P.conv3(p), "b": P.bias(p)}
         w["out"] = {"g": P.f32("conv_norm_out.weight"), "b": P.f32("conv_norm_out.bias"),
                     "w": P.conv3("conv_out"), "cb": P.bias("conv_out")}
         self.temb_w = P.f16(torch.cat(temb_w, 0))
@@ -266,10 +334,27 @@ class UNetEngine:
                     w[block].pop(k, None)
         self.weight_bytes = sum(t.numel() * t.element_size() for t in self._tensors())
 
+    def stored_bits(self):
+        """layer -> (nominal bits of the recipe, bits per weight the engine stores: the container width of its launch,
+        or 16 where it is held decoded in fp16).  Palettes and per-k scales are not included."""
+        out = {name: (nbits, 16) for name, nbits in (self.palettization or {}).items()}
+
+        def visit(o):
+            if isinstance(o, Pz.PalettizedWeight):
+                for n in o.layers:
+                    out[n] = (out[n][0], o.nbits)
+            elif isinstance(o, (dict, list)):
+                for v in (o.values() if isinstance(o, dict) else o):
+                    visit(v)
+        visit(self.w)
+        return out
+
     def _tensors(self):
         def walk(o):
             if torch.is_tensor(o):
                 yield o
+            elif isinstance(o, Pz.PalettizedWeight):
+                yield from o.tensors()
             elif isinstance(o, dict):
                 for v in o.values():
                     yield from walk(v)
