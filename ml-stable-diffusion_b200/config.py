@@ -81,6 +81,24 @@ def num_time_ids(cfg, pooled_dim=SDXL_POOLED_DIM) -> int:
     return rest // ate
 
 
+def latent_multiple(cfg) -> int:
+    """What the latent height and width of a UNet or ControlNet must be a multiple of: each of its
+    len(block_out_channels) - 1 down-samplers halves the map (stride 2), and the up-samplers double it back onto the
+    skip connections, so every halving must be exact.  8 (images of a multiple of 64 pixels) for SD 1.x / 2.x and the
+    SDXL refiner, 4 (32 pixels) for SDXL-base."""
+    return 2 ** (len(cfg["block_out_channels"]) - 1)
+
+
+def check_latent_size(cfg, height, width, what="UNet"):
+    """ValueError unless latents of height x width can be halved by every down-sampler of the model
+    (latent_multiple)."""
+    m = latent_multiple(cfg)
+    if height % m or width % m:
+        raise ValueError(f"{what}: latents of {height}x{width} ({8 * height}x{8 * width} pixels) cannot be halved "
+                         f"{len(cfg['block_out_channels']) - 1} times; height and width must be multiples of {8 * m} "
+                         f"pixels ({m} latent pixels) for this model")
+
+
 # small config for fast CPU/GPU parity tests (same topology, d_head = 64)
 TINY_UNET = dict(
     sample_size=16, in_channels=4, out_channels=4,

@@ -8,6 +8,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from . import config as C
 from . import lib as L
 from .model import B200Model
 from .unet import UNetEngine, _Packer
@@ -120,6 +121,7 @@ class ControlNetModel(B200Model):
 
     def __init__(self, cfg, state_dict, batch=2, height=64, width=64, seq_len=77, device="cuda", io_dtype=np.float16,
                  use_cuda_graph=True):
+        C.check_latent_size(cfg, height, width, "ControlNet")
         self.engine = ControlNetEngine(cfg, state_dict, device)
         self.use_cuda_graph = use_cuda_graph
         self._graph = None

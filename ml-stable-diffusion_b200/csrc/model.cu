@@ -859,6 +859,13 @@ extern "C" int b200sd_unet_create(const b200sd_unet_config* cfg, const b200sd_we
     B200SD_REQUIRE(cfg && weights && out && n_weights > 0, "b200sd_unet_create: null argument");
     B200SD_REQUIRE(cfg->n_blocks >= 1 && cfg->n_blocks <= 8 && cfg->batch >= 1 && cfg->height >= 1 && cfg->width >= 1 && cfg->seq_len >= 1,
                    "b200sd_unet_create: bad geometry");
+    {  // every down-sampler halves the map exactly (config.latent_multiple)
+        const int mult = 1 << (cfg->n_blocks - 1);
+        B200SD_REQUIRE(cfg->height % mult == 0 && cfg->width % mult == 0,
+                       "b200sd_unet_create: latents of %dx%d cannot be halved %d times; height and width must be multiples of %d pixels "
+                       "(%d latent pixels) for this model",
+                       cfg->height, cfg->width, cfg->n_blocks - 1, 8 * mult, mult);
+    }
     size_t attn_ws_bytes = 0;  // stream-K workspace for the largest head dim of the net
     for (int i = 0; i < cfg->n_blocks; ++i) {
         const int c = cfg->block_out_channels[i], heads = cfg->attention_heads[i];

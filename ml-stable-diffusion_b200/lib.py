@@ -300,7 +300,18 @@ def describe_plan(mode, m=0, n=0, c0=0, c1=0, n_img=0, h=0, w=0, stride=1, geglu
 
 
 TILED_WEIGHTS = os.environ.get("B200SD_TILED_W", "1") != "0"
-_tiled_cache = {}
+_tiled_cache = {}  # key -> (weakref to the source weight, its _version, packed copy)
+
+
+def _cache_tiled(key, wgt, packed):
+    """Cache `packed` for as long as its source tensor lives: the entry (and the packed device copy) is dropped when
+    `wgt` is freed, so the tiled weights of a model that is gone do not stay resident.  A lookup only ever hits the
+    live source tensor itself, so nothing is lost."""
+    def drop(ref, key=key):
+        if _tiled_cache.get(key, (None,))[0] is ref:  # not an entry a newer tensor at the same address has taken
+            del _tiled_cache[key]
+
+    _tiled_cache[key] = (weakref.ref(wgt, drop), wgt._version, packed)
 
 
 def pack_tiled(w2d, c0, c1, taps, bn, chunk_major=False, extra=(0, 0), chunk=64):
@@ -360,10 +371,7 @@ def _maybe_tile_weights(args, wgt, taps):
         if torch.cuda.is_current_stream_capturing():
             return  # never pack during capture; the warm-up pass has populated the cache for these shapes
         packed = pack_tiled(wgt, args.c0, args.c1, taps, bn, chunk_major=bool(args.halo), extra=(args.c2, args.c3))
-        if len(_tiled_cache) > 4096:  # drop entries whose source tensor is gone
-            for k in [k for k, v in _tiled_cache.items() if v[0]() is None]:
-                del _tiled_cache[k]
-        _tiled_cache[key] = (weakref.ref(wgt), wgt._version, packed)
+        _cache_tiled(key, wgt, packed)
     args.wgt = packed.data_ptr()
     args.block_n = bn
     args.wgt_tiled = 1
@@ -647,7 +655,7 @@ def _tiled_s8(args, wgt):
         raise B200SDError("conv3x3_s8: weights of this shape were not tiled before CUDA-graph capture; run one eager "
                           "call with the same shapes first")
     packed = pack_tiled(wgt, args.c0, 0, 9, bn, chunk=128)
-    _tiled_cache[key] = (weakref.ref(wgt), wgt._version, packed)
+    _cache_tiled(key, wgt, packed)
     return packed, bn
 
 

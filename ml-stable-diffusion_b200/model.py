@@ -14,6 +14,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from . import config as C
 from . import lib as L
 from .unet import UNetEngine
 
@@ -56,6 +57,7 @@ class UNetModel(B200Model):
     def __init__(self, cfg, state_dict, batch=2, height=64, width=64, seq_len=77, device="cuda",
                  use_cuda_graph=True, io_dtype=np.float16, quantization=None, palettization=None):
         """quantization: a W8A8Recipe or the path of a saved one; palettization: n-bit palettized weights (UNetEngine)."""
+        C.check_latent_size(cfg, height, width)
         self.engine = UNetEngine(cfg, state_dict, device, quantization=quantization, palettization=palettization)
         e = self.engine
         self.batch, self.h, self.w, self.seq = batch, height, width, seq_len

@@ -40,8 +40,13 @@ import torch.nn.functional as F
 # --------------------------------------------------------------------------------------
 # helpers
 # --------------------------------------------------------------------------------------
+def _f(t):
+    """fp32, or fp64 when given fp64 (a state dict and inputs in fp64 run the whole restatement in fp64)."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
 def _w(sd, key):
-    return sd[key].float()
+    return _f(sd[key])
 
 
 def _conv(sd, prefix, x, stride=1, padding=0):
@@ -49,7 +54,7 @@ def _conv(sd, prefix, x, stride=1, padding=0):
     if w.dim() == 2:
         w = w[:, :, None, None]
     b = sd.get(prefix + ".bias")
-    return F.conv2d(x, w, None if b is None else b.float(), stride=stride, padding=padding)
+    return F.conv2d(x, w, None if b is None else _f(b), stride=stride, padding=padding)
 
 
 def _gn(sd, prefix, x, groups, eps):
@@ -82,8 +87,9 @@ def attention(q, k, v, heads, dim_head, mask=None):
 
 def timestep_embedding(timesteps, dim, flip_sin_to_cos=True, freq_shift=0.0, max_period=10000):
     half = dim // 2
-    freqs = torch.exp(-math.log(max_period) * torch.arange(half, dtype=torch.float32) / (half - freq_shift))
-    ang = timesteps.float()[:, None] * freqs[None, :]
+    freqs = torch.exp(-math.log(max_period) * torch.arange(half, dtype=torch.float32, device=timesteps.device)
+                      / (half - freq_shift))
+    ang = _f(timesteps)[:, None] * freqs[None, :]
     s, c = torch.sin(ang), torch.cos(ang)
     return torch.cat([c, s], dim=-1) if flip_sin_to_cos else torch.cat([s, c], dim=-1)
 
@@ -151,7 +157,7 @@ def unet_forward(sd, cfg, sample, timestep, encoder_hidden_states, time_ids=None
                          ("CrossAttnDownBlock2D",) * (nb - 1) + ("DownBlock2D",))
     up_types = cfg.get("up_block_types", ("UpBlock2D",) + ("CrossAttnUpBlock2D",) * (nb - 1))
 
-    sample, ctx = sample.float(), encoder_hidden_states.float()
+    sample, ctx = _f(sample), _f(encoder_hidden_states)
     temb = _time_mlp(sd, "time_embedding",
                      timestep_embedding(timestep, boc[0], cfg.get("flip_sin_to_cos", True),
                                         cfg.get("freq_shift", 0)))
@@ -159,7 +165,7 @@ def unet_forward(sd, cfg, sample, timestep, encoder_hidden_states, time_ids=None
         te = timestep_embedding(time_ids.flatten(), cfg["addition_time_embed_dim"],
                                 cfg.get("flip_sin_to_cos", True), cfg.get("freq_shift", 0))
         te = te.reshape(text_embeds.shape[0], -1)
-        temb = temb + _time_mlp(sd, "add_embedding", torch.cat([text_embeds.float(), te], dim=-1))
+        temb = temb + _time_mlp(sd, "add_embedding", torch.cat([_f(text_embeds), te], dim=-1))
 
     x = _conv(sd, "conv_in", sample, padding=1)
     skips = [x]
@@ -173,13 +179,13 @@ def unet_forward(sd, cfg, sample, timestep, encoder_hidden_states, time_ids=None
             x = _conv(sd, f"down_blocks.{i}.downsamplers.0.conv", x, stride=2, padding=1)
             skips.append(x)
     if additional_residuals is not None:
-        skips = [s + r.float() for s, r in zip(skips, additional_residuals[:-1])]
+        skips = [s + _f(r) for s, r in zip(skips, additional_residuals[:-1])]
 
     x = _resnet(sd, "mid_block.resnets.0", x, temb, groups, eps)
     x = _spatial_transformer(sd, "mid_block.attentions.0", x, ctx, heads[-1], depth[-1])
     x = _resnet(sd, "mid_block.resnets.1", x, temb, groups, eps)
     if additional_residuals is not None:
-        x = x + additional_residuals[-1].float()
+        x = x + _f(additional_residuals[-1])
 
     rheads, rdepth = heads[::-1], depth[::-1]
     for i, typ in enumerate(up_types):

@@ -13,24 +13,40 @@ pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def _inputs(cfg, seed, batch=2, hw=16):
+def _size_id(hw):
+    return f"{hw[0]}x{hw[1]}"
+
+
+def _inputs(cfg, seed, batch=2, hw=16, w=None):
     g = torch.Generator().manual_seed(seed)
-    return (torch.randn(batch, 4, hw, hw, generator=g), torch.randn(batch, cfg["cross_attention_dim"], 1, 77, generator=g))
+    return (torch.randn(batch, 4, hw, w or hw, generator=g),
+            torch.randn(batch, cfg["cross_attention_dim"], 1, 77, generator=g))
 
 
 def test_capi_unet_tiny_matches_python_engine_and_oracle(cuda_lib):
+    _capi_unet_tiny_matches_python_engine_and_oracle((16, 16))
+
+
+@pytest.mark.parametrize("hw", [(16, 24)], ids=_size_id)
+def test_capi_unet_tiny_matches_python_engine_and_oracle_non_square(cuda_lib, hw):
+    _capi_unet_tiny_matches_python_engine_and_oracle(hw)
+
+
+def _capi_unet_tiny_matches_python_engine_and_oracle(hw):
+    """Square and at 16x24 latents (the C handle's own NHWC / NCHW conversions see h != w)."""
     from b200sd.capi import CUNet
     from b200sd.model import UNetModel
 
     cfg = config.TINY_UNET
     sd = config.random_state_dict(config.unet_param_shapes(cfg), seed=3)
-    x, c = _inputs(cfg, 4)
+    x, c = _inputs(cfg, 4, hw=hw[0], w=hw[1])
     t = torch.tensor([501.0, 21.0])
-    h = CUNet(cfg, sd, batch=2, height=16, width=16)
+    h = CUNet(cfg, sd, batch=2, height=hw[0], width=hw[1])
     out = h.forward(x.half().cuda(), t.cuda(), c.half().cuda())
     again = h.forward(x.half().cuda(), t.cuda(), c.half().cuda())
     assert torch.equal(out, again)
-    py = UNetModel(cfg, sd, batch=2, height=16, width=16, use_cuda_graph=False)(
+    assert out.shape == (2, 4, *hw)
+    py = UNetModel(cfg, sd, batch=2, height=hw[0], width=hw[1], use_cuda_graph=False)(
         sample=x.half().numpy(), timestep=t.half().numpy(), encoder_hidden_states=c.half().numpy())["noise_pred"]
     # same kernels and launch order; the host-side weight folds (LayerNorm into the consumer GEMM) sum in a different
     # order in C++ and torch, so agreement is to fp32 rounding of those folds, not bitwise

@@ -71,3 +71,38 @@ def test_describe_plan_reports_the_variant_of_the_default_plan():
     assert p["variant"] == -1 and p["halo_kind"] == 2
     p = G.parse_plan(lib.describe_plan(1, n=320, c0=320, n_img=2, h=64, w=64, halo=1, gn=True))
     assert p["variant"] == -1 and p["halo_kind"] == 0
+
+
+@pytest.mark.parametrize("h,w,c", [(12, 21, 1536), (24, 42, 1536), (8, 12, 1280), (12, 8, 1280), (9, 9, 1280)])
+def test_non_square_maps_plan_boxes_that_do_not_tile_them(monkeypatch, h, w, c):
+    """The 3x3 convolutions of the deepest maps of model_cases' non-square and odd sizes (the refiner at 768x1344:
+    12x21 and 24x42; SD at 512x768 / 768x512: 8x12 and 12x8; SD-2.1 at 576^2: 9x9) get TMA boxes that overhang the
+    map, in one dimension only where the map is non-square and in both on the odd square: the per-launch replays of
+    those names check the clipped edges."""
+    from b200sd import lib
+
+    for k in ("B200SD_CLUSTER_SPLITK", "B200SD_STAGED"):
+        monkeypatch.delenv(k, raising=False)
+    p = G.parse_plan(lib.describe_plan(1, n=c, c0=c, n_img=2, h=h, w=w))
+    _, bh, bw = p["box"]
+    ragged = (h % bh != 0, w % bw != 0)
+    assert (ragged[0] != ragged[1]) if h != w else all(ragged), (h, w, p["box"])
+
+
+def test_tiled_weight_cache_lives_as_long_as_its_source():
+    """A packed (tiled) weight is cached only while its source tensor lives: the entry goes with the tensor, and an
+    older tensor that dies after a newer one took its key (same address) leaves the newer entry in place."""
+    import torch
+
+    from b200sd import lib
+
+    a, b, c = torch.randn(8, 8), torch.randn(8, 8), torch.randn(8, 8)
+    lib._cache_tiled(("t", 1), a, torch.zeros(4))
+    lib._cache_tiled(("t", 2), b, torch.zeros(4))
+    del a
+    assert ("t", 1) not in lib._tiled_cache and lib._tiled_cache[("t", 2)][0]() is b
+    lib._cache_tiled(("t", 2), c, torch.zeros(4))
+    del b
+    assert lib._tiled_cache[("t", 2)][0]() is c
+    del c
+    assert not [k for k in lib._tiled_cache if k[0] == "t"]

@@ -417,13 +417,14 @@ class _Replay:
         return "\n".join(lines)
 
 
-MODELS = MC.SHIPPED + ["sd21_b2_fused", "sd21_b2_halo_tma"]
+MODELS = MC.SHIPPED + ["sd21_b2_fused", "sd21_b2_halo_tma", "sd15_512x768_b2_fused", "sd15_512x768_b2_halo_tma"]
 
 
 @pytest.mark.parametrize("name", MODELS)
 def test_model_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
     """Every model of model_cases.SHIPPED from random-init weights (the bf16 VAEs against the bf16 output bound); SD-2.1
-    twice more with the opt-in halo convolutions: B200SD_FUSED=1 (GroupNorm + SiLU in the halo kernel's operand path,
+    and SD-1.5 at 512x768 (halo windows and the cs_hw tile-to-image mapping on a non-square map) twice more with the
+    opt-in halo convolutions: B200SD_FUSED=1 (GroupNorm + SiLU in the halo kernel's operand path,
     kinds 0 / 1) and B200SD_HALO_TMA=1024 (plain convolutions on maps of >= 1024 pixels with TMA patches, kind 2).
     Under B200SD_FUSED=1 every convolution behind a GroupNorm takes the GroupNorm-fused kernel, so B200SD_HALO_TMA has
     nothing left to take there: kind 2 needs the run of its own.  Prints one line per distinct plan and the wall time

@@ -129,18 +129,24 @@ def test_blend_kernel_vs_fp64(cuda_lib, n, hw, noised):
 
 
 # ---------------------------------------------------------------- device loop
-def _pipe(name, cin, images=2, **kw):
+def _pipe(name, cin, images=2, px=(64, 64), **kw):
     from b200sd.pipeline import B200StableDiffusionPipeline
     ucfg = TINY9 if cin == 9 else config.TINY_UNET
-    return B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=images, height=64, width=64, seed=31,
-                                                        scheduler=name, with_vae_encoder=True, unet_cfg=ucfg, **kw)
+    return B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=images, height=px[0], width=px[1],
+                                                        seed=31, scheduler=name, with_vae_encoder=True, unet_cfg=ucfg,
+                                                        **kw)
 
 
-def _images(seed, b=2):
+def _images(seed, b=2, px=(64, 64)):
+    """Images and masks: discs at 64^2; at any other size the left third of the image (a mask that changes when h and
+    w are swapped)."""
     g = torch.Generator().manual_seed(seed)
-    img = (torch.rand(b, 3, 64, 64, generator=g) * 2 - 1).half().numpy()
-    yy, xx = np.meshgrid(np.arange(64), np.arange(64), indexing="ij")
-    mask = np.stack([((yy - 20 - 8 * i) ** 2 + (xx - 30) ** 2 < 300).astype(np.float32)[None] for i in range(b)])
+    img = (torch.rand(b, 3, *px, generator=g) * 2 - 1).half().numpy()
+    yy, xx = np.meshgrid(np.arange(px[0]), np.arange(px[1]), indexing="ij")
+    if px == (64, 64):
+        mask = np.stack([((yy - 20 - 8 * i) ** 2 + (xx - 30) ** 2 < 300).astype(np.float32)[None] for i in range(b)])
+    else:
+        mask = np.stack([(xx < px[1] // 3).astype(np.float32)[None] for _ in range(b)])
     return img, mask
 
 
@@ -157,23 +163,35 @@ def _loop_cases():
                                                                       (f"c{v}" if isinstance(v, int) else
                                                                        ("vpred" if v else "eps"))))
 def test_inpaint_device_loop_vs_oracle(cuda_lib, name, cin, strength, skw):
+    _inpaint_device_loop_vs_oracle(name, cin, strength, skw)
+
+
+@pytest.mark.parametrize("cin", [4, 9])
+def test_inpaint_device_loop_vs_oracle_non_square(cuda_lib, cin):
+    """DDIM at 64x96 pixels (16x24 latents) with the left third masked."""
+    _inpaint_device_loop_vs_oracle("DDIM", cin, 1.0, {}, px=(64, 96))
+
+
+def _inpaint_device_loop_vs_oracle(name, cin, strength, skw, px=(64, 64)):
     """(a) the restated inpaint loop fed the engine's recorded noise predictions reproduces the recorded latents;
     (b) ``__call__`` end to end against the all-oracle pipeline (restated UNet and VAE); (c) 4-channel UNets: the
     latents where the latent mask is 0 are the image latents bit for bit."""
     from b200sd.pipeline import InpaintInputs, latent_mask, prepare_mask_and_masked_image
 
-    pipe = _pipe(name, cin, scheduler_kwargs=skw)
+    pipe = _pipe(name, cin, px=px, scheduler_kwargs=skw)
     steps, g, key = 6, 5.0, 77
-    img, mask = _images(3)
+    img, mask = _images(3, px=px)
+    lh, lw = px[0] // 4, px[1] // 4  # the tiny VAE downsamples by 4
     emb = pipe._encode_prompt(["a red cube", "a blue sphere"], True, None)
     gen = torch.Generator().manual_seed(4)
-    noise = torch.randn(2, 4, 16, 16, generator=gen).half().float()
-    x0_img = torch.randn(2, 4, 16, 16, generator=gen)
-    masked_lat = torch.randn(2, 4, 16, 16, generator=gen)
+    noise = torch.randn(2, 4, lh, lw, generator=gen).half().float()
+    x0_img = torch.randn(2, 4, lh, lw, generator=gen)
+    masked_lat = torch.randn(2, 4, lh, lw, generator=gen)
     sched = S.make_scheduler(name, steps, **pipe.scheduler_kwargs)
     start = sched.inpaint_start_step(strength)
     m_img, _ = prepare_mask_and_masked_image(img, mask)
-    m_lat = latent_mask(m_img, pipe.vae_scale_factor)  # the tiny VAE downsamples by 4
+    m_lat = latent_mask(m_img, pipe.vae_scale_factor)
+    assert m_lat.shape[-2:] == (lh, lw)
     if start:
         a, b = sched.noise_coeffs(start)
         lat0 = (np.float32(a) * x0_img.numpy() + np.float32(b) * noise.numpy()).astype(np.float32)
@@ -203,20 +221,22 @@ def test_inpaint_device_loop_vs_oracle(cuda_lib, name, cin, strength, skw):
         assert torch.equal(final[keep], x0_img[keep])
     # (b) end to end through __call__, against the restated UNet / VAE
     np.random.seed(8)
-    out = pipe(["a red cube", "a blue sphere"], height=64, width=64, num_inference_steps=steps, guidance_scale=g,
+    out = pipe(["a red cube", "a blue sphere"], height=px[0], width=px[1], num_inference_steps=steps, guidance_scale=g,
                starting_image=img, mask_image=mask, strength=strength, output_type="np", seed=key, rng="nvidia").images
+    assert out.shape == (2, *px, 3)
     ucfg = TINY9 if cin == 9 else config.TINY_UNET
     vcfg = config.TINY_VAE
     usd = config.random_state_dict(config.unet_param_shapes(ucfg), seed=31, dtype=torch.float16)
     vsd = config.random_state_dict(config.vae_decoder_param_shapes(vcfg), seed=32, dtype=torch.float16)
     esd = config.random_state_dict(config.vae_encoder_param_shapes(vcfg), seed=81, dtype=torch.float16)
     src0 = NvRandomSource(key)
-    lat_noise = torch.from_numpy(np.stack([src0.normal_array(4 * 16 * 16).reshape(4, 16, 16) for _ in range(2)])).float()
+    lat_noise = torch.from_numpy(np.stack([src0.normal_array(4 * lh * lw).reshape(4, lh, lw)
+                                           for _ in range(2)])).float()
     np.random.seed(8)
     enc_noises = []
 
     def encode_ref(im):
-        z = torch.from_numpy(np.random.randn(2, 4, 16, 16).astype(np.float32))
+        z = torch.from_numpy(np.random.randn(2, 4, lh, lw).astype(np.float32))
         enc_noises.append(z)
         return R.sample_latents(R.vae_encode(esd, vcfg, im.half().float()), z)
 
@@ -236,7 +256,7 @@ def test_inpaint_device_loop_vs_oracle(cuda_lib, name, cin, strength, skw):
                       **({"final_sigmas_type": "zero"} if name == "DPMSolverMultistep" else {}))
         ref_img = R.postprocess_image(R.vae_decode(vsd, vcfg, x.float() / 0.18215)).numpy()
     err = float(np.abs(out - ref_img).max())
-    print(f"inpaint {name} c{cin} strength {strength} {skw}: image max_abs={err:.3e}")
+    print(f"inpaint {name} c{cin} strength {strength} {skw} {px[0]}x{px[1]}: image max_abs={err:.3e}")
     assert err < 5e-2, err
 
 

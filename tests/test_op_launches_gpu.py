@@ -208,7 +208,7 @@ class _Replay:
         return "\n".join(lines)
 
 
-MODELS = MC.SHIPPED + ["sd21_b2_fused2"]
+MODELS = MC.SHIPPED + ["sd21_b2_fused2", "sd15_512x768_b2_fused2"]
 
 
 def _gn_channels(rows):
@@ -218,9 +218,9 @@ def _gn_channels(rows):
 
 @pytest.mark.parametrize("name", MODELS)
 def test_model_op_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
-    """One eager forward of each model of model_cases.SHIPPED (sd21_b2_fused2: SD-2.1 under B200SD_FUSED=2, where
-    group_norm_apply normalises from the producers' channel sums), every wrapped launch checked.  Prints the table and
-    the wall time of the build, forward and checks (run with -s)."""
+    """One eager forward of each model of model_cases.SHIPPED (*_fused2: SD-2.1 and SD-1.5 at 512x768 under
+    B200SD_FUSED=2, where group_norm_apply normalises from the producers' channel sums), every wrapped launch checked.
+    Prints the table and the wall time of the build, forward and checks (run with -s)."""
     lib = cuda_lib
     for k in ("B200SD_CLUSTER_SPLITK", "B200SD_STAGED", "B200SD_FUSED", "B200SD_HALO_TMA"):
         monkeypatch.delenv(k, raising=False)
@@ -248,11 +248,36 @@ def test_model_op_launches_match_fp64_reference(cuda_lib, monkeypatch, name):
     if name.startswith("sdxl_refiner"):  # groups of 12, 36 and 96 channels: none a whole number of 8-channel vectors
         assert {384, 1152, 3072} <= _gn_channels(rep.rows), sorted(_gn_channels(rep.rows))
         assert {key[1][4] for key in rep.rows if key[0] == "attention"} == {64}
-    if name == "controlnet_sd15":
+    if name.startswith(("controlnet_sd15", "sd15")):
         assert {key[1][4] for key in rep.rows if key[0] == "attention"} == {40, 80, 160}
     if name.endswith("_768") and name.startswith("vae_decoder"):
         assert any(key[0] == "softmax_rows" and key[1][1] == 96 * 96 for key in rep.rows)
         assert any(key[0] == "group_norm" and key[1][1:3] == (768, 768) for key in rep.rows)
+    # the non-square and odd maps: the deepest map and the attention token counts each size exists for
+    gn_maps = {tuple(key[1][1:3]) for key in rep.rows if key[0].startswith("group_norm")}
+    tokens = {key[1][2] for key in rep.rows if key[0] == "attention"}
+    want = NON_SQUARE_SHAPES.get(name[: -len("_fused2")] if name.endswith("_fused2") else name)
+    if want is not None:
+        assert want["maps"] <= gn_maps, (sorted(want["maps"]), sorted(gn_maps))
+        assert want.get("tokens", set()) <= tokens, (sorted(want.get("tokens", set())), sorted(tokens))
+        if "softmax" in want:
+            assert any(key[0] == "softmax_rows" and key[1][1] == want["softmax"] for key in rep.rows), sorted(rep.rows)
+
+
+# (h, w) maps some GroupNorm of the model must run on, attention query counts it must reach, softmax_rows columns
+NON_SQUARE_SHAPES = {
+    "sd15_512x768_b2": dict(maps={(64, 96), (8, 12)}, tokens={6144, 1536, 384, 96}),
+    "sd15_768x512_b2": dict(maps={(96, 64), (12, 8)}, tokens={6144, 1536, 384, 96}),
+    "sd21_576x576_b2": dict(maps={(72, 72), (18, 18), (9, 9)}, tokens={5184, 1296, 324, 81}),
+    "sdxl_768x1344_b2": dict(maps={(96, 168), (24, 42)}, tokens={4032, 1008}),
+    "sdxl_1216x832_b2": dict(maps={(152, 104), (38, 26)}, tokens={3952, 988}),
+    "sdxl_refiner_768x1344_b2": dict(maps={(96, 168), (12, 21)}, tokens={4032, 1008, 252}),
+    "controlnet_sd15_512x768": dict(maps={(64, 96), (8, 12)}, tokens={6144, 96}),
+    "vae_decoder_512x768": dict(maps={(64, 96), (512, 768)}, softmax=64 * 96),
+    "vae_decoder_bf16_768x1344": dict(maps={(96, 168), (768, 1344)}, softmax=96 * 168),
+    "vae_encoder_768x512": dict(maps={(768, 512), (96, 64)}, softmax=96 * 64),
+    "vae_encoder_bf16_1216x832": dict(maps={(1216, 832), (152, 104)}, softmax=152 * 104),
+}
 
 
 # ---------------------------------------------------------------------------------------------------------------------

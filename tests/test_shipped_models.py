@@ -1,6 +1,7 @@
 """Host-only tests of the shipped-model list both per-launch replays run (model_cases.SHIPPED) and of the SDXL refiner's
 configuration."""
 import os
+import re
 import sys
 import types
 
@@ -74,7 +75,10 @@ def test_shipped_list_covers_every_path():
     for name in ("sdxl_1024_b2", "sdxl_refiner_1024_b2", "sdxl_refiner_768_b2", "vae_decoder_768", "vae_decoder_bf16_768",
                  "vae_encoder_512", "vae_encoder_768", "vae_encoder_bf16_1024", "controlnet_sd15", "controlnet_sd21_768",
                  "sd21_b2", "sd21_b16", "sd15_b2", "sdxl_768_b2", "controlnet_sd21", "vae_decoder", "openclip_h", "clip_l",
-                 "sd21_768_b2", "vae_decoder_bf16", "vae_encoder_bf16", "openclip_bigg"):
+                 "sd21_768_b2", "vae_decoder_bf16", "vae_encoder_bf16", "openclip_bigg", "sd15_512x768_b2",
+                 "sd15_768x512_b2", "sd21_576x576_b2", "sdxl_768x1344_b2", "sdxl_1216x832_b2",
+                 "sdxl_refiner_768x1344_b2", "controlnet_sd15_512x768", "vae_decoder_512x768", "vae_decoder_bf16_768x1344", "vae_encoder_768x512",
+                 "vae_encoder_bf16_1216x832"):
         assert name in MC.SHIPPED, name
 
 
@@ -83,8 +87,75 @@ def test_both_replays_run_the_shipped_list():
     import test_op_launches_gpu as OP
 
     assert set(MC.SHIPPED) <= set(GP.MODELS) and set(MC.SHIPPED) <= set(OP.MODELS)
-    assert set(GP.MODELS) - set(MC.SHIPPED) == {"sd21_b2_fused", "sd21_b2_halo_tma"}
-    assert set(OP.MODELS) - set(MC.SHIPPED) == {"sd21_b2_fused2"}
+    assert set(GP.MODELS) - set(MC.SHIPPED) == {"sd21_b2_fused", "sd21_b2_halo_tma", "sd15_512x768_b2_fused",
+                                                "sd15_512x768_b2_halo_tma"}
+    assert set(OP.MODELS) - set(MC.SHIPPED) == {"sd21_b2_fused2", "sd15_512x768_b2_fused2"}
+    # every non-square or off-grid shipped name has the shapes it exists for asserted in the op replay
+    assert {n for n in MC.SHIPPED if re.search(r"_\d+x\d+", n)} == set(OP.NON_SQUARE_SHAPES)
+
+
+# latents of every name with an explicit pixel size, and of the square names as they were before sizes were parsed
+LATENT_HW = {
+    "sd15_512x768_b2": (64, 96), "sd15_768x512_b2": (96, 64), "sd21_576x576_b2": (72, 72),
+    "sdxl_768x1344_b2": (96, 168), "sdxl_1216x832_b2": (152, 104), "sdxl_refiner_768x1344_b2": (96, 168),
+    "controlnet_sd15_512x768": (64, 96), "vae_decoder_512x768": (64, 96), "vae_decoder_bf16_768x1344": (96, 168),
+    "vae_encoder_768x512": (96, 64), "vae_encoder_bf16_1216x832": (152, 104),
+    "sd21_b2": (64, 64), "sd21_b16": (64, 64), "sd15_b2": (64, 64), "sd21_768_b2": (96, 96), "sdxl_768_b2": (96, 96),
+    "sdxl_1024_b2": (128, 128), "sdxl_refiner_1024_b2": (128, 128), "sdxl_refiner_768_b2": (96, 96),
+    "controlnet_sd21": (64, 64), "controlnet_sd15": (64, 64), "controlnet_sd21_768": (96, 96), "vae_decoder": (64, 64),
+    "vae_decoder_768": (96, 96), "vae_decoder_bf16": (128, 128), "vae_decoder_bf16_768": (96, 96),
+    "vae_encoder_512": (64, 64), "vae_encoder_768": (96, 96), "vae_encoder_bf16": (64, 64),
+    "vae_encoder_bf16_1024": (128, 128),
+}
+
+
+def test_every_name_maps_to_its_size():
+    """An explicit <height>x<width> is parsed before the "768" / "1024" substrings (sd15_512x768_b2 is 64x96, not 96^2),
+    and the square names keep the geometry they had."""
+    assert set(LATENT_HW) == {n for n in MC.SHIPPED if not n.startswith(("openclip", "clip"))}
+    for name, hw in LATENT_HW.items():
+        assert MC.latent_hw(name) == hw, name
+    for name in ("sd15_512x768_b2_fused", "sd15_512x768_b2_halo_tma", "sd15_512x768_b2_fused2"):
+        assert MC.latent_hw(name) == (64, 96), name
+    assert MC.latent_hw("sd21_b2_fused") == (64, 64)
+
+
+def _model_cfg(name):
+    if name.startswith("controlnet"):
+        return C.SD15_CONTROLNET if name.startswith("controlnet_sd15") else C.SD21_CONTROLNET
+    if name.startswith("sdxl_refiner"):
+        return C.SDXL_REFINER_UNET
+    return C.SD21_UNET if name.startswith("sd21_768") else {"sd21": C.SD21_BASE_UNET, "sd15": C.SD15_UNET,
+                                                             "sdxl": C.SDXL_BASE_UNET}[name[:4]]
+
+
+@pytest.mark.parametrize("name", [n for n in MC.SHIPPED if n.startswith(("sd", "controlnet"))])
+def test_shipped_unet_sizes_halve_exactly(name):
+    """Every down-sampler of a shipped UNet / ControlNet halves its map exactly: the latents divide by
+    2^(levels - 1), so the constructor's size check accepts them."""
+    cfg = _model_cfg(name)
+    h, w = MC.latent_hw(name)
+    levels = len(cfg["block_out_channels"])
+    assert h % 2 ** (levels - 1) == 0 and w % 2 ** (levels - 1) == 0, (name, h, w)
+    C.check_latent_size(cfg, h, w)
+
+
+def test_latent_multiple():
+    """64 pixels for SD 1.x / 2.x, their ControlNets and the refiner (four levels), 32 for SDXL-base (three); the check
+    names the pixel multiple and rejects either dimension alone."""
+    for cfg in (C.SD21_BASE_UNET, C.SD21_UNET, C.SD15_UNET, C.SDXL_REFINER_UNET, C.SD21_CONTROLNET, C.SD15_CONTROLNET):
+        assert C.latent_multiple(cfg) == 8
+    assert C.latent_multiple(C.SDXL_BASE_UNET) == 4
+    assert C.latent_multiple(C.TINY_UNET) == 4 and C.latent_multiple(C.TINY_XL_UNET) == 2
+    C.check_latent_size(C.SD15_UNET, 64, 96)
+    C.check_latent_size(C.SDXL_BASE_UNET, 100, 132)  # 800x1056: SDXL-base takes multiples of 32 pixels
+    for h, w in ((68, 68), (64, 68), (68, 64), (72, 76)):  # 544^2 halves 68 -> 34 -> 17 and cannot go on
+        with pytest.raises(ValueError, match="multiples of 64 pixels"):
+            C.check_latent_size(C.SD15_UNET, h, w)
+    with pytest.raises(ValueError, match="multiples of 64 pixels"):
+        C.check_latent_size(C.SDXL_REFINER_UNET, 96, 164)
+    with pytest.raises(ValueError, match="multiples of 32 pixels"):
+        C.check_latent_size(C.SDXL_BASE_UNET, 96, 166)
 
 
 @pytest.mark.parametrize("nid,h,want", [(6, 128, [1024.0, 1024.0, 0.0, 0.0, 1024.0, 1024.0]),

@@ -14,12 +14,19 @@ from oracle import restated as R
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 MAX_ABS, MIN_PSNR = 1e-2, 35.0
+# latent (h, w) at which the tiny live-oracle tests run again beside their square size: portrait and landscape (at a
+# square size a kernel or the host may confuse h with w unseen); the pipeline tests run at 64x96 pixels
+NON_SQUARE_HW = [(16, 24), (24, 16)]
 
 
-def _inputs(cfg, seed, batch=2, seq=77):
+def _size_id(hw):
+    return f"{hw[0]}x{hw[1]}"
+
+
+def _inputs(cfg, seed, batch=2, seq=77, hw=None):
     g = torch.Generator().manual_seed(seed)
-    s = cfg["sample_size"]
-    x = torch.randn(batch, cfg["in_channels"], s, s, generator=g)
+    h, w = hw or (cfg["sample_size"], cfg["sample_size"])
+    x = torch.randn(batch, cfg["in_channels"], h, w, generator=g)
     c = torch.randn(batch, cfg["cross_attention_dim"], 1, seq, generator=g)
     return x, c
 
@@ -34,6 +41,17 @@ def _check(out, ref, what, max_abs=MAX_ABS):
 
 @pytest.mark.parametrize("impl", ["ORIGINAL", "SPLIT_EINSUM", "SPLIT_EINSUM_V2"])
 def test_unet_tiny_vs_oracle_and_golden(cuda_lib, impl):
+    _unet_tiny_vs_oracle_and_golden(impl, (16, 16))
+
+
+@pytest.mark.parametrize("hw", NON_SQUARE_HW, ids=_size_id)
+@pytest.mark.parametrize("impl", ["ORIGINAL", "SPLIT_EINSUM", "SPLIT_EINSUM_V2"])
+def test_unet_tiny_vs_oracle_and_golden_non_square(cuda_lib, impl, hw):
+    _unet_tiny_vs_oracle_and_golden(impl, hw)
+
+
+def _unet_tiny_vs_oracle_and_golden(impl, hw):
+    """The golden is square (16^2); every size is checked against the live oracle."""
     from b200sd import unet as U
     from b200sd.model import UNetModel
 
@@ -41,15 +59,16 @@ def test_unet_tiny_vs_oracle_and_golden(cuda_lib, impl):
     cfg = config.TINY_UNET
     gold = np.load(os.path.join(GOLD, "unet_tiny.npz"))
     sd = config.random_state_dict(config.unet_param_shapes(cfg), seed=int(gold["weight_seed"]))
-    x, c = _inputs(cfg, int(gold["input_seed"]))
+    x, c = _inputs(cfg, int(gold["input_seed"]), hw=hw)
     t = np.array([float(gold["timestep"])] * 2, np.float16)
-    m = UNetModel(cfg, sd, batch=2, height=16, width=16, use_cuda_graph=False)
+    m = UNetModel(cfg, sd, batch=2, height=hw[0], width=hw[1], use_cuda_graph=False)
     out = m(sample=x.half().numpy(), timestep=t, encoder_hidden_states=c.half().numpy())["noise_pred"]
-    assert out.dtype == np.float32 and out.shape == (2, 4, 16, 16)
-    _check(out, gold[f"noise_pred_{impl}"], f"tiny unet vs reference golden [{impl}]")
+    assert out.dtype == np.float32 and out.shape == (2, 4, *hw)
+    if hw == (16, 16):
+        _check(out, gold[f"noise_pred_{impl}"], f"tiny unet vs reference golden [{impl}]")
     with torch.no_grad():
         live = R.unet_forward(sd, cfg, x, torch.tensor([981.0, 981.0]), c).numpy()
-    _check(out, live, f"tiny unet vs live oracle [{impl}]")
+    _check(out, live, f"tiny unet {hw[0]}x{hw[1]} vs live oracle [{impl}]")
 
 
 def test_unet_tiny_cuda_graph_equals_eager_and_validates(cuda_lib):
@@ -97,12 +116,21 @@ def test_unet_sd21_base_vs_reference_golden(cuda_lib):
 
 
 def test_unet_tiny_controlnet_residuals(cuda_lib):
+    _unet_tiny_controlnet_residuals((16, 16))
+
+
+@pytest.mark.parametrize("hw", NON_SQUARE_HW, ids=_size_id)
+def test_unet_tiny_controlnet_residuals_non_square(cuda_lib, hw):
+    _unet_tiny_controlnet_residuals(hw)
+
+
+def _unet_tiny_controlnet_residuals(hw):
     from b200sd.model import UNetModel
 
     cfg = dict(config.TINY_UNET, support_controlnet=True)
     sd = config.random_state_dict(config.unet_param_shapes(cfg), seed=5)
-    x, c = _inputs(cfg, 6)
-    m = UNetModel(cfg, sd, batch=2, height=16, width=16, use_cuda_graph=False)
+    x, c = _inputs(cfg, 6, hw=hw)
+    m = UNetModel(cfg, sd, batch=2, height=hw[0], width=hw[1], use_cuda_graph=False)
     g = torch.Generator().manual_seed(7)
     res = [torch.randn(s, generator=g) * 0.5 for s in m.residual_shapes()]
     assert len(res) == 7  # conv_in + (res[, down]) per level + mid (controlnet.py:218-229 order)
@@ -111,36 +139,56 @@ def test_unet_tiny_controlnet_residuals(cuda_lib):
             encoder_hidden_states=c.half().numpy(), **kw)["noise_pred"]
     with torch.no_grad():
         ref = R.unet_forward(sd, cfg, x, torch.tensor([301.0, 301.0]), c, additional_residuals=res).numpy()
-    _check(out, ref, "tiny control-unet")
+    _check(out, ref, f"tiny control-unet {hw[0]}x{hw[1]}")
 
 
 def test_vae_decoder_tiny_vs_oracle(cuda_lib):
+    _vae_decoder_tiny_vs_oracle((16, 16))
+
+
+@pytest.mark.parametrize("hw", NON_SQUARE_HW, ids=_size_id)
+def test_vae_decoder_tiny_vs_oracle_non_square(cuda_lib, hw):
+    _vae_decoder_tiny_vs_oracle(hw)
+
+
+def _vae_decoder_tiny_vs_oracle(hw):
     from b200sd.vae import VAEDecoderModel
 
     cfg = config.TINY_VAE
     sd = config.random_state_dict(config.vae_decoder_param_shapes(cfg), seed=3)
-    z = torch.randn(1, 4, 16, 16, generator=torch.Generator().manual_seed(1))
-    m = VAEDecoderModel(cfg, sd, batch=1, height=16, width=16)
+    z = torch.randn(1, 4, *hw, generator=torch.Generator().manual_seed(1))
+    m = VAEDecoderModel(cfg, sd, batch=1, height=hw[0], width=hw[1])
     img = m(z=z.half().numpy())["image"]
-    assert img.shape == (1, 3, 64, 64)
+    assert img.shape == (1, 3, 4 * hw[0], 4 * hw[1])
     with torch.no_grad():
         ref = R.vae_decode(sd, cfg, z).numpy()
-    _check(img, ref, "tiny vae decoder", max_abs=2e-2 * max(1.0, float(np.abs(ref).max())))
+    _check(img, ref, f"tiny vae decoder {hw[0]}x{hw[1]}", max_abs=2e-2 * max(1.0, float(np.abs(ref).max())))
 
 
 def test_pipeline_tiny_end_to_end_vs_oracle(cuda_lib):
-    """20-step DDIM txt2img on the tiny models vs the same loop run with the oracle on the CPU."""
+    _pipeline_tiny_end_to_end_vs_oracle((64, 64))
+
+
+@pytest.mark.parametrize("px", [(64, 96)], ids=_size_id)
+def test_pipeline_tiny_end_to_end_vs_oracle_non_square(cuda_lib, px):
+    _pipeline_tiny_end_to_end_vs_oracle(px)
+
+
+def _pipeline_tiny_end_to_end_vs_oracle(px):
+    """6-step DDIM txt2img on the tiny models vs the same loop run with the oracle on the CPU, square and at 64x96
+    (height x width) pixels."""
     from b200sd.pipeline import B200StableDiffusionPipeline
     from b200sd import scheduler as S
 
-    pipe = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=64, width=64, seed=11)
+    H, W = px
+    pipe = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=H, width=W, seed=11)
     np.random.seed(93)
-    lat0 = np.random.randn(1, 4, 16, 16).astype(np.float16)
+    lat0 = np.random.randn(1, 4, H // 4, W // 4).astype(np.float16)
     steps, g = 6, 7.5
-    res = pipe("a photo of an astronaut riding a horse", height=64, width=64, num_inference_steps=steps,
+    res = pipe("a photo of an astronaut riding a horse", height=H, width=W, num_inference_steps=steps,
                guidance_scale=g, latents=lat0, output_type="np")
     img = res.images
-    assert img.shape == (1, 64, 64, 3) and img.min() >= 0 and img.max() <= 1
+    assert img.shape == (1, H, W, 3) and img.min() >= 0 and img.max() <= 1
     # oracle loop
     ucfg, vcfg = config.TINY_UNET, config.TINY_VAE
     usd = config.random_state_dict(config.unet_param_shapes(ucfg), seed=11, dtype=torch.float16)
@@ -159,16 +207,16 @@ def test_pipeline_tiny_end_to_end_vs_oracle(cuda_lib):
     # the call above replayed the whole loop as one CUDA graph; the step-by-step path must agree bit for bit
     assert pipe.loop_graph and len(pipe._loop_graphs) == 1
     pipe.loop_graph = False
-    img2 = pipe("a photo of an astronaut riding a horse", height=64, width=64, num_inference_steps=steps,
+    img2 = pipe("a photo of an astronaut riding a horse", height=H, width=W, num_inference_steps=steps,
                 guidance_scale=g, latents=lat0, output_type="np").images
     pipe.loop_graph = True
     assert np.array_equal(img, img2), float(np.abs(img - img2).max())
-    img3 = pipe("a photo of an astronaut riding a horse", height=64, width=64, num_inference_steps=steps,
+    img3 = pipe("a photo of an astronaut riding a horse", height=H, width=W, num_inference_steps=steps,
                 guidance_scale=g, latents=lat0, output_type="np").images  # second replay of the cached graph
     assert np.array_equal(img, img3)
-    # PIL output + generate() alias + return_dict=False
-    out = pipe.generate("x", num_inference_steps=2, guidance_scale=7.5, height=64, width=64, return_dict=False)
-    assert out[1] is None and out[0][0].size == (64, 64)
+    # PIL output (size is (width, height)) + generate() alias + return_dict=False
+    out = pipe.generate("x", num_inference_steps=2, guidance_scale=7.5, height=H, width=W, return_dict=False)
+    assert out[1] is None and out[0][0].size == (W, H)
 
 
 def test_unet_tiny_batched_prompts_vs_oracle(cuda_lib):
@@ -231,27 +279,46 @@ def test_pipeline_tiny_batched_and_schedulers(cuda_lib):
 
 
 def test_unet_tiny_xl_text_time_conditioning(cuda_lib):
+    _unet_tiny_xl_text_time_conditioning((16, 16))
+
+
+@pytest.mark.parametrize("hw", NON_SQUARE_HW, ids=_size_id)
+def test_unet_tiny_xl_text_time_conditioning_non_square(cuda_lib, hw):
+    _unet_tiny_xl_text_time_conditioning(hw)
+
+
+def _unet_tiny_xl_text_time_conditioning(hw):
     """SDXL-style forward (UNet2DConditionModelXL.forward, unet.py:1051-1152): text_time added conditioning,
     DownBlock2D first level, transformer depth > 1."""
     from b200sd.model import UNetModel
 
     cfg = config.TINY_XL_UNET
     sd = config.random_state_dict(config.unet_param_shapes(cfg), seed=3)
-    x, c = _inputs(cfg, 9)
+    x, c = _inputs(cfg, 9, hw=hw)
     g = torch.Generator().manual_seed(10)
-    tid = torch.tensor([[64.0, 64.0, 0.0, 0.0, 64.0, 64.0]] * 2)
+    H, W = 8.0 * hw[0], 8.0 * hw[1]
+    tid = torch.tensor([[H, W, 0.0, 0.0, H, W]] * 2)
     te = torch.randn(2, 64, generator=g)
     t = np.array([981.0, 981.0], np.float16)
-    m = UNetModel(cfg, sd, batch=2, height=16, width=16, use_cuda_graph=False)
+    m = UNetModel(cfg, sd, batch=2, height=hw[0], width=hw[1], use_cuda_graph=False)
     out = m(sample=x.half().numpy(), timestep=t, encoder_hidden_states=c.half().numpy(),
             time_ids=tid.half().numpy(), text_embeds=te.half().numpy())["noise_pred"]
     with torch.no_grad():
         ref = R.unet_forward(sd, cfg, x, torch.tensor([981.0, 981.0]), c, time_ids=tid,
                              text_embeds=te.half().float()).numpy()
-    _check(out, ref, "tiny SDXL-style unet")
+    _check(out, ref, f"tiny SDXL-style unet {hw[0]}x{hw[1]}")
 
 
 def test_controlnet_tiny_vs_oracle_and_chain_into_unet(cuda_lib):
+    _controlnet_tiny_vs_oracle_and_chain_into_unet((16, 16))
+
+
+@pytest.mark.parametrize("hw", NON_SQUARE_HW, ids=_size_id)
+def test_controlnet_tiny_vs_oracle_and_chain_into_unet_non_square(cuda_lib, hw):
+    _controlnet_tiny_vs_oracle_and_chain_into_unet(hw)
+
+
+def _controlnet_tiny_vs_oracle_and_chain_into_unet(hw):
     """ControlNetModel.forward (controlnet.py:199-250) residuals, then fed to the control-UNet exactly like the
     reference loop does (pipeline.py:516-536)."""
     from b200sd.controlnet import ControlNetModel
@@ -261,10 +328,10 @@ def test_controlnet_tiny_vs_oracle_and_chain_into_unet(cuda_lib):
     csd = config.random_state_dict(config.controlnet_param_shapes(ccfg), seed=4)
     ucfg = dict(config.TINY_UNET, support_controlnet=True)
     usd = config.random_state_dict(config.unet_param_shapes(ucfg), seed=5)
-    x, c = _inputs(config.TINY_UNET, 6)
-    cond = torch.rand(2, 3, 128, 128, generator=torch.Generator().manual_seed(7))
+    x, c = _inputs(config.TINY_UNET, 6, hw=hw)
+    cond = torch.rand(2, 3, 8 * hw[0], 8 * hw[1], generator=torch.Generator().manual_seed(7))
     t = np.array([501.0, 501.0], np.float16)
-    cn = ControlNetModel(ccfg, csd, batch=2, height=16, width=16)
+    cn = ControlNetModel(ccfg, csd, batch=2, height=hw[0], width=hw[1])
     res = cn(sample=x.half().numpy(), timestep=t, encoder_hidden_states=c.half().numpy(),
              controlnet_cond=cond.half().numpy())
     with torch.no_grad():
@@ -273,7 +340,7 @@ def test_controlnet_tiny_vs_oracle_and_chain_into_unet(cuda_lib):
     for i, r in enumerate(ref):
         _check(res[f"additional_residual_{i}"], r.numpy(), f"controlnet residual {i}",
                max_abs=1e-2 * max(1.0, float(r.abs().max())))
-    unet = UNetModel(ucfg, usd, batch=2, height=16, width=16, use_cuda_graph=False)
+    unet = UNetModel(ucfg, usd, batch=2, height=hw[0], width=hw[1], use_cuda_graph=False)
     kw = {k: v.astype(np.float16) for k, v in res.items()}
     out = unet(sample=x.half().numpy(), timestep=t, encoder_hidden_states=c.half().numpy(), **kw)["noise_pred"]
     with torch.no_grad():
@@ -282,21 +349,31 @@ def test_controlnet_tiny_vs_oracle_and_chain_into_unet(cuda_lib):
 
 
 def test_pipeline_tiny_with_controlnet_vs_oracle(cuda_lib):
+    _pipeline_tiny_with_controlnet_vs_oracle((64, 64))
+
+
+@pytest.mark.parametrize("px", [(64, 96)], ids=_size_id)
+def test_pipeline_tiny_with_controlnet_vs_oracle_non_square(cuda_lib, px):
+    _pipeline_tiny_with_controlnet_vs_oracle(px)
+
+
+def _pipeline_tiny_with_controlnet_vs_oracle(px):
     """BASELINE configs[4] shape class: ControlNet residuals computed every step inside the pipeline loop
     (pipeline.py:488-494, 515-536), checked against the same loop run with the oracle."""
     from b200sd.pipeline import B200StableDiffusionPipeline
     from b200sd import scheduler as S
 
-    pipe = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=64, width=64, seed=21,
+    H, W = px
+    pipe = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=H, width=W, seed=21,
                                                         controlnet_cfgs=[config.TINY_CONTROLNET])
     np.random.seed(5)
-    lat0 = np.random.randn(1, 4, 16, 16).astype(np.float16)
-    cond = np.random.rand(3, 128, 128).astype(np.float16)
+    lat0 = np.random.randn(1, 4, H // 4, W // 4).astype(np.float16)
+    cond = np.random.rand(3, 2 * H, 2 * W).astype(np.float16)
     steps, g = 3, 5.0
     rec = []
     emb_np = pipe._encode_prompt(["a cat"], True, None)
     cc = pipe.prepare_control_cond([cond], True, 1, 1)
-    assert cc[0].shape == (2, 3, 128, 128)
+    assert cc[0].shape == (2, 3, 2 * H, 2 * W)
     final = pipe.denoise(emb_np, lat0.astype(np.float32), steps, g, record=rec, controlnet_cond=cc).cpu().numpy()
     # oracle loop
     ucfg = dict(config.TINY_UNET, support_controlnet=True)
@@ -315,16 +392,16 @@ def test_pipeline_tiny_with_controlnet_vs_oracle(cuda_lib):
             x = R.ddim_step(R.cfg_combine(eps[:1], eps[1:], g), t, x, abar, steps)
     _check(final, x.numpy(), "pipeline + controlnet latents", max_abs=2e-2 * max(1.0, float(x.abs().max())))
     # the public call accepts the reference's argument and rejects it without modules
-    out = pipe("a cat", height=64, width=64, num_inference_steps=2, controlnet_cond=[cond], output_type="np")
-    assert out.images.shape == (1, 64, 64, 3)
+    out = pipe("a cat", height=H, width=W, num_inference_steps=2, controlnet_cond=[cond], output_type="np")
+    assert out.images.shape == (1, H, W, 3)
     # without conditions the static residual buffers are cleared: two such calls agree bit for bit even though a
     # ControlNet call ran in between (its last-step residuals must not leak into the next image)
     first = pipe.denoise(emb_np, lat0.astype(np.float32), steps, g).clone()
     pipe.denoise(emb_np, lat0.astype(np.float32), steps, g, controlnet_cond=cc)
     assert torch.equal(first, pipe.denoise(emb_np, lat0.astype(np.float32), steps, g))
-    plain = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=64, width=64, seed=21)
+    plain = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=H, width=W, seed=21)
     with pytest.raises(ValueError, match="no controlnet modules"):
-        plain("a cat", height=64, width=64, num_inference_steps=1, controlnet_cond=[cond])
+        plain("a cat", height=H, width=W, num_inference_steps=1, controlnet_cond=[cond])
 
 
 def test_unet_sdxl_base_768_vs_reference_golden(cuda_lib):
@@ -418,42 +495,61 @@ def test_text_encoder_sdxl_outputs_vs_oracle(cuda_lib):
 
 
 def test_vae_encoder_tiny_vs_oracle(cuda_lib):
+    _vae_encoder_tiny_vs_oracle((16, 16))
+
+
+@pytest.mark.parametrize("hw", NON_SQUARE_HW, ids=_size_id)
+def test_vae_encoder_tiny_vs_oracle_non_square(cuda_lib, hw):
+    _vae_encoder_tiny_vs_oracle(hw)
+
+
+def _vae_encoder_tiny_vs_oracle(hw):
     """vae_encoder(x) -> moments = quant_conv(encoder(x)) (torch2coreml.py:739-756) and the Swift sampling rule."""
     from b200sd.vae import VAEEncoderModel
 
     cfg = config.TINY_VAE
     sd = config.random_state_dict(config.vae_encoder_param_shapes(cfg), seed=13)
-    x = torch.rand(1, 3, 64, 64, generator=torch.Generator().manual_seed(14)) * 2 - 1
-    m = VAEEncoderModel(cfg, sd, batch=1, height=64, width=64)
+    x = torch.rand(1, 3, 4 * hw[0], 4 * hw[1], generator=torch.Generator().manual_seed(14)) * 2 - 1
+    m = VAEEncoderModel(cfg, sd, batch=1, height=4 * hw[0], width=4 * hw[1])
     mom = m(x=x.half().numpy())["latent"]
-    assert mom.shape == (1, 8, 16, 16)
+    assert mom.shape == (1, 8, *hw)
     with torch.no_grad():
         ref = R.vae_encode(sd, cfg, x.half().float())
     _check(mom, ref.numpy(), "tiny vae encoder moments", max_abs=2e-2 * max(1.0, float(ref.abs().max())))
-    noise = torch.randn(1, 4, 16, 16, generator=torch.Generator().manual_seed(15))
+    noise = torch.randn(1, 4, *hw, generator=torch.Generator().manual_seed(15))
     lat = m.encode(x.half().numpy(), noise)
     _check(lat.numpy(), R.sample_latents(ref, noise).numpy(), "tiny vae encoder sample",
            max_abs=2e-2 * max(1.0, float(R.sample_latents(ref, noise).abs().max())))
 
 
 def test_pipeline_tiny_image_to_image_vs_oracle(cuda_lib):
+    _pipeline_tiny_image_to_image_vs_oracle((64, 64))
+
+
+@pytest.mark.parametrize("px", [(64, 96)], ids=_size_id)
+def test_pipeline_tiny_image_to_image_vs_oracle_non_square(cuda_lib, px):
+    _pipeline_tiny_image_to_image_vs_oracle(px)
+
+
+def _pipeline_tiny_image_to_image_vs_oracle(px):
     """Swift image-to-image mode (StableDiffusionPipeline.swift:250-262, 361-378; Scheduler.swift:83-114): encode,
     noise to timeSteps[startStep], run the remaining steps, decode -- against the same procedure on the oracle."""
     from b200sd.pipeline import B200StableDiffusionPipeline
     from b200sd import scheduler as S
 
-    pipe = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=64, width=64, seed=31,
+    H, W = px
+    pipe = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=H, width=W, seed=31,
                                                         with_vae_encoder=True)
-    img0 = (torch.rand(1, 3, 64, 64, generator=torch.Generator().manual_seed(32)) * 2 - 1).half().numpy()
+    img0 = (torch.rand(1, 3, H, W, generator=torch.Generator().manual_seed(32)) * 2 - 1).half().numpy()
     steps, g, strength = 8, 6.0, 0.5
     np.random.seed(33)
-    out = pipe("a cat", height=64, width=64, num_inference_steps=steps, guidance_scale=g, starting_image=img0,
+    out = pipe("a cat", height=H, width=W, num_inference_steps=steps, guidance_scale=g, starting_image=img0,
                strength=strength, output_type="np").images
-    assert out.shape == (1, 64, 64, 3)
+    assert out.shape == (1, H, W, 3)
     # oracle: same RNG stream (noise samples first, then the encoder noise), same schedule truncation
     np.random.seed(33)
-    noise = np.random.randn(1, 4, 16, 16).astype(np.float16).astype(np.float32)
-    enc_noise = np.random.randn(1, 4, 16, 16).astype(np.float32)
+    noise = np.random.randn(1, 4, H // 4, W // 4).astype(np.float16).astype(np.float32)
+    enc_noise = np.random.randn(1, 4, H // 4, W // 4).astype(np.float32)
     ucfg, vcfg = config.TINY_UNET, config.TINY_VAE
     usd = config.random_state_dict(config.unet_param_shapes(ucfg), seed=31, dtype=torch.float16)
     vsd = config.random_state_dict(config.vae_decoder_param_shapes(vcfg), seed=32, dtype=torch.float16)
@@ -473,9 +569,9 @@ def test_pipeline_tiny_image_to_image_vs_oracle(cuda_lib):
     err = float(np.abs(out - ref).max())
     print(f"img2img tiny: image max_abs={err:.3e}")
     assert err < 3e-2
-    plain = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=64, width=64, seed=31)
+    plain = B200StableDiffusionPipeline.from_random_init("tiny", images_per_call=1, height=H, width=W, seed=31)
     with pytest.raises(ValueError, match="no vae_encoder"):
-        plain("a cat", height=64, width=64, num_inference_steps=2, starting_image=img0)
+        plain("a cat", height=H, width=W, num_inference_steps=2, starting_image=img0)
 
 
 def test_controlnet_sd21_vs_reference_golden(cuda_lib):
@@ -505,3 +601,133 @@ def test_controlnet_sd21_vs_reference_golden(cuda_lib):
                                     torch.tensor([501.0, 501.0]), c.half().float(), cond.half().float())
     for i, r in enumerate(live):
         _check(out[f"additional_residual_{i}"], r.numpy(), f"SD-2.1 controlnet residual {i} (full grid)")
+
+
+def test_unet_sd15_512x768_vs_fp64_oracle(cuda_lib):
+    """SD-1.5 at its usual portrait size, 512x768 (64x96 latents down to 8x12; head dims 40 / 80 / 160), one forward
+    through the captured graph against the oracle run in fp64 on the device from the same fp16 weights and inputs."""
+    from b200sd.model import UNetModel
+
+    cfg = config.SD15_UNET
+    sd = config.random_state_dict(config.unet_param_shapes(cfg), seed=61, dtype=torch.float16)
+    g = torch.Generator().manual_seed(62)
+    x = torch.randn(2, 4, 64, 96, generator=g).half()
+    c = torch.randn(2, 768, 1, 77, generator=g).half()
+    t = torch.tensor([801.0, 301.0])
+    m = UNetModel(cfg, sd, batch=2, height=64, width=96, use_cuda_graph=True)
+    out = m(sample=x.numpy(), timestep=t.half().numpy(), encoder_hidden_states=c.numpy())["noise_pred"]
+    assert out.shape == (2, 4, 64, 96)
+    del m
+    torch.cuda.empty_cache()
+    sd64 = {k: v.cuda().double() for k, v in sd.items()}
+    del sd
+    with torch.no_grad():
+        ref = R.unet_forward(sd64, cfg, x.cuda().double(), t.cuda().double(), c.cuda().double()).cpu().numpy()
+    del sd64
+    torch.cuda.empty_cache()
+    _check(out, ref, "SD-1.5 unet 512x768 vs fp64 oracle")
+
+
+def test_pipeline_tiny_sdxl_non_square_time_ids_vs_oracle(cuda_lib):
+    """An SDXL pipeline with a refiner at 64x96 (height x width) pixels through __call__: the base UNet's time ids
+    are (original size, crop, target size) = [H, W, 0, 0, H, W], the refiner's (original size, crop, aesthetic score)
+    = [H, W, 0, 0, score] with the negative score on the unconditional row, height first; the final latents match the
+    oracle loop run with those ids."""
+    from b200sd.model import UNetModel
+    from b200sd.pipeline import B200StableDiffusionPipeline
+    from b200sd.vae import VAEDecoderModel
+
+    H, W = 64, 96
+    h, w = H // 4, W // 4  # the tiny VAE scales by 4
+    bcfg = config.TINY_XL_UNET
+    rcfg = dict(bcfg, projection_class_embeddings_input_dim=64 + 5 * 32, num_time_ids=5)
+    bsd = config.random_state_dict(config.unet_param_shapes(bcfg), seed=71, dtype=torch.float16)
+    rsd = config.random_state_dict(config.unet_param_shapes(rcfg), seed=72, dtype=torch.float16)
+    vsd = config.random_state_dict(config.vae_decoder_param_shapes(config.TINY_VAE), seed=73, dtype=torch.float16)
+    pipe = B200StableDiffusionPipeline(UNetModel(bcfg, bsd, batch=2, height=h, width=w),
+                                       VAEDecoderModel(config.TINY_VAE, vsd, batch=1, height=h, width=w),
+                                       scheduler="DDIM", xl=True,
+                                       unet_refiner=UNetModel(rcfg, rsd, batch=2, height=h, width=w))
+    g = torch.Generator().manual_seed(74)
+    emb = torch.randn(2, 96, 1, 77, generator=g).half()
+    pooled = torch.randn(2, 64, generator=g)
+    remb = torch.randn(2, 96, 1, 77, generator=g).half()
+    rpooled = torch.randn(2, 64, generator=g)
+    lat0 = torch.randn(1, 4, h, w, generator=g).half()
+    steps, gs, rstart = 5, 4.0, 0.6
+    img = pipe("x", height=H, width=W, num_inference_steps=steps, guidance_scale=gs, latents=lat0.numpy(),
+               prompt_embeds=emb.numpy(), pooled_prompt_embeds=pooled, refiner_prompt_embeds=remb.numpy(),
+               refiner_pooled_prompt_embeds=rpooled.numpy(), refiner_start=rstart, output_type="np").images
+    assert img.shape == (1, H, W, 3)
+    final = pipe._latents.cpu().clone()
+    tid = torch.tensor([[H, W, 0.0, 0.0, H, W]] * 2)
+    rtid = torch.tensor([[H, W, 0.0, 0.0, 2.5], [H, W, 0.0, 0.0, 6.0]])
+    assert torch.equal(pipe.unet._time_ids.cpu(), tid), pipe.unet._time_ids
+    assert torch.equal(pipe.unet_refiner._time_ids.cpu(), rtid), pipe.unet_refiner._time_ids
+    abar = R.alphas_cumprod()
+    x = lat0.float()
+    switch = int(np.float32(steps) * np.float32(rstart))
+    with torch.no_grad():
+        for i, t in enumerate(R.leading_timesteps(steps)):
+            tt = torch.tensor([float(t)] * 2)
+            xin = torch.cat([x, x]).half().float()
+            if i < switch:
+                eps = R.unet_forward(bsd, bcfg, xin, tt, emb, time_ids=tid, text_embeds=pooled)
+            else:
+                eps = R.unet_forward(rsd, rcfg, xin, tt, remb, time_ids=rtid, text_embeds=rpooled)
+            x = R.ddim_step(R.cfg_combine(eps[:1], eps[1:], gs), t, x, abar, steps)
+    err = float((final - x).abs().max())
+    rel = err / float(x.abs().max())
+    print(f"SDXL tiny pipeline {H}x{W}: latent max_abs={err:.3e} rel={rel:.3e} after {steps} steps")
+    assert rel < 3e-2
+
+
+def test_off_grid_sizes_are_rejected_at_construction(cuda_lib):
+    """Latents the down-samplers cannot halve exactly (SD at 544^2 halves 68 -> 34 -> 17 and cannot go on) are refused
+    when the model is built, naming the pixel multiple, before any kernel runs: the Python UNet and ControlNet and the
+    C handle."""
+    from b200sd.capi import CUNet
+    from b200sd.controlnet import ControlNetModel
+    from b200sd.model import UNetModel
+
+    usd = config.random_state_dict(config.unet_param_shapes(config.TINY_UNET), seed=3, dtype=torch.float16)
+    xsd = config.random_state_dict(config.unet_param_shapes(config.TINY_XL_UNET), seed=3, dtype=torch.float16)
+    csd = config.random_state_dict(config.controlnet_param_shapes(config.TINY_CONTROLNET), seed=4, dtype=torch.float16)
+    n0 = cuda_lib.launch_count()
+    for h, w in ((16, 18), (18, 16), (14, 14)):  # the tiny UNet has three levels: multiples of 4 latents, 32 pixels
+        with pytest.raises(ValueError, match="multiples of 32 pixels"):
+            UNetModel(config.TINY_UNET, usd, batch=2, height=h, width=w)
+        with pytest.raises(ValueError, match="multiples of 32 pixels"):
+            ControlNetModel(config.TINY_CONTROLNET, csd, batch=2, height=h, width=w)
+        with pytest.raises(cuda_lib.B200SDError, match="multiples of 32 pixels"):
+            CUNet(config.TINY_UNET, usd, batch=2, height=h, width=w)
+    with pytest.raises(ValueError, match="multiples of 16 pixels"):  # two levels
+        UNetModel(config.TINY_XL_UNET, xsd, batch=2, height=16, width=17)
+    assert cuda_lib.launch_count() == n0
+    UNetModel(config.TINY_UNET, usd, batch=2, height=20, width=28, use_cuda_graph=False)  # 80x112: on the grid
+
+
+def test_tiled_weights_are_freed_with_their_model(cuda_lib):
+    """The tiled copies the GEMM / convolution launches make of a model's weights are released with the model: building
+    models at several sizes one after another does not keep the dead ones' packed weights on the device."""
+    import gc
+
+    from b200sd.model import UNetModel
+
+    cfg = config.TINY_UNET
+    sd = config.random_state_dict(config.unet_param_shapes(cfg), seed=3, dtype=torch.float16)
+    x, c = _inputs(cfg, 4, hw=(16, 24))
+    gc.collect()
+    keys0 = set(cuda_lib._tiled_cache)
+    m = UNetModel(cfg, sd, batch=2, height=16, width=24, use_cuda_graph=False)
+    m(sample=x.half().numpy(), timestep=np.array([501.0, 501.0], np.float16), encoder_hidden_states=c.half().numpy())
+    torch.cuda.synchronize()
+    new = set(cuda_lib._tiled_cache) - keys0
+    tiled = sum(cuda_lib._tiled_cache[k][2].numel() * cuda_lib._tiled_cache[k][2].element_size() for k in new)
+    assert tiled > 0, "the tiny UNet made no tiled weight copies"
+    before = torch.cuda.memory_allocated()
+    del m
+    gc.collect()
+    torch.cuda.synchronize()
+    assert not new & set(cuda_lib._tiled_cache)
+    assert before - torch.cuda.memory_allocated() >= tiled, (before - torch.cuda.memory_allocated(), tiled)

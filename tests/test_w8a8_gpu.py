@@ -287,9 +287,10 @@ _FUSION_ENV = ("B200SD_FUSED", "B200SD_HALO_TMA", "B200SD_FOLD_SC", "B200SD_CLUS
                "B200SD_STAGED", "B200SD_TILED_W")
 
 
-@pytest.mark.parametrize("name", ["sd21_b2", "sd15_b2", "sdxl_1024_b2"])
+@pytest.mark.parametrize("name", ["sd21_b2", "sd15_b2", "sdxl_1024_b2", "sd15_512x768_b2", "sdxl_768x1344_b2"])
 def test_every_int8_launch_of_the_w8a8_models_is_exact(cuda_lib, monkeypatch, name):
-    """W8A8 SD-2.1-base and SD-1.5 at 512^2 and SDXL at 1024^2 (random init, batch 2), every eligible layer quantized
+    """W8A8 SD-2.1-base and SD-1.5 at 512^2, SDXL at 1024^2, and SD-1.5 at 512x768 and SDXL at 768x1344 on non-square
+    maps (random init, batch 2), every eligible layer quantized
     with scales from a calibration pass of the fp16 engine on the same inputs.  Every conv3x3_s8 launch of one forward
     is recorded and replayed exactly on the CPU (a sample of 1024 rows plus the tail tile per launch), with the plan the
     planner picks for it."""
@@ -302,7 +303,7 @@ def test_every_int8_launch_of_the_w8a8_models_is_exact(cuda_lib, monkeypatch, na
     for k in _FUSION_ENV:
         monkeypatch.delenv(k, raising=False)
     m = MC.build(name)  # fp16, random init seed 5
-    cfg, batch, hw = dict(m.engine.cfg), m.batch, m.h
+    cfg, batch, lat_h, lat_w = dict(m.engine.cfg), m.batch, m.h, m.w
     inputs = MC.model_inputs(m, seed=1)
     slots = m.engine.set_calibration(True)
     m(**inputs)
@@ -311,7 +312,7 @@ def test_every_int8_launch_of_the_w8a8_models_is_exact(cuda_lib, monkeypatch, na
     del m, slots
     torch.cuda.empty_cache()
     sd = C.random_state_dict(C.unet_param_shapes(cfg), seed=5, dtype=torch.float16)
-    qm = UNetModel(cfg, sd, batch=batch, height=hw, width=hw, use_cuda_graph=False, quantization=recipe)
+    qm = UNetModel(cfg, sd, batch=batch, height=lat_h, width=lat_w, use_cuda_graph=False, quantization=recipe)
     del sd
     calls = []
     orig = L.conv3x3_s8
