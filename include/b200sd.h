@@ -135,6 +135,10 @@ typedef struct {
     const void* a2;
     const void* a3;
     int32_t c2, c3;
+    /* > 0: int8 output (the operand of a W8A8 consumer) instead of fp16: out[row, col] = clamp(rint(y * out_s8_inv_scale),
+     * -127, 127) of the fp32 y after bias / GEGLU / residual.  Linear GEMMs (mode 0) of b200sd_gemm and
+     * b200sd_gemm_s8_linear on the plain or GEGLU epilogue: n a multiple of 32, no split-K, out_f32, act, cs_* or rs_out. */
+    float out_s8_inv_scale;
 } b200sd_gemm_args;
 
 int b200sd_gemm(const b200sd_gemm_args* args, void* stream);
@@ -152,7 +156,7 @@ int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8);
 int b200sd_gemm_plan_ex_bf16(const b200sd_gemm_args* args, int32_t* out8);
 /* host-only: human-readable tiling plan the launcher would use, "key=value" fields separated by spaces (tile shape,
  * split-K, pipeline depth, ..., variant = epilogue instantiation of the GEMM kernel: 0 generic, 1 split-K partial,
- * 2 GEGLU, 3 fp32 output, 4 plain, 5 staged, -1 halo convolution; halo_kind 0 / 1 / 2 and halo_wide for the halo
+ * 2 GEGLU, 3 fp32 output, 4 plain, 5 staged, 6 int8 output, 7 GEGLU with int8 output, -1 halo convolution; halo_kind 0 / 1 / 2 and halo_wide for the halo
  * kernel's instantiation).  Halo calls are planned like b200sd_gemm_plan_ex */
 int b200sd_gemm_describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size);
 int b200sd_gemm_describe_plan_bf16(const b200sd_gemm_args* args, char* buf, size_t buf_size);
@@ -170,6 +174,18 @@ int b200sd_gemm_s8(const b200sd_gemm_args* args, const float* col_scale, void* s
 int b200sd_gemm_plan_ex_s8(const b200sd_gemm_args* args, int32_t* out8);
 int b200sd_gemm_describe_plan_s8(const b200sd_gemm_args* args, char* buf, size_t buf_size);
 size_t b200sd_gemm_workspace_bytes_s8(const b200sd_gemm_args* args);
+
+/* ---- W8A8 linear GEMM (int8 wgmma, s32 accumulators): the UNet transformers' projections --------------------------
+ * a0: int8 [m, c0] (c0 a multiple of 16); wgt: int8 pre-tiled [n_tiles][k_blocks][block_n][128] (each row zero padded to
+ * whole 128-channel k-blocks; wgt_tiled = 1 and the planned block_n); col_scale: fp32 [n], s_a * s_w[col].
+ * y[row, col] = float(acc) * col_scale[col] + bias[col], then GEGLU (interleaved value / gate rows, as b200sd_gemm) and
+ * + fp16 residual; stored fp16 (with rs_out row statistics if asked) or int8 (out_s8_inv_scale > 0).  Split-K as
+ * b200sd_gemm for fp16 outputs without GEGLU / rs_out.  Supports mode 0 only; rejects mode 1, a1 / a2 / a3, act,
+ * out_f32, bias_rows, pad_after_only, halo, upsample2x, gn_*, cs_* and ln_* with an error naming the field. */
+int b200sd_gemm_s8_linear(const b200sd_gemm_args* args, const float* col_scale, void* stream);
+int b200sd_gemm_plan_ex_s8_linear(const b200sd_gemm_args* args, int32_t* out8);
+int b200sd_gemm_describe_plan_s8_linear(const b200sd_gemm_args* args, char* buf, size_t buf_size);
+size_t b200sd_gemm_workspace_bytes_s8_linear(const b200sd_gemm_args* args);
 
 /* ---- palettized weights (n-bit lookup-table weights decoded in the GEMM producer) -------------------------------
  * The B operand of b200sd_gemm given as palette indices: weight[j, k] = fp16_rn(float(lut[seg(j)][idx[j, k]]) *
@@ -235,6 +251,10 @@ int b200sd_group_norm_apply(const void* x0, const void* x1, int32_t c0, int32_t 
  * x_hat*w+b convention of the checkpoint, cf. unet.py:132-138). */
 int b200sd_layer_norm(const void* x, const float* gamma, const float* beta, void* out, int32_t rows,
                       int32_t c, float eps, void* stream);
+/* b200sd_layer_norm whose output is the int8 operand of b200sd_gemm_s8_linear: the fp32 normalised value y is stored as
+ * q = clamp(rint(y * inv_scale), -127, 127) (inv_scale = 1 / s_a > 0). */
+int b200sd_layer_norm_s8(const void* x, const float* gamma, const float* beta, float inv_scale, void* out, int32_t rows,
+                         int32_t c, float eps, void* stream);
 
 /* row softmax of fp32 scores [rows, cols] -> fp16 probabilities, exp2 domain; used only for the VAE
  * decoder's single-head d=512 mid-block attention (diffusers AutoencoderKL via torch2coreml.py:584-594),

@@ -107,6 +107,7 @@ struct __align__(64) GemmParams {
     const __half* lut;         // [3][256] palettes of output rows [0, seg_end0), [seg_end0, seg_end1), [seg_end1, N)
     const float* kscale;       // [kb_total * 64] per-k scale (LayerNorm fold) or null
     int nbits, pk_box, pk_slots, seg_end0, seg_end1;
+    float out_inv_scale;       // int8 output (kOutS8): q = clamp(rint(y * out_inv_scale), -127, 127)
 };
 
 struct TileCoord {
@@ -177,7 +178,9 @@ __device__ __forceinline__ void split_range(const GemmParams& p, int split, int&
 // kGeneric = false: compile-time variant for the hot shapes (N % 16 == 0, 16-byte aligned rows): straight-line
 // vector code only, which keeps the kernel small enough for the instruction cache of these microsecond kernels.
 // T: the 16-bit type of the residual and of a 16-bit output (fp16, or bf16 for the overflow-prone VAEs).
-template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial>
+// kOutS8: the output is int8, q = clamp(rint(y * p.out_inv_scale), -127, 127) of the fp32 y after bias / GEGLU /
+// residual (the operand of an int8 consumer); regular variants only (!kGeneric, no partials, no row statistics).
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kOutS8 = false>
 __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&acc)[16], int out_row, int col0,
                                                  int split, const float* bias, const T* res, float2& rowacc) {
     using E = Elem16<T>;
@@ -249,6 +252,23 @@ __device__ __forceinline__ void epilogue_store16(const GemmParams& p, float (&ac
             for (int j = 0; j < 16; ++j)
                 if (j < nvals && ocol0 + j < ld) acc[j] += E::to_float(res[j]);
         }
+    }
+    if constexpr (kOutS8) {
+        static_assert(!kGeneric && !kPartial && !kOutF32, "int8 output: regular epilogue variants only");
+        int8_t* o = reinterpret_cast<int8_t*>(p.out) + off;
+        float f[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] = acc[e];
+        const uint2 lo = quantize8_s8(f, p.out_inv_scale);
+        if (nvals == 8) {
+            *reinterpret_cast<uint2*>(o) = lo;
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) f[e] = acc[8 + e];
+            const uint2 hi = quantize8_s8(f, p.out_inv_scale);
+            *reinterpret_cast<uint4*>(o) = make_uint4(lo.x, lo.y, hi.x, hi.y);
+        }
+        return;
     }
     if (out_f32) {
         float* o = reinterpret_cast<float*>(p.out) + off;
@@ -782,7 +802,8 @@ __device__ __forceinline__ void lut_decode_stage(const GemmParams& p, const uint
     }
 }
 
-template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN, bool kS8, bool kLut = false>
+template <typename T, bool kGeneric, bool kGeglu, bool kOutF32, bool kPartial, bool kStaged, int kBN, bool kS8, bool kLut = false,
+          bool kOutS8 = false>
 __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
     constexpr int kChunk = kS8 ? 2 * kBK : kBK;  // channels per k-block (128 bytes either way)
     // 1024-byte aligned by declaration (SWIZZLE_128B atoms): keeping the base a plain shared-memory symbol -- not an
@@ -1086,7 +1107,8 @@ __device__ __forceinline__ void gemm_kernel_body(const GemmParams& p) {
                         else if (kGeneric && p.residual != nullptr)
                             rptr = reinterpret_cast<const T*>(p.residual + static_cast<size_t>(out_row) * p.n_store +
                                                               ((ncol0 + c) >> (p.geglu ? 1 : 0)));
-                        epilogue_store16<T, kGeneric, kGeglu, kOutF32, kPartial>(p, a16, out_row, ncol0 + c, t.split, bptr, rptr, rowacc);
+                        epilogue_store16<T, kGeneric, kGeglu, kOutF32, kPartial, kOutS8>(p, a16, out_row, ncol0 + c, t.split, bptr, rptr,
+                                                                                          rowacc);
                     };
                     auto process32 = [&](const uint32_t (&v)[32], int c) {
                         if (!valid) return;
@@ -1158,6 +1180,22 @@ __global__ void __launch_bounds__(kGemmThreads, 1) igmma_conv_kernel(const __gri
     gemm_kernel_body<__half, kGeneric, false, false, kPartial, false, kBN, true>(p);
 }
 
+// W8A8 linear GEMM (b200sd_gemm_s8_linear), the epilogues only its launches use: GEGLU (fp16 or int8 output) and a
+// plain int8 output.  Its generic, plain and split-K launches run igmma_conv_kernel, whose body branches on p.mode.
+template <bool kGeglu, bool kOutS8, int kBN>
+__global__ void __launch_bounds__(kGemmThreads, 1) igmma_linear_kernel(const __grid_constant__ GemmParams p) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gemm_kernel_body<__half, false, kGeglu, false, false, false, kBN, true, false, kOutS8>(p);
+}
+
+// fp16 linear GEMM whose output is the int8 operand of a W8A8 consumer (b200sd_gemm with out_s8_inv_scale > 0):
+// plain and GEGLU epilogues.
+template <bool kGeglu, int kBN>
+__global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_s8out_kernel(const __grid_constant__ GemmParams p) {
+    // the shared body executes pdl_wait() before its first access to global memory
+    gemm_kernel_body<__half, false, kGeglu, false, false, false, kBN, false, false, true>(p);
+}
+
 
 // Tile widths the GEMM kernel is compiled for; plan_gemm chooses among exactly these (widest first).
 static constexpr int kGemmWidths[] = {256, 192, 160, 128, 96, 64, 32, 16};
@@ -1197,6 +1235,22 @@ static KernelFn s8_kernel(int width_index) {
                                                  B200SD_S8_FN(128), B200SD_S8_FN(96),  B200SD_S8_FN(64),
                                                  B200SD_S8_FN(32),  B200SD_S8_FN(16)};
 #undef B200SD_S8_FN
+    return fns[width_index];
+}
+// the int8-output and int8 GEGLU epilogues are regular variants only: widths >= 32
+template <bool kS8, bool kGeglu, bool kOutS8, int kBN>
+static constexpr KernelFn s8io_fn() {
+    if constexpr (kBN == 16) return nullptr;
+    else if constexpr (kS8) return igmma_linear_kernel<kGeglu, kOutS8, kBN>;
+    else return wgmma_gemm_s8out_kernel<kGeglu, kBN>;
+}
+template <bool kS8, bool kGeglu, bool kOutS8>
+static KernelFn s8io_kernel(int width_index) {
+#define B200SD_S8IO_FN(bn) s8io_fn<kS8, kGeglu, kOutS8, bn>()
+    static const KernelFn fns[kNumGemmWidths] = {B200SD_S8IO_FN(256), B200SD_S8IO_FN(192), B200SD_S8IO_FN(160),
+                                                 B200SD_S8IO_FN(128), B200SD_S8IO_FN(96),  B200SD_S8IO_FN(64),
+                                                 B200SD_S8IO_FN(32),  B200SD_S8IO_FN(16)};
+#undef B200SD_S8IO_FN
     return fns[width_index];
 }
 
@@ -1670,7 +1724,8 @@ struct GemmPlan {
 // Epilogue instantiations of wgmma_gemm_kernel, each compiled for every width of kGemmWidths (plan_gemm sends width 16
 // to the generic one: the others need block_n % 32 == 0)
 enum GemmVariant {
-    kVariantGeneric = 0, kVariantSplitK = 1, kVariantGeglu = 2, kVariantF32 = 3, kVariantPlain = 4, kVariantStaged = 5
+    kVariantGeneric = 0, kVariantSplitK = 1, kVariantGeglu = 2, kVariantF32 = 3, kVariantPlain = 4, kVariantStaged = 5,
+    kVariantS8Out = 6, kVariantGegluS8Out = 7  // int8 output: wgmma_gemm_s8out_kernel / igmma_linear_kernel
 };
 
 static bool cluster_splitk_enabled() {
@@ -1800,8 +1855,26 @@ static int halo_pick_block_n(const b200sd_gemm_args& a) {
 // s8: the W8A8 convolution (b200sd_gemm_s8): int8 activations and weights, k-blocks of 128 channels.  It serves the
 // stride-1 pad-1 3x3 convolution of one source with a bias vector or per-image bias rows, an fp16 residual, fp16 output
 // and split-K; everything else is rejected by name.
-static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false, bool s8 = false) {
-    if (s8) {
+// s8_linear: the W8A8 linear GEMM (b200sd_gemm_s8_linear, s8 set too): mode 0, one int8 source [m, c0], bias, fp16
+// residual, GEGLU, row statistics, fp16 or int8 output, split-K (fp16 output); everything else is rejected by name.
+// out_s8_inv_scale > 0 (fp16 or int8 operands): int8 output of a linear GEMM on the plain or GEGLU epilogue, no split-K.
+static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false, bool s8 = false, bool s8_linear = false) {
+    if (s8_linear) {
+        B200SD_REQUIRE(a.mode == 0, "b200sd_gemm_s8_linear: mode=%d is not supported (the linear GEMM, mode 0)", a.mode);
+        B200SD_REQUIRE(!a.a1 && a.c1 == 0, "b200sd_gemm_s8_linear: a1 (second source) is not supported");
+        B200SD_REQUIRE(!a.a2 && !a.a3 && a.c2 == 0 && a.c3 == 0, "b200sd_gemm_s8_linear: a2 / a3 (folded shortcut) are not supported");
+        B200SD_REQUIRE(!a.pad_after_only, "b200sd_gemm_s8_linear: pad_after_only is not supported");
+        B200SD_REQUIRE(a.act == 0, "b200sd_gemm_s8_linear: act=%d is not supported", a.act);
+        B200SD_REQUIRE(!a.out_f32, "b200sd_gemm_s8_linear: out_f32 is not supported (fp16 or int8 output)");
+        B200SD_REQUIRE(a.bias_rows == 0, "b200sd_gemm_s8_linear: bias_rows is not supported (one bias vector)");
+        B200SD_REQUIRE(!a.halo, "b200sd_gemm_s8_linear: halo is not supported");
+        B200SD_REQUIRE(!a.upsample2x, "b200sd_gemm_s8_linear: upsample2x is not supported");
+        B200SD_REQUIRE(a.gn_groups == 0 && !a.gn_chan0 && !a.gn_chan1 && !a.gn_gamma && !a.gn_beta,
+                       "b200sd_gemm_s8_linear: gn_* (fused GroupNorm) is not supported");
+        B200SD_REQUIRE(!a.cs_partial && !a.cs_chan && !a.cs_tickets, "b200sd_gemm_s8_linear: cs_* (column statistics) are not supported");
+        B200SD_REQUIRE(a.ln_parts == 0 && !a.ln_stat && !a.ln_wg, "b200sd_gemm_s8_linear: ln_* (LayerNorm fold) is not supported");
+        B200SD_REQUIRE(a.c0 > 0 && a.c0 % 16 == 0, "b200sd_gemm_s8_linear: c0=%d must be a positive multiple of 16 (TMA row stride)", a.c0);
+    } else if (s8) {
         B200SD_REQUIRE(a.mode == 1, "b200sd_gemm_s8: mode=%d is not supported (the 3x3 convolution, mode 1)", a.mode);
         B200SD_REQUIRE(a.stride == 1, "b200sd_gemm_s8: stride=%d is not supported (1)", a.stride);
         B200SD_REQUIRE(!a.pad_after_only, "b200sd_gemm_s8: pad_after_only is not supported");
@@ -1853,6 +1926,13 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false,
                    "b200sd_gemm: statistics outputs need a plain fp16 epilogue without split-K");
     B200SD_REQUIRE(a.ln_parts == 0 || (a.mode == 0 && a.ln_stat && a.ln_wg && a.split_k <= 1),
                    "b200sd_gemm: LayerNorm fold needs mode 0, statistics, the fold vector and no split-K");
+    const bool out_s8 = a.out_s8_inv_scale != 0.f;
+    B200SD_REQUIRE(!out_s8 || (std::isfinite(a.out_s8_inv_scale) && a.out_s8_inv_scale > 0.f),
+                   "b200sd_gemm: out_s8_inv_scale=%g must be positive and finite", static_cast<double>(a.out_s8_inv_scale));
+    B200SD_REQUIRE(!out_s8 || (!bf16 && a.mode == 0 && !a.halo && !a.out_f32 && !want_stats && a.act == 0 && a.split_k <= 1 &&
+                               a.n % 32 == 0),
+                   "b200sd_gemm: out_s8_inv_scale (int8 output) needs an fp16 / int8 linear GEMM (mode 0) without halo, out_f32, "
+                   "cs_* / rs_out, act or split-K, n a multiple of 32");
     if (a.halo) return plan_halo(a, pl);
     if (a.mode == 0) {
         B200SD_REQUIRE(a.m > 0, "b200sd_gemm: m=%d", a.m);
@@ -1892,7 +1972,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false,
     // spread of a single shape), so they were kept.  The largest misses: conv 2560->1280 at 8x8 (1.3x) and linear
     // 1280->1280 at M = 512 (1.25x). ----
     const int sms = num_sms();
-    const bool can_split = !bf16 && !a.geglu && a.n % 4 == 0 && a.act == 0 && !want_stats && a.ln_parts == 0;
+    const bool can_split = !bf16 && !a.geglu && a.n % 4 == 0 && a.act == 0 && !want_stats && a.ln_parts == 0 && !out_s8;
     auto epi_cycles = [&](int bn) { return 400.0 + (bn / 32.0) * (a.geglu ? 520.0 : 230.0); };
     auto kb_cycles = [&](int bn) { return std::max(2.0 * bn, (kAStage + 128.0 * bn) / 38.0); };
     double best_t = 1e30;
@@ -1903,7 +1983,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false,
         if (a.block_n > 0 && bn != a.block_n) continue;
         const int nt = (a.n + bn - 1) / bn;
         if (a.block_n == 0 && bn > 16 && nt * bn > a.n + a.n / 4 + 15) continue;  // > 25 % padding
-        if (want_stats && bn % 32 != 0) continue;
+        if ((want_stats || out_s8) && bn % 32 != 0) continue;
         const int stages_bn = std::min(kMaxStages, (smem_budget() - kEpiFixed) / (kAStage + bn * kBK * 2));
         for (int sp : kSplits) {
             if (a.split_k > 0 && sp != a.split_k) continue;
@@ -1974,7 +2054,7 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false,
     const int per_stage = kAStage + pl.block_n * kBK * 2;
     {
         // staged epilogue: fp16 tile in shared memory, row-contiguous residual reads / stores, statistics outputs
-        const bool eligible = !bf16 && !s8 && regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
+        const bool eligible = !bf16 && !s8 && !out_s8 && regular && pl.splits == 1 && !a.geglu && !a.out_f32 && a.n % 8 == 0;
         // column statistics need the staged epilogue; row statistics alone ride on the register epilogue (every thread
         // owns a row there), which keeps the residual tile prefetched in shared memory during the main loop
         pl.staged = (eligible && (a.cs_partial != nullptr || (a.residual != nullptr && staged_enabled()))) ? 1 : 0;
@@ -2010,7 +2090,10 @@ static int plan_gemm(const b200sd_gemm_args& a, GemmPlan& pl, bool bf16 = false,
     // compile-time epilogue variants for the hot shapes; anything irregular takes the generic kernel (split-K and the
     // staged epilogue read the residual row-contiguously, so they need no residual tile in shared memory)
     const bool regular_epi = regular || (regular_shape && a.residual != nullptr && (pl.splits > 1 || pl.staged));
-    if (!regular_epi) pl.variant = kVariantGeneric;
+    B200SD_REQUIRE(!out_s8 || regular, "b200sd_gemm: out_s8_inv_scale (int8 output) needs the regular epilogue (n=%d block_n=%d)",
+                   a.n, pl.block_n);
+    if (out_s8) pl.variant = a.geglu ? kVariantGegluS8Out : kVariantS8Out;
+    else if (!regular_epi) pl.variant = kVariantGeneric;
     else if (pl.staged) pl.variant = kVariantStaged;
     else if (pl.splits > 1) pl.variant = kVariantSplitK;
     else if (a.geglu) pl.variant = kVariantGeglu;
@@ -2036,6 +2119,7 @@ static int plan_lut(const b200sd_gemm_args& a, const b200sd_lut_args& l, GemmPla
     B200SD_REQUIRE(!a.cs_partial && !a.cs_chan && !a.cs_tickets, "b200sd_gemm_lut: cs_* (column statistics) are not supported");
     B200SD_REQUIRE(!a.a2 && !a.a3 && a.c2 == 0 && a.c3 == 0, "b200sd_gemm_lut: a2 / a3 (folded shortcut) are not supported");
     B200SD_REQUIRE(!a.out_f32, "b200sd_gemm_lut: out_f32 is not supported");
+    B200SD_REQUIRE(a.out_s8_inv_scale == 0.f, "b200sd_gemm_lut: out_s8_inv_scale (int8 output) is not supported");
     // whole 64-channel k-blocks per source: k-block kb holds weight columns [64 kb, 64 kb + 64), no padding positions
     B200SD_REQUIRE(a.c0 % kBK == 0 && a.c1 % kBK == 0, "b200sd_gemm_lut: c0=%d / c1=%d must be multiples of 64", a.c0, a.c1);
     B200SD_REQUIRE(l.packed && l.lut, "b200sd_gemm_lut: packed / lut is null");
@@ -2069,16 +2153,17 @@ static int plan_lut(const b200sd_gemm_args& a, const b200sd_lut_args& l, GemmPla
 extern void count_launch(int n);
 
 static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16, const float* col_scale = nullptr,
-                       const b200sd_lut_args* lut = nullptr) {
+                       const b200sd_lut_args* lut = nullptr, bool s8_linear = false) {
     const bool s8 = col_scale != nullptr;
+    const char* s8_name = s8_linear ? "b200sd_gemm_s8_linear" : "b200sd_gemm_s8";
     GemmPlan pl;
     if (lut) {
         if (int rc = plan_lut(a, *lut, pl)) return rc;
-    } else if (int rc = plan_gemm(a, pl, bf16, s8)) {
+    } else if (int rc = plan_gemm(a, pl, bf16, s8, s8_linear)) {
         return rc;
     }
     B200SD_REQUIRE(a.a0 && (a.wgt || lut) && a.out, "b200sd_gemm: null pointer");
-    B200SD_REQUIRE(!s8 || a.wgt_tiled, "b200sd_gemm_s8: the weights must be pre-tiled (wgt_tiled = 1, explicit block_n)");
+    B200SD_REQUIRE(!s8 || a.wgt_tiled, "%s: the weights must be pre-tiled (wgt_tiled = 1, explicit block_n)", s8_name);
     B200SD_REQUIRE(a.c1 == 0 || a.a1, "b200sd_gemm: a1 is null but c1 > 0");
     const size_t ws = plan_workspace(pl);
     B200SD_REQUIRE(ws == 0 || (a.workspace && a.workspace_bytes >= ws),
@@ -2108,6 +2193,13 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
                     return rc;
             }
         }
+    } else if (s8 && a.mode == 0) {
+        // int8 [m, c0] source: a box is 128 channels (128 bytes, one swizzle row) of 128 rows, the channel tail is zero filled
+        const uint32_t box[2] = {2 * kBK, kBM};
+        const uint64_t dims[2] = {static_cast<uint64_t>(a.c0), static_cast<uint64_t>(a.m)};
+        const uint64_t str[1] = {static_cast<uint64_t>(a.c0)};
+        if (int rc = encode_tmap(&p.tmA0, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.a0, 2, dims, str, box, es1)) return rc;
+        p.tmA1 = p.tmA2 = p.tmA3 = p.tmA0;
     } else if (a.mode == 0) {
         const uint32_t box[2] = {kBK, kBM};
         {
@@ -2166,7 +2258,7 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
         p.nbits = lut->nbits, p.pk_box = pl.pk_box, p.pk_slots = pl.pk_slots;
         p.seg_end0 = lut->seg_end0, p.seg_end1 = lut->seg_end1;
     } else if (s8) {
-        B200SD_REQUIRE(a.block_n == pl.block_n, "b200sd_gemm_s8: tiled weights need an explicit block_n");
+        B200SD_REQUIRE(a.block_n == pl.block_n, "%s: tiled weights need an explicit block_n", s8_name);
         const uint64_t rows = static_cast<uint64_t>(pl.n_tiles) * pl.kb_total * pl.block_n;
         const uint64_t dims[2] = {2 * kBK, rows};
         const uint64_t str[1] = {2 * kBK};
@@ -2278,6 +2370,7 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
     const int variant = pl.variant;
     KernelFn fn = nullptr;
     p.col_scale = col_scale;
+    p.out_inv_scale = a.out_s8_inv_scale;
     if (lut) {
         switch (variant) {
             case kVariantGeneric: fn = lut_kernel<true, false, false>(wi); break;
@@ -2286,11 +2379,14 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
             case kVariantPlain: fn = lut_kernel<false, false, false>(wi); break;
             default: break;
         }
-    } else if (s8) {  // plan_gemm gives int8 only these three variants
+    } else if (s8) {  // plan_gemm gives the int8 convolution the first three variants only
         switch (variant) {
             case kVariantGeneric: fn = s8_kernel<true, false>(wi); break;
             case kVariantSplitK: fn = s8_kernel<false, true>(wi); break;
             case kVariantPlain: fn = s8_kernel<false, false>(wi); break;
+            case kVariantGeglu: fn = s8io_kernel<true, true, false>(wi); break;
+            case kVariantS8Out: fn = s8io_kernel<true, false, true>(wi); break;
+            case kVariantGegluS8Out: fn = s8io_kernel<true, true, true>(wi); break;
             default: break;
         }
     } else if (bf16) {  // plan_gemm gives bf16 only these three variants
@@ -2307,6 +2403,8 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
             case kVariantSplitK: fn = gemm_kernel<__half, false, false, false, true, false>(wi); break;
             case kVariantGeglu: fn = gemm_kernel<__half, false, true, false, false, false>(wi); break;
             case kVariantF32: fn = gemm_kernel<__half, false, false, true, false, false>(wi); break;
+            case kVariantS8Out: fn = s8io_kernel<false, false, true>(wi); break;
+            case kVariantGegluS8Out: fn = s8io_kernel<false, true, true>(wi); break;
             default: fn = gemm_kernel<__half, false, false, false, false, false>(wi); break;
         }
     }
@@ -2318,7 +2416,7 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
         p.bias = nullptr;
         p.residual = nullptr;
     }
-    static bool attr_set[4][6][kNumGemmWidths] = {};
+    static bool attr_set[4][8][kNumGemmWidths] = {};
     const int dt = lut ? 3 : (s8 ? 2 : (bf16 ? 1 : 0));
     if (!attr_set[dt][variant][wi]) {
         B200SD_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -2367,13 +2465,16 @@ static int launch_gemm(const b200sd_gemm_args& a, cudaStream_t stream, bool bf16
 
 }  // namespace b200sd
 
-static int gemm_entry(const b200sd_gemm_args* args, void* stream, bool bf16, const float* col_scale = nullptr) {
+static int gemm_entry(const b200sd_gemm_args* args, void* stream, bool bf16, const float* col_scale = nullptr,
+                      bool s8_linear = false) {
     if (!b200sd::launch_class_enabled(1)) return 0;  // bench.py's per-class timing graphs
     if (!args) {
-        b200sd::set_error(col_scale ? "b200sd_gemm_s8: args is null" : (bf16 ? "b200sd_gemm_bf16: args is null" : "b200sd_gemm: args is null"));
+        b200sd::set_error(s8_linear ? "b200sd_gemm_s8_linear: args is null"
+                                    : (col_scale ? "b200sd_gemm_s8: args is null"
+                                                 : (bf16 ? "b200sd_gemm_bf16: args is null" : "b200sd_gemm: args is null")));
         return 2;
     }
-    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream), bf16, col_scale);
+    return b200sd::launch_gemm(*args, static_cast<cudaStream_t>(stream), bf16, col_scale, nullptr, s8_linear);
 }
 
 extern "C" int b200sd_gemm(const b200sd_gemm_args* args, void* stream) { return gemm_entry(args, stream, false); }
@@ -2384,6 +2485,13 @@ extern "C" int b200sd_gemm_s8(const b200sd_gemm_args* args, const float* col_sca
         return 2;
     }
     return gemm_entry(args, stream, false, col_scale);
+}
+extern "C" int b200sd_gemm_s8_linear(const b200sd_gemm_args* args, const float* col_scale, void* stream) {
+    if (!col_scale) {
+        b200sd::set_error("b200sd_gemm_s8_linear: col_scale is null");
+        return 2;
+    }
+    return gemm_entry(args, stream, false, col_scale, true);
 }
 
 extern "C" int b200sd_gemm_lut(const b200sd_gemm_args* args, const b200sd_lut_args* lut, void* stream) {
@@ -2416,19 +2524,19 @@ extern "C" int b200sd_gemm_plan(const b200sd_gemm_args* args, int32_t* out4) {
 
 // Planning query before the weights are tiled: a halo call plans for chunk-major tiled weights of the requested (or the
 // preferred) width.
-static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl, bool bf16, bool s8 = false) {
+static int plan_query(const b200sd_gemm_args* args, b200sd::GemmPlan& pl, bool bf16, bool s8 = false, bool s8_linear = false) {
     b200sd_gemm_args a = *args;
     if (a.halo && !bf16 && !s8) {
         if (a.block_n == 0) a.block_n = b200sd::halo_pick_block_n(a);
         a.wgt_tiled = 1;
     }
-    return b200sd::plan_gemm(a, pl, bf16, s8);
+    return b200sd::plan_gemm(a, pl, bf16, s8, s8_linear);
 }
 
-static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16, bool s8 = false) {
+static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16, bool s8 = false, bool s8_linear = false) {
     if (!args || !out8) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = plan_query(args, pl, bf16, s8)) return rc;
+    if (int rc = plan_query(args, pl, bf16, s8, s8_linear)) return rc;
     out8[0] = pl.block_n, out8[1] = pl.splits, out8[2] = pl.kb_total, out8[3] = pl.n_tiles;
     out8[4] = pl.cs_slots, out8[5] = pl.staged, out8[6] = pl.stages, out8[7] = pl.m_tiles;
     return 0;
@@ -2437,11 +2545,15 @@ static int plan_ex(const b200sd_gemm_args* args, int32_t* out8, bool bf16, bool 
 extern "C" int b200sd_gemm_plan_ex(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, false); }
 extern "C" int b200sd_gemm_plan_ex_bf16(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, true); }
 extern "C" int b200sd_gemm_plan_ex_s8(const b200sd_gemm_args* args, int32_t* out8) { return plan_ex(args, out8, false, true); }
+extern "C" int b200sd_gemm_plan_ex_s8_linear(const b200sd_gemm_args* args, int32_t* out8) {
+    return plan_ex(args, out8, false, true, true);
+}
 
-static int describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size, bool bf16, bool s8 = false) {
+static int describe_plan(const b200sd_gemm_args* args, char* buf, size_t buf_size, bool bf16, bool s8 = false,
+                         bool s8_linear = false) {
     if (!args || !buf || buf_size == 0) return 2;
     b200sd::GemmPlan pl;
-    if (int rc = plan_query(args, pl, bf16, s8)) return rc;
+    if (int rc = plan_query(args, pl, bf16, s8, s8_linear)) return rc;
     // variant: GemmVariant of the GEMM kernel (-1: halo convolution); halo_kind / halo_wide: which halo_conv_kernel
     // instantiation runs (-1 / 0 for the GEMM kernel); win: the halo walk over th x tw windows instead of image rows
     snprintf(buf, buf_size,
@@ -2462,6 +2574,9 @@ extern "C" int b200sd_gemm_describe_plan_bf16(const b200sd_gemm_args* args, char
 extern "C" int b200sd_gemm_describe_plan_s8(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
     return describe_plan(args, buf, buf_size, false, true);
 }
+extern "C" int b200sd_gemm_describe_plan_s8_linear(const b200sd_gemm_args* args, char* buf, size_t buf_size) {
+    return describe_plan(args, buf, buf_size, false, true, true);
+}
 
 extern "C" size_t b200sd_gemm_workspace_bytes(const b200sd_gemm_args* args) {
     if (!args) return 0;
@@ -2474,5 +2589,12 @@ extern "C" size_t b200sd_gemm_workspace_bytes_s8(const b200sd_gemm_args* args) {
     if (!args) return 0;
     b200sd::GemmPlan pl;
     if (b200sd::plan_gemm(*args, pl, false, true)) return 0;
+    return b200sd::plan_workspace(pl);
+}
+
+extern "C" size_t b200sd_gemm_workspace_bytes_s8_linear(const b200sd_gemm_args* args) {
+    if (!args) return 0;
+    b200sd::GemmPlan pl;
+    if (b200sd::plan_gemm(*args, pl, false, true, true)) return 0;
     return b200sd::plan_workspace(pl);
 }

@@ -517,12 +517,12 @@ static unsigned int* gn_tickets() {
 }
 
 // ---- LayerNorm over channels of [rows, c]; one warp per row, two-pass in registers -----------
-template <int kVecsPerLane>
-__global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restrict__ x, const float* __restrict__ gamma,
-                                                         const float* __restrict__ beta, __half* __restrict__ out,
-                                                         int rows, int c, float eps) {
-    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
-    pdl_wait();
+// kS8: the W8A8 linear's operand -- the fp32 result y is stored as int8 q = clamp(rint(y * inv_scale), -127, 127) to
+// out_s8 instead of as fp16 to out.
+template <int kVecsPerLane, bool kS8>
+__device__ __forceinline__ void layer_norm_body(const __half* __restrict__ x, const float* __restrict__ gamma,
+                                                const float* __restrict__ beta, __half* __restrict__ out,
+                                                int8_t* __restrict__ out_s8, float inv_scale, int rows, int c, float eps) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (warp >= rows) return;
@@ -566,7 +566,7 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restric
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
     const float rstd = rsqrtf(sq / c + eps);
-    __half* dst = out + static_cast<size_t>(warp) * c;
+    __half* dst = kS8 ? nullptr : out + static_cast<size_t>(warp) * c;
 #pragma unroll
     for (int k = 0; k < kVecsPerLane; ++k) {
         const int v = lane + 32 * k;
@@ -580,6 +580,10 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restric
             const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
             for (int e = 0; e < 8; ++e) y[e] = (f[k][e] - mean) * rstd * gg[e] + bb[e];
+            if constexpr (kS8) {
+                *reinterpret_cast<uint2*>(out_s8 + static_cast<size_t>(warp) * c + v * 8) = quantize8_s8(y, inv_scale);
+                continue;
+            }
             uint4 pk;
             pk.x = pack_half2(y[0], y[1]);
             pk.y = pack_half2(y[2], y[3]);
@@ -588,6 +592,24 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restric
             *reinterpret_cast<uint4*>(dst + v * 8) = pk;
         }
     }
+}
+
+template <int kVecsPerLane>
+__global__ void __launch_bounds__(256) layer_norm_kernel(const __half* __restrict__ x, const float* __restrict__ gamma,
+                                                         const float* __restrict__ beta, __half* __restrict__ out,
+                                                         int rows, int c, float eps) {
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
+    pdl_wait();
+    layer_norm_body<kVecsPerLane, false>(x, gamma, beta, out, nullptr, 0.f, rows, c, eps);
+}
+
+template <int kVecsPerLane>
+__global__ void __launch_bounds__(256) layer_norm_s8_kernel(const __half* __restrict__ x, const float* __restrict__ gamma,
+                                                            const float* __restrict__ beta, int8_t* __restrict__ out,
+                                                            float inv_scale, int rows, int c, float eps) {
+    pdl_trigger();
+    pdl_wait();
+    layer_norm_body<kVecsPerLane, true>(x, gamma, beta, nullptr, out, inv_scale, rows, c, eps);
 }
 
 
@@ -830,6 +852,29 @@ extern "C" int b200sd_layer_norm(const void* x, const float* gamma, const float*
         B200SD_CHECK_CUDA(launch_kernel(layer_norm_kernel<5>, dim3(blocks), dim3(256), 0, stream, xi, gamma, beta, xo, rows, c, eps));
     else
         B200SD_CHECK_CUDA(launch_kernel(layer_norm_kernel<8>, dim3(blocks), dim3(256), 0, stream, xi, gamma, beta, xo, rows, c, eps));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_layer_norm_s8(const void* x, const float* gamma, const float* beta, float inv_scale, void* out,
+                                    int32_t rows, int32_t c, float eps, void* stream_) {
+    if (!b200sd::launch_class_enabled(4)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(x && gamma && beta && out, "b200sd_layer_norm_s8: null pointer");
+    B200SD_REQUIRE(c % 8 == 0 && c > 0 && c <= 2048, "b200sd_layer_norm_s8: c=%d must be a multiple of 8, <= 2048", c);
+    B200SD_REQUIRE(std::isfinite(inv_scale) && inv_scale > 0.f, "b200sd_layer_norm_s8: inv_scale=%g must be positive and finite",
+                   static_cast<double>(inv_scale));
+    const int per_lane = (c / 8 + 31) / 32;
+    const int blocks = (rows + 7) / 8;
+    const __half* xi = reinterpret_cast<const __half*>(x);
+    int8_t* xo = static_cast<int8_t*>(out);
+    if (per_lane <= 2)
+        B200SD_CHECK_CUDA(launch_kernel(layer_norm_s8_kernel<2>, dim3(blocks), dim3(256), 0, stream, xi, gamma, beta, xo, inv_scale, rows, c, eps));
+    else if (per_lane <= 5)
+        B200SD_CHECK_CUDA(launch_kernel(layer_norm_s8_kernel<5>, dim3(blocks), dim3(256), 0, stream, xi, gamma, beta, xo, inv_scale, rows, c, eps));
+    else
+        B200SD_CHECK_CUDA(launch_kernel(layer_norm_s8_kernel<8>, dim3(blocks), dim3(256), 0, stream, xi, gamma, beta, xo, inv_scale, rows, c, eps));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;

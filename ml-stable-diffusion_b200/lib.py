@@ -37,6 +37,7 @@ class GemmArgs(C.Structure):
         ("rs_out", C.c_void_p),
         ("ln_stat", C.c_void_p), ("ln_wg", C.c_void_p), ("ln_parts", C.c_int32), ("ln_eps", C.c_float),
         ("a2", C.c_void_p), ("a3", C.c_void_p), ("c2", C.c_int32), ("c3", C.c_int32),
+        ("out_s8_inv_scale", C.c_float),  # > 0: int8 output (the operand of a W8A8 consumer)
     ]
 
 
@@ -117,6 +118,12 @@ _SIGNATURES = {
     "b200sd_gemm_plan_ex_s8": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(C.c_int32)]),
     "b200sd_gemm_describe_plan_s8": (C.c_int, [C.POINTER(GemmArgs), C.c_char_p, C.c_size_t]),
     "b200sd_gemm_workspace_bytes_s8": (C.c_size_t, [C.POINTER(GemmArgs)]),
+    "b200sd_gemm_s8_linear": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p, C.c_void_p]),
+    "b200sd_gemm_plan_ex_s8_linear": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(C.c_int32)]),
+    "b200sd_gemm_describe_plan_s8_linear": (C.c_int, [C.POINTER(GemmArgs), C.c_char_p, C.c_size_t]),
+    "b200sd_gemm_workspace_bytes_s8_linear": (C.c_size_t, [C.POINTER(GemmArgs)]),
+    "b200sd_layer_norm_s8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32, C.c_int32,
+                                       C.c_float, C.c_void_p]),
     "b200sd_group_norm_s8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_float, C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p,
                                        C.c_size_t, C.c_void_p]),
@@ -271,11 +278,11 @@ def gemm_args(mode, a0, wgt, out, *, a1=None, bias=None, residual=None, m=0, n=0
 def describe_plan(mode, m=0, n=0, c0=0, c1=0, n_img=0, h=0, w=0, stride=1, geglu=False, has_bias=True,
                   has_residual=False, bias_rows=0, split_k=0, block_n=0, out_f32=False, act=0, pad_after_only=False,
                   rowstats=False, stats=False, cs_hw=0, ln=False, c2=0, c3=0, halo=0, upsample=False, gn=False,
-                  bf16=False) -> str:
+                  bf16=False, out_s8=False) -> str:
     """Host-only: the tiling the launcher would choose (no GPU needed).  The flags mirror linear() / conv3x3():
     rowstats / stats (with cs_hw, the rows per image of a linear) ask for the statistics outputs, ln for the LayerNorm
     fold, c2 / c3 are the folded shortcut's channels, halo / upsample / gn select the halo convolution (mode 0 with halo:
-    its 1x1 form; m = n_img * h * w); bf16 plans the bf16 call (b200sd_gemm_bf16)."""
+    its 1x1 form; m = n_img * h * w); bf16 plans the bf16 call (b200sd_gemm_bf16); out_s8 an int8 output."""
     a = GemmArgs()
     a.mode, a.m, a.n, a.c0, a.c1, a.n_img, a.h, a.w, a.stride = mode, m, n, c0, c1, n_img, h, w, stride
     a.geglu, a.bias_rows, a.split_k, a.block_n = int(geglu), bias_rows, split_k, block_n
@@ -291,6 +298,7 @@ def describe_plan(mode, m=0, n=0, c0=0, c1=0, n_img=0, h=0, w=0, stride=1, geglu
         a.ln_stat, a.ln_wg, a.ln_parts = 1, 1, 1
     a.c2, a.c3 = c2, c3
     a.halo, a.upsample2x, a.gn_groups = int(halo), int(upsample), 32 if gn else 0
+    a.out_s8_inv_scale = 1.0 if out_s8 else 0.0
     if stats or rowstats or ln or gn:
         a.split_k = 1  # as linear() / conv3x3() ask for the fused outputs
     buf = C.create_string_buffer(512)
@@ -510,12 +518,13 @@ def _fused_args(args, x_dev, *, n_img, cout, gn=None, stats=None, cs_hw=0, ln=No
 
 def linear(x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=None, split_k=0,
            block_n=0, bias_rows=0, bias_stride=0, out=None, static_w=False, act=0, ln=None, stats=None, cs_hw=0,
-           rowstats=None):
+           rowstats=None, out_inv_scale=None):
     """out[M, N] = epilogue([x | x1] @ wgt^T).  x [M, C0] fp16, wgt [N, C0(+C1)] fp16, bias fp32 [N].
     x bf16 runs the bf16 kernels: then wgt, x1, residual and a 16-bit output are bf16 too (out_dtype None: x's type).
     static_w: `wgt` is a model weight (constant address/content) and may be re-tiled + cached.
     ln: LayerNorm of x folded into this GEMM (wgt = gamma (.) W, bias = W beta + b; dict(stat, parts, wg, eps));
-    stats / rowstats: dicts that receive the per-channel / per-row sums of the output (see _fused_args)."""
+    stats / rowstats: dicts that receive the per-channel / per-row sums of the output (see _fused_args).
+    out_inv_scale: int8 output q = clamp(rint(y * out_inv_scale), -127, 127) for a W8A8 consumer (fp16 x)."""
     dt = _act_dtype(x, "linear x")
     lut = _is_lut(wgt)
     if lut:
@@ -526,11 +535,18 @@ def linear(x, wgt, bias=None, residual=None, *, x1=None, geglu=False, out_dtype=
     _same16(dt, x1, residual, "linear x1 / residual")
     m, n = x.shape[0], wgt.shape[0]
     n_out = n // 2 if geglu else n
+    if out_inv_scale is not None:
+        out_dtype = torch.int8
     if out is None:
         out = torch.empty(m, n_out, dtype=out_dtype or dt, device=x.device)
-    _check_out(out, dt, "linear out")
+    if out_inv_scale is None:
+        _check_out(out, dt, "linear out")
+    else:
+        _req(out, torch.int8, "linear out (int8 output)")
     args = gemm_args(0, x, wgt.packed if lut else wgt, out, a1=x1, bias=bias, residual=residual, m=m, n=n, geglu=geglu,
                      bias_rows=bias_rows, bias_stride=bias_stride, split_k=split_k, block_n=block_n, act=act)
+    if out_inv_scale is not None:
+        args.out_s8_inv_scale = float(out_inv_scale)
     if ln is not None or stats is not None or rowstats is not None:
         args.split_k = 1
         _keep = _fused_args(args, x.device, n_img=(m // cs_hw if cs_hw else 0), cout=n, stats=stats, cs_hw=cs_hw, ln=ln,
@@ -644,17 +660,19 @@ def describe_plan_s8(n, c0, n_img, h, w, has_bias=True, has_residual=False, bias
     return buf.value.decode()
 
 
-def _tiled_s8(args, wgt):
-    """int8 [Cout, 9*C0] OHWI weights -> the pre-tiled layout of the planned width (cached per (weight, block_n))."""
-    bn = args.block_n if args.block_n > 0 else plan_ex_s8(args)[0]
-    key = (wgt.data_ptr(), bn, args.c0, "s8")
+def _tiled_s8(args, wgt, taps=9):
+    """int8 [Cout, taps*C0] (OHWI for the convolution) weights -> the pre-tiled layout of the planned width (cached per
+    (weight, block_n))."""
+    what = "conv3x3_s8" if taps == 9 else "linear_s8"
+    bn = args.block_n if args.block_n > 0 else (plan_ex_s8 if taps == 9 else plan_ex_s8_linear)(args)[0]
+    key = (wgt.data_ptr(), bn, args.c0, "s8") if taps == 9 else (wgt.data_ptr(), bn, args.c0, "s8_linear")
     hit = _tiled_cache.get(key)
     if hit is not None and hit[0]() is wgt and hit[1] == wgt._version:
         return hit[2], bn
     if torch.cuda.is_current_stream_capturing():
-        raise B200SDError("conv3x3_s8: weights of this shape were not tiled before CUDA-graph capture; run one eager "
+        raise B200SDError(f"{what}: weights of this shape were not tiled before CUDA-graph capture; run one eager "
                           "call with the same shapes first")
-    packed = pack_tiled(wgt, args.c0, 0, 9, bn, chunk=128)
+    packed = pack_tiled(wgt, args.c0, 0, taps, bn, chunk=128)
     _cache_tiled(key, wgt, packed)
     return packed, bn
 
@@ -688,6 +706,85 @@ def conv3x3_s8(x, wgt, col_scale, bias=None, residual=None, *, bias_rows=0, bias
         args.workspace = ws.data_ptr()
         args.workspace_bytes = ws.numel() * 4
     _check(load().b200sd_gemm_s8(C.byref(args), _ptr(col_scale), _stream()), "b200sd_gemm_s8")
+    return out
+
+
+def plan_ex_s8_linear(args):
+    """plan_ex of the int8 linear GEMM (k-blocks of 128 channels)."""
+    plan = (C.c_int32 * 8)()
+    _check(load().b200sd_gemm_plan_ex_s8_linear(C.byref(args), plan), "b200sd_gemm_plan_ex_s8_linear")
+    return tuple(int(v) for v in plan)
+
+
+def describe_plan_s8_linear(m, n, c0, geglu=False, has_bias=True, has_residual=False, rowstats=False, out_s8=False,
+                            split_k=0, block_n=0) -> str:
+    """Host-only: the tiling b200sd_gemm_s8_linear would choose (see describe_plan); out_s8: int8 output."""
+    a = GemmArgs()
+    a.mode, a.m, a.n, a.c0, a.geglu, a.split_k, a.block_n = 0, m, n, c0, int(geglu), split_k, block_n
+    a.bias = 1 if has_bias else None
+    a.residual = 1 if has_residual else None
+    if rowstats:
+        a.rs_out, a.split_k = 1, 1
+    if out_s8:
+        a.out_s8_inv_scale = 1.0
+    buf = C.create_string_buffer(512)
+    _check(load().b200sd_gemm_describe_plan_s8_linear(C.byref(a), buf, 512), "b200sd_gemm_describe_plan_s8_linear")
+    return buf.value.decode()
+
+
+def linear_s8(x, wgt, col_scale, bias=None, residual=None, *, geglu=False, rowstats=None, out_inv_scale=None,
+              split_k=0, block_n=0, out=None):
+    """W8A8 linear on int8 wgmma.  x int8 [M, C] (C a multiple of 16); wgt int8 [N, C] (symmetric per-output-channel
+    quantized; GEGLU: value / gate rows interleaved as for linear()); col_scale fp32 [N] = s_a * s_w; bias fp32 [N];
+    residual fp16 [M, N_out].  y = acc * col_scale + bias (-> GEGLU) + residual, stored fp16, or int8
+    clamp(rint(y * out_inv_scale), -127, 127) when out_inv_scale is given.  rowstats: dict that receives the per-row
+    sums of the fp16 output for a LayerNorm folded into the consumer (see _fused_args)."""
+    _req(x, torch.int8, "linear_s8 x")
+    _req(wgt, torch.int8, "linear_s8 wgt")
+    _req(col_scale, torch.float32, "linear_s8 col_scale")
+    if residual is not None:
+        _req(residual, torch.float16, "linear_s8 residual")
+    m, c = x.shape
+    n = wgt.shape[0]
+    if wgt.shape[1] != c or col_scale.numel() != n:
+        raise B200SDError(f"linear_s8: weight {tuple(wgt.shape)} / col_scale {col_scale.numel()} do not match {c} input "
+                          f"and {n} output channels")
+    out_dtype = torch.int8 if out_inv_scale is not None else torch.float16
+    if out is None:
+        out = torch.empty(m, n // 2 if geglu else n, dtype=out_dtype, device=x.device)
+    _req(out, out_dtype, "linear_s8 out")
+    args = gemm_args(0, x, wgt, out, bias=bias, residual=residual, m=m, n=n, geglu=geglu, split_k=split_k,
+                     block_n=block_n)
+    if out_inv_scale is not None:
+        args.out_s8_inv_scale = float(out_inv_scale)
+    _keep = None
+    if rowstats is not None:
+        args.rs_out, args.split_k = 1, 1
+        pl = plan_ex_s8_linear(args)
+        rows = torch.empty(2 * pl[3], m, 2, dtype=torch.float32, device=x.device)  # one partial per column half of a tile
+        args.rs_out = rows.data_ptr()
+        rowstats["rows"], rowstats["parts"] = rows, 2 * pl[3]
+        _keep = rows
+    packed, bn = _tiled_s8(args, wgt, taps=1)
+    args.wgt, args.block_n, args.wgt_tiled = packed.data_ptr(), bn, 1
+    need = int(load().b200sd_gemm_workspace_bytes_s8_linear(C.byref(args)))
+    if need:
+        ws = _workspace(need, x.device)
+        args.workspace = ws.data_ptr()
+        args.workspace_bytes = ws.numel() * 4
+    _check(load().b200sd_gemm_s8_linear(C.byref(args), _ptr(col_scale), _stream()), "b200sd_gemm_s8_linear")
+    return out
+
+
+def layer_norm_s8(x, gamma, beta, inv_scale, eps=1e-5, out=None):
+    """layer_norm (fp16 [rows, c]) whose output is int8: q = clamp(rint(y * inv_scale), -127, 127) of the fp32 y."""
+    _req(x, torch.float16, "layer_norm_s8 x")
+    rows, c = x.shape
+    if out is None:
+        out = torch.empty(rows, c, dtype=torch.int8, device=x.device)
+    _req(out, torch.int8, "layer_norm_s8 out")
+    _check(load().b200sd_layer_norm_s8(_ptr(x), _ptr(gamma), _ptr(beta), float(inv_scale), _ptr(out), rows, c, float(eps),
+                                       _stream()), "b200sd_layer_norm_s8")
     return out
 
 

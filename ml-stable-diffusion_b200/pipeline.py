@@ -755,17 +755,18 @@ class B200StableDiffusionPipeline:
                 callback(i, st.timestep, x_space(i + 1))
         return self._denoised if return_denoised else self._latents
 
-    def calibrate_unet(self, prompts, num_inference_steps=50, guidance_scale=7.5, seed=0):
+    def calibrate_unet(self, prompts, num_inference_steps=50, guidance_scale=7.5, seed=0, linear=False):
         """W8A8 calibration: runs the denoising loop eagerly with the fp16 UNet once per prompt (seed, seed + 1, ...)
         and records max |x| at the input of every convolution the engine can quantize, over every UNet call (all
-        steps, both classifier-free-guidance halves).  Returns the ``quantization.W8A8Recipe`` with s_a = amax / 127 for
-        all of them; ``from_pretrained(..., unet_quantization=recipe)`` (or ``recipe.save(path)``) applies it."""
-        from .quantization import W8A8Recipe
+        steps, both classifier-free-guidance halves).  linear: the transformer linears too (the recipe's linear
+        section).  Returns the ``quantization.W8A8Recipe`` with s_a = amax / 127 for all of them;
+        ``from_pretrained(..., unet_quantization=recipe)`` (or ``recipe.save(path)``) applies it."""
+        from .quantization import W8A8Recipe, quantizable_linear_layers
         if isinstance(prompts, str):
             prompts = [prompts]
         u = self.unet
         eng = u.engine
-        slots = eng.set_calibration(True)
+        slots = eng.set_calibration(True, linear=linear)
         graphed, u.use_cuda_graph = u.use_cuda_graph, False  # the probes must not enter a captured graph
         try:
             for i, p in enumerate(prompts):
@@ -776,7 +777,10 @@ class B200StableDiffusionPipeline:
         finally:
             u.use_cuda_graph = graphed
             eng.set_calibration(False)
-        return W8A8Recipe.from_amax({n: float(t.item()) for n, t in slots.items()}, eng.cfg)
+        amax = {n: float(t.item()) for n, t in slots.items()}
+        lin = quantizable_linear_layers(eng.cfg)
+        return W8A8Recipe.from_amax({n: v for n, v in amax.items() if n not in lin}, eng.cfg,
+                                    {n: v for n, v in amax.items() if n in lin})
 
     def decode_latents(self, latents, want_u8=False):
         """pipeline.py:313-320 on the device: z / scaling -> decoder -> clip(x/2+0.5, 0, 1) -> NHWC fp32 (and, with

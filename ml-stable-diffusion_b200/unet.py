@@ -47,6 +47,12 @@ def _as_list(v, n):
     return list(v) if isinstance(v, (list, tuple)) else [v] * n
 
 
+def _int8_out(inv_scale):
+    """lib.linear's int8-output argument, given only when the consumer runs in W8A8: a launch whose consumer is fp16 is
+    called exactly as without a recipe."""
+    return {} if inv_scale is None else {"out_inv_scale": inv_scale}
+
+
 def _w2d(sd, key):
     w = sd[key]
     return w.reshape(w.shape[0], -1) if w.dim() == 4 and w.shape[2] == 1 else w
@@ -87,7 +93,8 @@ class UNetEngine:
 
     def __init__(self, cfg: dict, state_dict: dict, device="cuda", quantization=None, palettization=None):
         """quantization: a W8A8Recipe (or the path of a saved one): the ResNet / up-sampler convolutions it names run
-        on the int8 convolution kernel with its activation scales; every other layer is unchanged.
+        on the int8 convolution kernel with its activation scales, the transformer linears of its linear section on the
+        int8 linear GEMM (their producers write the int8 operand); every other layer is unchanged.
         palettization: n-bit palettized weights (palettization.as_recipe: an nbits int, a {layer: nbits} dict or
         (json path, recipe key)).  The layers run per step keep only packed indices and palettes on the device and
         decode them in the GEMM kernel; the once-per-call layers (time / add embeddings, time_emb_proj, cross-attention
@@ -332,7 +339,41 @@ class UNetEngine:
             else:
                 for k in (("c1",) if conv == "conv1" else ("c2", "c2sc")):
                     w[block].pop(k, None)
+        self._pack_linear_s8(sd, w)
         self.weight_bytes = sum(t.numel() * t.element_size() for t in self._tensors())
+
+    def _pack_linear_s8(self, sd, w):
+        """W8A8 transformer linears: int8 [N, K] weights (GEGLU rows interleaved like the fp16 launch), col_scale =
+        s_a * s_w, 1 / s_a for the producer of the int8 operand.  The fp16 copies (and LayerNorm folds) of a quantized
+        launch are never launched and are dropped; its bias stays."""
+        lin = self.recipe.linear_scales if self.recipe is not None else {}
+        if not lin:
+            return
+
+        def qpack(names, geglu=False):
+            qw, s_w = Q.quantize_weight(torch.cat([_w2d(sd, n + ".weight").float() for n in names], 0))
+            if geglu:  # (value_i, gate_i) row pairs, as the fp16 GEGLU launch
+                h = qw.shape[0] // 2
+                qw = torch.stack([qw[:h], qw[h:]], 1).reshape(qw.shape)
+                s_w = torch.stack([s_w[:h], s_w[h:]], 1).reshape(-1)
+            s_a = lin[names[0]]
+            return {"w": qw.to(self.dev).contiguous(), "cs": (s_w * s_a).to(self.dev).contiguous(), "inv": 1.0 / s_a}
+
+        for p, t in w.items():
+            if "blocks" not in t:
+                continue
+            for key, layer in (("pi", ".proj_in"), ("po", ".proj_out")):
+                if p + layer in lin:
+                    t["q_" + key] = qpack([p + layer])
+                    del t[key]
+            for d, blk in enumerate(t["blocks"]):
+                b = f"{p}.transformer_blocks.{d}"
+                for key, names in (("qkv", [f"{b}.attn1.to_{n}" for n in "qkv"]), ("q2", [f"{b}.attn2.to_q"]),
+                                   ("gg", [f"{b}.ff.net.0.proj"]), ("f2", [f"{b}.ff.net.2"])):
+                    if names[0] in lin:
+                        blk["q_" + key] = qpack(names, geglu=key == "gg")
+                        for k in (key, key + "_ln", key + "_wg", key + "_lnb"):
+                            blk.pop(k, None)
 
     def stored_bits(self):
         """layer -> (nominal bits of the recipe, bits per weight the engine stores: the container width of its launch,
@@ -369,10 +410,12 @@ class UNetEngine:
         yield from walk(getattr(self, "q", {}))
 
     # ------------------------------------------------------------------ W8A8 calibration
-    def set_calibration(self, on: bool):
+    def set_calibration(self, on: bool, linear: bool = False):
         """Calibration mode: every forward folds max |x| at the input of every quantizable layer into a device slot
-        (deterministic).  Returns the slots (layer -> fp32 [1] tensor) when switched on; they accumulate until the
-        mode is switched on again."""
+        (deterministic).  linear: the transformer linears too (quantizable_linear_layers; attn1 to_q / to_k / to_v share
+        one slot, their one input; the LayerNorm outputs, folded into their GEMMs otherwise, are computed for the probe).
+        Returns the slots (layer -> fp32 [1] tensor) when switched on; they accumulate until the mode is switched on
+        again."""
         if not on:
             self.calib = None
             return None
@@ -381,11 +424,21 @@ class UNetEngine:
         self._require_default_level("W8A8 calibration")
         layers = [n for n, c in Q.quantizable_layers(self.cfg).items() if c % 16 == 0]
         self.calib = {n: torch.zeros(1, dtype=torch.float32, device=self.dev) for n in layers}
+        for n, c in (Q.quantizable_linear_layers(self.cfg).items() if linear else ()):
+            if c % 16 == 0:
+                shared = n.endswith((".attn1.to_k", ".attn1.to_v"))
+                self.calib[n] = (self.calib[n.rsplit(".", 1)[0] + ".to_q"] if shared
+                                 else torch.zeros(1, dtype=torch.float32, device=self.dev))
         return self.calib
 
     def _probe(self, name, x):
         if self.calib is not None and name in self.calib:
             L.absmax(x, self.calib[name])
+
+    def _probe_ln(self, name, tok, gamma, beta):
+        """Calibration probe of a LayerNorm output that the fp16 path folds into its consumer GEMM."""
+        if self.calib is not None and name in self.calib:
+            L.absmax(L.layer_norm(tok, gamma, beta), self.calib[name])
 
     # ------------------------------------------------------------------ blocks
     def _resnet(self, p, x, x1, temb_all):
@@ -487,32 +540,73 @@ class UNetEngine:
         n, h, wd, c = x.shape
         m, s = n * h * wd, h * wd
         impl = _IMPL_CODE[ATTENTION_IMPLEMENTATION_IN_EFFECT]
+        blocks = t["blocks"]
+
+        def folded(bi, name):
+            """The consumer `name` of block bi is the fp16 GEMM with its LayerNorm folded in: its producer leaves the
+            row statistics behind.  (A W8A8 consumer normalises its input itself, in b200sd_layer_norm_s8.)"""
+            return bi < len(blocks) and ("q_" + name) not in blocks[bi]
+
         rs = {}
+        qpi, qpo = t.get("q_pi"), t.get("q_po")
         if self.fuse_gn and xs is not None and self._use_halo(x):
             gn = dict(chan0=xs, chan1=None, gamma=t["ng"], beta=t["nb"], groups=32, eps=1e-6, silu=False)
             tok = L.conv3x3(x, t["pi"], t["pib"], halo=True, taps=1, gn=gn, rowstats=rs).reshape(m, c)
+        elif qpi is not None:  # W8A8: GroupNorm straight to int8, int8 GEMM
+            hq = L.group_norm_s8(x, t["ng"], t["nb"], 32, 1e-6, qpi["inv"], silu=False)
+            tok = L.linear_s8(hq.reshape(m, c), qpi["w"], qpi["cs"], t["pib"], rowstats=rs if folded(0, "qkv") else None)
         else:
             hn = (L.group_norm_apply(x, xs, t["ng"], t["nb"], 32, 1e-6) if (self.fuse_gn and xs is not None)
                   else L.group_norm(x, t["ng"], t["nb"], 32, 1e-6, silu=False))
-            tok = L.linear(hn.reshape(m, c), t["pi"], t["pib"], static_w=True, rowstats=rs)
+            self._probe(p + ".proj_in", hn)
+            tok = L.linear(hn.reshape(m, c), t["pi"], t["pib"], static_w=True, rowstats=rs if folded(0, "qkv") else None)
 
         def ln_of(rs, blk, name):
             return dict(stat=rs["rows"], parts=rs["parts"], wg=blk[name + "_wg"], eps=1e-5)
 
-        nblk = len(t["blocks"])
-        for bi, blk in enumerate(t["blocks"]):
-            qkv = L.linear(tok, blk["qkv_ln"], blk["qkv_lnb"], ln=ln_of(rs, blk, "qkv"), static_w=True)
+        nblk = len(blocks)
+        for bi, blk in enumerate(blocks):
+            b = f"{p}.transformer_blocks.{bi}"
+            q8 = blk.get("q_qkv")
+            if q8 is not None:
+                qkv = L.linear_s8(L.layer_norm_s8(tok, blk["ln1g"], blk["ln1b"], q8["inv"]), q8["w"], q8["cs"])
+            else:
+                self._probe_ln(b + ".attn1.to_q", tok, blk["ln1g"], blk["ln1b"])
+                qkv = L.linear(tok, blk["qkv_ln"], blk["qkv_lnb"], ln=ln_of(rs, blk, "qkv"), static_w=True)
             a = L.attention(qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:], batch, heads, s, s, d=c // heads, impl=impl)
             rs = {}
-            tok = L.linear(a, blk["o1"], blk["o1b"], tok, static_w=True, rowstats=rs)
-            q = L.linear(tok, blk["q2_ln"], blk["q2_lnb"], ln=ln_of(rs, blk, "q2"), static_w=True)
+            tok = L.linear(a, blk["o1"], blk["o1b"], tok, static_w=True, rowstats=rs if folded(bi, "q2") else None)
+            q8 = blk.get("q_q2")
+            if q8 is not None:
+                q = L.linear_s8(L.layer_norm_s8(tok, blk["ln2g"], blk["ln2b"], q8["inv"]), q8["w"], q8["cs"])
+            else:
+                self._probe_ln(b + ".attn2.to_q", tok, blk["ln2g"], blk["ln2b"])
+                q = L.linear(tok, blk["q2_ln"], blk["q2_lnb"], ln=ln_of(rs, blk, "q2"), static_w=True)
             ko = blk["kv_off"]
             a = L.attention(q, kv_all[:, ko:ko + c], kv_all[:, ko + c:ko + 2 * c], batch, heads, s, s_ctx, d=c // heads, impl=impl)
             rs = {}
-            tok = L.linear(a, blk["o2"], blk["o2b"], tok, static_w=True, rowstats=rs)
-            g = L.linear(tok, blk["gg_ln"], blk["gg_lnb"], geglu=True, ln=ln_of(rs, blk, "gg"), static_w=True)
+            tok = L.linear(a, blk["o2"], blk["o2b"], tok, static_w=True, rowstats=rs if folded(bi, "gg") else None)
+            qg, qf = blk.get("q_gg"), blk.get("q_f2")
+            g_inv = None if qf is None else qf["inv"]  # a W8A8 ff.net.2 reads the GEGLU output in int8
+            if qg is not None:
+                g = L.linear_s8(L.layer_norm_s8(tok, blk["ln3g"], blk["ln3b"], qg["inv"]), qg["w"], qg["cs"], blk["ggb"],
+                                geglu=True, out_inv_scale=g_inv)
+            else:
+                self._probe_ln(b + ".ff.net.0.proj", tok, blk["ln3g"], blk["ln3b"])
+                g = L.linear(tok, blk["gg_ln"], blk["gg_lnb"], geglu=True, ln=ln_of(rs, blk, "gg"), static_w=True,
+                             **_int8_out(g_inv))
             rs = {}
-            tok = L.linear(g, blk["f2"], blk["f2b"], tok, static_w=True, rowstats=rs if bi + 1 < nblk else None)
+            last = bi + 1 == nblk
+            f_rs = rs if (not last and folded(bi + 1, "qkv")) else None
+            f_inv = qpo["inv"] if (last and qpo is not None) else None  # a W8A8 proj_out reads the last output in int8
+            if qf is not None:
+                tok = L.linear_s8(g, qf["w"], qf["cs"], blk["f2b"], tok, rowstats=f_rs, out_inv_scale=f_inv)
+            else:
+                self._probe(b + ".ff.net.2", g)
+                tok = L.linear(g, blk["f2"], blk["f2b"], tok, static_w=True, rowstats=f_rs, **_int8_out(f_inv))
+        if qpo is not None:  # no column statistics: the next GroupNorm takes its standalone two-pass path
+            return L.linear_s8(tok, qpo["w"], qpo["cs"], t["pob"], x.reshape(m, c)).reshape(n, h, wd, c), None
+        self._probe(p + ".proj_out", tok)
         st = {}
         ok = self.fuse_gn and (s % 128 == 0 or (s >= 16 and 128 % s == 0))   # geometries whose tiles map onto whole images
         out = L.linear(tok, t["po"], t["pob"], x.reshape(m, c), static_w=True, stats=st if ok else None, cs_hw=s)

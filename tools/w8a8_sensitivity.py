@@ -3,6 +3,9 @@ the engine can quantize, quantize that layer alone, run the denoising loop to th
 the mean PSNR against the fp16 UNet's latents (the formula of oracle.restated.compute_psnr).  Writes the reference's
 JSON format, {"conv": {layer: psnr}, "einsum": {}, "model_version": ...}, which quantization.select_from_sensitivity
 reads with a conv_psnr threshold.  Prompts come from the user.  SD 1.x / 2.x pipelines (one text encoder).
+--linear: the transformer linears too, under the reference's names in the same "conv" section (its UNet runs them as 1x1
+convolutions); an attn1 to_q / to_k / to_v triple is one launch here, so its three entries get the PSNR of quantizing the
+triple.
 
     python tools/w8a8_sensitivity.py --model-dir DIR --prompt "..." --prompt "..." --steps 20 --out sens.json
     python tools/w8a8_sensitivity.py --random-init sd21-base --prompt "..." --out sens.json   (random weights)
@@ -29,6 +32,7 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--recipe", help="calibrated W8A8Recipe JSON (default: calibrate on the prompts)")
     ap.add_argument("--layers", nargs="*", help="restrict to these layers")
+    ap.add_argument("--linear", action="store_true", help="also the transformer linears (select_from_sensitivity(linear=True))")
     ap.add_argument("--out", required=True)
     args = ap.parse_args()
     from b200sd import checkpoint as K
@@ -50,7 +54,8 @@ def main():
     if pipe.xl:
         raise SystemExit("w8a8_sensitivity: SD 1.x / 2.x pipelines only")
     recipe = W8A8Recipe.load(args.recipe) if args.recipe else pipe.calibrate_unet(
-        args.prompt, num_inference_steps=args.steps, guidance_scale=args.guidance_scale, seed=args.seed)
+        args.prompt, num_inference_steps=args.steps, guidance_scale=args.guidance_scale, seed=args.seed,
+        linear=args.linear)
     u16 = pipe.unet
     rs = np.random.RandomState(args.seed)
     lat = torch.from_numpy(rs.randn(1, 4, u16.h, u16.w).astype(np.float32))
@@ -63,10 +68,20 @@ def main():
 
     ref = final_latents(u16)
     results = {}
-    for layer in (args.layers or list(recipe.scales)):
-        uq = UNetModel(cfg, sd, batch=u16.batch, height=u16.h, width=u16.w, quantization=recipe.subset([layer]))
+    layers = args.layers or (list(recipe.scales) + (list(recipe.linear_scales) if args.linear else []))
+    for layer in layers:
+        if layer in results:
+            continue
+        if layer in recipe.linear_scales:
+            block = layer.rsplit(".", 1)[0]
+            group = [f"{block}.to_{n}" for n in "qkv"] if block.endswith(".attn1") else [layer]
+            sub = recipe.subset([], group)
+        else:
+            group, sub = [layer], recipe.subset([layer])
+        uq = UNetModel(cfg, sd, batch=u16.batch, height=u16.h, width=u16.w, quantization=sub)
         outs = final_latents(uq)
-        results[layer] = float(np.mean([compute_psnr(r, o) for r, o in zip(ref, outs)]))
+        for n in group:
+            results[n] = float(np.mean([compute_psnr(r, o) for r, o in zip(ref, outs)]))
         print(f"{layer}: {results[layer]:.2f} dB", flush=True)
         del uq
         torch.cuda.empty_cache()
