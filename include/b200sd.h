@@ -344,7 +344,8 @@ typedef struct {
     int32_t push_x0_slot;    /* >= 0: hist[slot] = x0    */
     int32_t push_x_slot;     /* >= 0: hist[slot] = x (sample before this update) */
     int32_t noise_pred_nhwc; /* 1: noise_pred is NHWC fp32 [2*n, h, w, c] (the UNet's conv_out epilogue output, no
-                                layout kernel in between); 0: NCHW */
+                                layout kernel in between); 0: NCHW.  b200sd_scheduler_step_guidance_free reads one
+                                prediction per image: NHWC fp32 [n, h, w, c], or NCHW [n, c, h, w] */
 } b200sd_step_coeffs;
 
 int b200sd_cfg_scheduler_step(const float* noise_pred, float* latents, float* hist /* [4][numel] */,
@@ -390,6 +391,19 @@ int b200sd_cfg_scheduler_step_blend(const float* noise_pred, float* latents, flo
                                     const b200sd_step_coeffs* coeffs /* host */, float noise_scale,
                                     const uint32_t* philox_key /* device or NULL */, uint32_t philox_offset,
                                     const b200sd_blend_args* blend /* host */, void* stream);
+
+/* The step without classifier-free guidance (diffusers runs guidance_scale <= 1 and guidance-embedding UNets at batch
+ * n): eps' = noise_pred, one prediction per image, fp32 [n, c, h, w] (NCHW) or [n, h, w, c] (noise_pred_nhwc); no
+ * uncond half and no `numel +` offset, coeffs->guidance unused.  `unet_in` (fp16 NHWC, may be NULL) receives the next
+ * UNet input in its first n rows only, [n, h, w, c_pad].  History, `denoised`, the ancestral noise (philox_key != NULL,
+ * as in b200sd_cfg_scheduler_step_noised) and the inpainting blend (blend != NULL, as in
+ * b200sd_cfg_scheduler_step_blend) are those of the guided steps. */
+int b200sd_scheduler_step_guidance_free(const float* noise_pred, float* latents, float* hist /* [4][numel] */,
+                                        float* denoised /* x0 out or NULL */, void* unet_in, int32_t c_pad,
+                                        int32_t n, int32_t c, int32_t h, int32_t w,
+                                        const b200sd_step_coeffs* coeffs /* host */, float noise_scale,
+                                        const uint32_t* philox_key /* device or NULL */, uint32_t philox_offset,
+                                        const b200sd_blend_args* blend /* host or NULL */, void* stream);
 
 /* VAE decoder input: out = post_quant_conv(z * inv_scale) as NHWC fp16 padded to c_pad channels
  * (pipeline.py:313-316 `z / 0.18215`; torch2coreml.py:590-594 post_quant_conv); z fp32 NCHW, c <= 8,

@@ -37,6 +37,9 @@ def _as_list(v, n):
 
 def make_config(cfg: dict, batch: int, height: int, width: int, seq_len: int = 77) -> UNetConfig:
     """The reference's UNet config keys (unet.py:733-800) -> ``b200sd_unet_config``."""
+    if cfg.get("time_cond_proj_dim"):
+        raise ValueError(f"the C handle takes no time condition: a UNet with time_cond_proj_dim="
+                         f"{cfg['time_cond_proj_dim']} (guidance embedding) runs through UNetModel only")
     boc = list(cfg["block_out_channels"])
     nb = len(boc)
     c = UNetConfig()

@@ -217,6 +217,8 @@ def unet_param_shapes(cfg) -> "OrderedDict[str, tuple]":
     _conv(sh, "conv_in", boc[0], cfg["in_channels"], 3)
     _conv(sh, "time_embedding.linear_1", temb, boc[0], 1)
     _conv(sh, "time_embedding.linear_2", temb, temb, 1)
+    if cfg.get("time_cond_proj_dim"):  # guidance-embedding (LCM) UNets: TimestepEmbedding(cond_proj_dim=...)
+        _conv(sh, "time_embedding.cond_proj", boc[0], cfg["time_cond_proj_dim"], 1, bias=False)
     if cfg.get("addition_embed_type") == "text_time":
         _conv(sh, "add_embedding.linear_1", temb, cfg["projection_class_embeddings_input_dim"], 1)
         _conv(sh, "add_embedding.linear_2", temb, temb, 1)

@@ -147,14 +147,15 @@ class ControlNetModel(B200Model):
         self._table = None   # time-embedding biases of all steps (device loop prologue)
 
     # -- per-prompt prologue + per-step core of the device loop (pipeline.denoise) ------------------------------
-    def prepare_prompt(self, ts_rows):
+    def prepare_prompt(self, ts_rows, rows=None):
         """Everything that does not change over a denoising loop: cross-attention K/V from `_ctx`, the embedding of
         the conditioning image `_cond` (the reference recomputes it every step, pipeline.py:516-522), the
-        time-embedding biases of all steps."""
-        e, b = self.engine, self.batch
+        time-embedding biases of all steps.  ``rows``: the first ``rows`` images only (the guidance-free loop);
+        ``ts_rows`` then holds ``rows`` entries per step."""
+        e, b = self.engine, rows or self.batch
         if self._kv_all is not None:
-            e.kv_project(L.ctx_to_tokens(self._ctx), out=self._kv_all)
-        self._emb = e.embed_condition(L.nchw_to_nhwc(self._cond, c_pad=8))
+            e.kv_project(L.ctx_to_tokens(self._ctx[:b]), out=self._kv_all[:b * self.seq])
+        self._emb = e.embed_condition(L.nchw_to_nhwc(self._cond[:b], c_pad=8))
         n_steps = ts_rows.shape[0] // b
         per = max(1, 32 // b)
         parts = [e.time_embedding(ts_rows[s0 * b:(s0 + min(per, n_steps - s0)) * b].contiguous())
@@ -163,19 +164,25 @@ class ControlNetModel(B200Model):
 
     def run_core(self, x_nhwc, step):
         """Residuals (NHWC fp16) for the UNet input `x_nhwc` at loop step `step` (after prepare_prompt)."""
-        return self.engine.forward(x_nhwc, None, None, self.seq, None, temb_all=self._table[step], kv_all=self._kv_all,
+        rows = x_nhwc.shape[0]
+        kv = self._kv_all[:rows * self.seq] if self._kv_all is not None else None
+        return self.engine.forward(x_nhwc, None, None, self.seq, None, temb_all=self._table[step], kv_all=kv,
                                    emb=self._emb)
 
-    def _run(self):
+    def _run(self, rows=None):
         e = self.engine
-        x = L.nchw_to_nhwc(self._sample, c_pad=e.in_pad)
-        ctx = L.ctx_to_tokens(self._ctx)
-        cond = L.nchw_to_nhwc(self._cond, c_pad=8)
-        return e.forward(x, self._t, ctx, self.seq, cond)
+        r = rows or self.batch
+        x = L.nchw_to_nhwc(self._sample[:r], c_pad=e.in_pad)
+        ctx = L.ctx_to_tokens(self._ctx[:r])
+        cond = L.nchw_to_nhwc(self._cond[:r], c_pad=8)
+        return e.forward(x, self._t[:r], ctx, self.seq, cond)
 
-    def forward_device(self):
+    def forward_device(self, rows=None):
         """Static input buffers -> list of NHWC fp16 residuals.  With CUDA graphs the list is a set of static
-        tensors owned by the captured graph (overwritten by the next call)."""
+        tensors owned by the captured graph (overwritten by the next call).  ``rows`` < batch (the step-by-step
+        guidance-free loop): the first ``rows`` images, eagerly."""
+        if rows is not None and rows != self.batch:
+            return self._run(rows)
         if not self.use_cuda_graph:
             return self._run()
         if self._graph is None:

@@ -288,27 +288,34 @@ __device__ __forceinline__ float philox_normal(uint32_t key, uint32_t offset, ui
 // instantiation never reads noise_scale / philox_key / philox_offset.  kBlend (inpainting): after the update and the
 // noise, x_prev = m x_prev + (1 - m)(a x0_img + b z); history pushes and `denoised` keep their pre-blend values.  The
 // kBlend = false instantiations never read `blend` (appended last, so the other parameters keep their offsets).
-template <bool kNoise, bool kBlend>
-__global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __restrict__ latents,
-                                float* __restrict__ hist, float* __restrict__ denoised, __half* __restrict__ unet_in,
-                                int c_pad, int n, int c, int hw, b200sd_step_coeffs k, float noise_scale,
-                                const uint32_t* __restrict__ philox_key, uint32_t philox_offset,
-                                b200sd_blend_args blend) {
-    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
-    pdl_wait();
+// kGuided = false (guidance-free): noise_pred holds one prediction per image, [n, ...], used as eps' directly (no
+// k.guidance), and only the first n rows of unet_in are written.  The body is shared by two kernel templates so the
+// guided kernels keep their names and their code.
+template <bool kNoise, bool kBlend, bool kGuided>
+__device__ __forceinline__ void step_body(const float* __restrict__ noise_pred, float* __restrict__ latents,
+                                          float* __restrict__ hist, float* __restrict__ denoised,
+                                          __half* __restrict__ unet_in, int c_pad, int n, int c, int hw,
+                                          const b200sd_step_coeffs& k, float noise_scale,
+                                          const uint32_t* __restrict__ philox_key, uint32_t philox_offset,
+                                          const b200sd_blend_args& blend) {
     const int numel = n * c * hw;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= numel) return;
     int ni = i;  // index of this element inside one CFG half of noise_pred
-    if (k.noise_pred_nhwc) {  // the UNet's conv_out output as it leaves the epilogue: [2n, h*w, c]
+    if (k.noise_pred_nhwc) {  // the UNet's conv_out output as it leaves the epilogue: [2n | n, h*w, c]
         const int p = i % hw;
         const int ch = (i / hw) % c;
         const int b = i / (hw * c);
         ni = (b * hw + p) * c + ch;
     }
-    const float eu = noise_pred[ni];
-    const float ec = noise_pred[numel + ni];
-    const float eps = eu + k.guidance * (ec - eu);
+    float eps;
+    if constexpr (kGuided) {
+        const float eu = noise_pred[ni];
+        const float ec = noise_pred[numel + ni];
+        eps = eu + k.guidance * (ec - eu);
+    } else {
+        eps = noise_pred[ni];
+    }
     const float x = latents[i];
     float xp = k.cx * x + k.ce * eps;
     float x0 = k.x0_cx * x + k.x0_ce * eps;
@@ -339,8 +346,33 @@ __global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __r
         const int b = i / (hw * c);
         const __half hv = __float2half_rn(xp);
         unet_in[(static_cast<size_t>(b) * hw + p) * c_pad + ch] = hv;
-        unet_in[(static_cast<size_t>(n + b) * hw + p) * c_pad + ch] = hv;
+        if constexpr (kGuided) unet_in[(static_cast<size_t>(n + b) * hw + p) * c_pad + ch] = hv;
     }
+}
+
+template <bool kNoise, bool kBlend>
+__global__ void cfg_step_kernel(const float* __restrict__ noise_pred, float* __restrict__ latents,
+                                float* __restrict__ hist, float* __restrict__ denoised, __half* __restrict__ unet_in,
+                                int c_pad, int n, int c, int hw, b200sd_step_coeffs k, float noise_scale,
+                                const uint32_t* __restrict__ philox_key, uint32_t philox_offset,
+                                b200sd_blend_args blend) {
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
+    pdl_wait();
+    step_body<kNoise, kBlend, true>(noise_pred, latents, hist, denoised, unet_in, c_pad, n, c, hw, k, noise_scale,
+                                    philox_key, philox_offset, blend);
+}
+
+template <bool kNoise, bool kBlend>
+__global__ void guidance_free_step_kernel(const float* __restrict__ noise_pred, float* __restrict__ latents,
+                                          float* __restrict__ hist, float* __restrict__ denoised,
+                                          __half* __restrict__ unet_in, int c_pad, int n, int c, int hw,
+                                          b200sd_step_coeffs k, float noise_scale,
+                                          const uint32_t* __restrict__ philox_key, uint32_t philox_offset,
+                                          b200sd_blend_args blend) {
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
+    pdl_wait();
+    step_body<kNoise, kBlend, false>(noise_pred, latents, hist, denoised, unet_in, c_pad, n, c, hw, k, noise_scale,
+                                     philox_key, philox_offset, blend);
 }
 
 // ---- image post-process: clip(x/2+0.5, 0, 1), NHWC(c_pad) -> NHWC(c) fp32 and/or u8 -------------
@@ -634,6 +666,35 @@ extern "C" int b200sd_cfg_scheduler_step_blend(const float* noise_pred, float* l
         B200SD_CHECK_CUDA(launch_kernel(cfg_step_kernel<false, true>, grid, dim3(256), 0, stream, noise_pred, latents,
                                         hist, denoised, reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w,
                                         *coeffs, 0.f, static_cast<const uint32_t*>(nullptr), 0u, *blend));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_scheduler_step_guidance_free(const float* noise_pred, float* latents, float* hist,
+                                                  float* denoised, void* unet_in, int32_t c_pad, int32_t n, int32_t c,
+                                                  int32_t h, int32_t w, const b200sd_step_coeffs* coeffs,
+                                                  float noise_scale, const uint32_t* philox_key,
+                                                  uint32_t philox_offset, const b200sd_blend_args* blend,
+                                                  void* stream_) {
+    if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(noise_pred && latents && coeffs, "b200sd_scheduler_step_guidance_free: null pointer");
+    B200SD_REQUIRE(!blend || (blend->mask && blend->image_latents && blend->noise),
+                   "b200sd_scheduler_step_guidance_free: null blend buffer");
+    B200SD_REQUIRE(coeffs->n_hist >= 0 && coeffs->n_hist <= 4 && (coeffs->n_hist == 0 || hist),
+                   "b200sd_scheduler_step_guidance_free: bad history arguments");
+    B200SD_REQUIRE(coeffs->push_eps_slot < 4 && coeffs->push_x0_slot < 4 && coeffs->push_x_slot < 4 &&
+                       (hist || (coeffs->push_eps_slot < 0 && coeffs->push_x0_slot < 0 && coeffs->push_x_slot < 0)),
+                   "b200sd_scheduler_step_guidance_free: bad history ring slot");
+    B200SD_REQUIRE(!unet_in || c_pad >= c, "b200sd_scheduler_step_guidance_free: c_pad < c");
+    const int numel = n * c * h * w;
+    auto* kern = philox_key ? (blend ? guidance_free_step_kernel<true, true> : guidance_free_step_kernel<true, false>)
+                            : (blend ? guidance_free_step_kernel<false, true> : guidance_free_step_kernel<false, false>);
+    B200SD_CHECK_CUDA(launch_kernel(kern, dim3((numel + 255) / 256), dim3(256), 0, stream, noise_pred, latents, hist,
+                                    denoised, reinterpret_cast<__half*>(unet_in), c_pad, n, c, h * w, *coeffs,
+                                    philox_key ? noise_scale : 0.f, philox_key, philox_key ? philox_offset : 0u,
+                                    blend ? *blend : b200sd_blend_args{}));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;

@@ -145,6 +145,10 @@ _SIGNATURES = {
                                                   C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                   C.POINTER(StepCoeffs), C.c_float, C.c_void_p, C.c_uint32,
                                                   C.POINTER(BlendArgs), C.c_void_p]),
+    "b200sd_scheduler_step_guidance_free": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                      C.POINTER(StepCoeffs), C.c_float, C.c_void_p, C.c_uint32,
+                                                      C.POINTER(BlendArgs), C.c_void_p]),
     "b200sd_image_postprocess":(C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     # safety checker (csrc/vision.cu)
@@ -1067,6 +1071,43 @@ def cfg_scheduler_step_blend(noise_pred, latents, coeffs: StepCoeffs, mask, imag
                                                   float(noise_scale), _ptr(key), int(offset) & 0xFFFFFFFF,
                                                   C.byref(args), _stream()),
            "b200sd_cfg_scheduler_step_blend")
+    return latents
+
+
+def scheduler_step_guidance_free(noise_pred, latents, coeffs: StepCoeffs, noise_scale=0.0, key=None, offset=0,
+                                 blend=None, hist=None, denoised=None, unet_in=None):
+    """The step without classifier-free guidance: ``noise_pred`` holds ONE prediction per image (fp32, the size of
+    ``latents``; NHWC when ``coeffs.noise_pred_nhwc``), ``unet_in`` receives the next UNet input in its first n rows.
+    ``key`` / ``offset``: the ancestral noise of ``cfg_scheduler_step_noised``; ``blend`` = (mask, image_latents,
+    noise, a, b): the inpainting blend of ``cfg_scheduler_step_blend``."""
+    what = "scheduler_step_guidance_free"
+    _req(noise_pred, torch.float32, f"{what} noise_pred")
+    _req(latents, torch.float32, f"{what} latents")
+    n, c, h, w = latents.shape
+    if noise_pred.numel() != latents.numel():
+        raise B200SDError(f"{what}: noise_pred has {noise_pred.numel()} elements, expected one prediction per image "
+                          f"({latents.numel()})")
+    if key is not None and not (key.is_cuda and key.numel() == 1 and key.element_size() == 4):
+        raise B200SDError(f"{what}: key must be a one-element 4-byte CUDA tensor")
+    args = None
+    if blend is not None:
+        mask, image_latents, noise, a, b = blend
+        _req(mask, torch.float32, f"{what} mask")
+        if mask.numel() != n * h * w:
+            raise B200SDError(f"{what}: mask has {mask.numel()} elements, expected {n * h * w}")
+        for name, t in (("image_latents", image_latents), ("noise", noise)):
+            _req(t, torch.float32, f"{what} {name}")
+            if tuple(t.shape) != (n, c, h, w):
+                raise B200SDError(f"{what}: {name} has shape {tuple(t.shape)}, expected {(n, c, h, w)}")
+        args = BlendArgs(_ptr(mask), _ptr(image_latents), _ptr(noise), float(a), float(b))
+    if unet_in is not None and unet_in.shape[0] < n:
+        raise B200SDError(f"{what}: unet_in has {unet_in.shape[0]} rows, expected at least {n}")
+    c_pad = 0 if unet_in is None else unet_in.shape[-1]
+    _check(load().b200sd_scheduler_step_guidance_free(_ptr(noise_pred), _ptr(latents), _ptr(hist), _ptr(denoised),
+                                                      _ptr(unet_in), c_pad, n, c, h, w, C.byref(coeffs),
+                                                      float(noise_scale), _ptr(key), int(offset) & 0xFFFFFFFF,
+                                                      None if args is None else C.byref(args), _stream()),
+           "b200sd_scheduler_step_guidance_free")
     return latents
 
 

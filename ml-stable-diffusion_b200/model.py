@@ -51,8 +51,12 @@ class B200Model:
 
 
 class UNetModel(B200Model):
-    """``unet(sample, timestep, encoder_hidden_states[, time_ids, text_embeds][, additional_residual_i])
-    -> {"noise_pred": fp32}`` (pipeline.py:531-536)."""
+    """``unet(sample, timestep, encoder_hidden_states[, time_ids, text_embeds][, timestep_cond][,
+    additional_residual_i]) -> {"noise_pred": fp32}`` (pipeline.py:531-536).  ``timestep_cond`` ([batch,
+    time_cond_proj_dim], the guidance embedding): guidance-embedding (LCM) UNets only.
+
+    The device-loop methods (``time_table``, ``prepare_prompt``, ``_run_core``, ``forward_device``) take ``rows``: run
+    on the first ``rows`` images of the static buffers only (the guidance-free loop runs batch // 2 of them)."""
 
     def __init__(self, cfg, state_dict, batch=2, height=64, width=64, seq_len=77, device="cuda",
                  use_cuda_graph=True, io_dtype=np.float16, quantization=None, palettization=None):
@@ -76,6 +80,8 @@ class UNetModel(B200Model):
             spec["time_ids"] = {"shape": (batch, nid), "dtype": dt}
             spec["text_embeds"] = {"shape": (batch, cfg["projection_class_embeddings_input_dim"]
                                              - nid * cfg["addition_time_embed_dim"]), "dtype": dt}
+        if e.time_cond_dim:
+            spec["timestep_cond"] = {"shape": (batch, e.time_cond_dim), "dtype": dt}
         self.res_shapes = []
         if e.support_controlnet:
             for i, shp in enumerate(self.residual_shapes()):
@@ -90,6 +96,8 @@ class UNetModel(B200Model):
         self._text_embeds = (torch.zeros(spec["text_embeds"]["shape"], dtype=torch.float32, device=dev)
                              if e.xl else None)
         self._res = [torch.zeros(s, dtype=torch.float16, device=dev) for s in self.res_shapes]
+        self._cond = (torch.zeros(batch, e.time_cond_dim, dtype=torch.float32, device=dev) if e.time_cond_dim
+                      else None)
         self._out = torch.zeros(batch, e.out_ch, height, width, dtype=torch.float32, device=dev)
         # device-resident loop (pipeline.denoise): the UNet input as the kernels read it (NHWC fp16, written by the
         # fused CFG + scheduler kernel), the per-prompt cross-attention K/V, the conv_out epilogue's NHWC output
@@ -116,42 +124,57 @@ class UNetModel(B200Model):
         return shapes
 
     # -- device-side sequence (captured) --------------------------------------------------------
-    def _run(self):
+    def _run(self, rows=None):
         e = self.engine
-        x = L.nchw_to_nhwc(self._sample, c_pad=e.in_pad)
-        ctx = L.ctx_to_tokens(self._ctx)
-        res = [L.nchw_to_nhwc(r) for r in self._res] if self._res else None
-        out = e.forward(x, self._t, ctx, self.seq, self._time_ids, self._text_embeds, res)
-        L.nhwc_to_nchw_f32(out, c=e.out_ch, out=self._out)
+        r = rows or self.batch
+        x = L.nchw_to_nhwc(self._sample[:r], c_pad=e.in_pad)
+        ctx = L.ctx_to_tokens(self._ctx[:r])
+        res = [L.nchw_to_nhwc(b[:r]) for b in self._res] if self._res else None
+        tid = self._time_ids[:r] if e.xl else None
+        te = self._text_embeds[:r] if e.xl else None
+        cond = self._cond[:r] if self._cond is not None else None
+        out = e.forward(x, self._t[:r], ctx, self.seq, tid, te, res, timestep_cond=cond)
+        L.nhwc_to_nchw_f32(out, c=e.out_ch, out=self._out[:r])
 
     # -- per-prompt prologue + per-step core of the device loop (pipeline.denoise) ------------------------------
-    def prepare_prompt(self):
+    def prepare_prompt(self, rows=None):
         """Cross-attention keys / values of every block from ``_ctx`` (constant over the denoising loop)."""
         if self._kv_all is not None:
-            self.engine.kv_project(L.ctx_to_tokens(self._ctx), out=self._kv_all)
+            r = rows or self.batch
+            self.engine.kv_project(L.ctx_to_tokens(self._ctx[:r]), out=self._kv_all[:r * self.seq])
 
-    def time_table(self, ts_rows):
-        """ts_rows: fp32 device tensor [n_steps * batch] (each step's timestep repeated per batch row) ->
-        [n_steps, batch, sum Cout] time-embedding biases of every ResNet block for ALL steps (unet.py:442,476-478
-        depend on t only): one small-M pass per 32 rows instead of three launches inside every step."""
-        e, b = self.engine, self.batch
+    def time_table(self, ts_rows, rows=None):
+        """ts_rows: fp32 device tensor [n_steps * rows] (each step's timestep repeated per batch row) ->
+        [n_steps, rows, sum Cout] time-embedding biases of every ResNet block for ALL steps (unet.py:442,476-478
+        depend on t only): one small-M pass per 32 rows instead of three launches inside every step.  A
+        guidance-embedding UNet reads the first ``rows`` rows of ``_cond``."""
+        e, b = self.engine, rows or self.batch
         n_steps = ts_rows.shape[0] // b
         per = max(1, 32 // b)
         parts = []
         for s0 in range(0, n_steps, per):
             k = min(per, n_steps - s0)
-            tid = self._time_ids.repeat(k, 1) if e.xl else None
-            te = self._text_embeds.repeat(k, 1) if e.xl else None
-            parts.append(e.time_embedding(ts_rows[s0 * b:(s0 + k) * b].contiguous(), tid, te))
+            tid = self._time_ids[:b].repeat(k, 1) if e.xl else None
+            te = self._text_embeds[:b].repeat(k, 1) if e.xl else None
+            cond = self._cond[:b].repeat(k, 1) if self._cond is not None else None
+            parts.append(e.time_embedding(ts_rows[s0 * b:(s0 + k) * b].contiguous(), tid, te, cond))
         return torch.cat(parts, 0).reshape(n_steps, b, -1)
 
-    def _run_core(self, temb, residuals=None):
-        """One UNet forward on ``_x_nhwc`` with precomputed time-embedding biases ``temb`` [batch, sum Cout] and the
+    def _run_core(self, temb, residuals=None, rows=None):
+        """One UNet forward on ``_x_nhwc`` with precomputed time-embedding biases ``temb`` [rows, sum Cout] and the
         prologue's K/V; the conv_out epilogue writes ``_out_nhwc``."""
-        self.engine.forward(self._x_nhwc, None, None, self.seq, additional_residuals=residuals, temb_all=temb,
-                            kv_all=self._kv_all, out=self._out_nhwc)
+        if rows is None or rows == self.batch:
+            self.engine.forward(self._x_nhwc, None, None, self.seq, additional_residuals=residuals, temb_all=temb,
+                                kv_all=self._kv_all, out=self._out_nhwc)
+            return
+        kv = self._kv_all[:rows * self.seq] if self._kv_all is not None else None
+        self.engine.forward(self._x_nhwc[:rows], None, None, self.seq, additional_residuals=residuals,
+                            temb_all=temb, kv_all=kv, out=self._out_nhwc[:rows])
 
-    def _launch(self):
+    def _launch(self, rows=None):
+        if rows is not None and rows != self.batch:  # the step-by-step guidance-free loop: eager, no graph of its own
+            self._run(rows)
+            return
         if not self.use_cuda_graph:
             self._run()
             return
@@ -172,18 +195,27 @@ class UNetModel(B200Model):
         self._graph.replay()
 
     def forward_device(self, sample, timestep, encoder_hidden_states, time_ids=None, text_embeds=None,
-                       additional_residuals=None):
-        """CUDA tensors in, CUDA fp32 ``noise_pred`` (a view of the static output buffer) out."""
-        self._sample.copy_(sample)
-        self._t.copy_(timestep)
-        self._ctx.copy_(encoder_hidden_states)
+                       additional_residuals=None, timestep_cond=None):
+        """CUDA tensors in, CUDA fp32 ``noise_pred`` (a view of the static output buffer) out.  ``sample`` may have
+        fewer rows than the batch the model was built for (the guidance-free loop): then every input has that many
+        rows and only those run."""
+        r = sample.shape[0]
+        if not 0 < r <= self.batch:
+            raise ValueError(f"sample has {r} rows, the UNet was built for at most {self.batch}")
+        self._sample[:r].copy_(sample)
+        self._t[:r].copy_(timestep)
+        self._ctx[:r].copy_(encoder_hidden_states)
         if self.engine.xl:
-            self._time_ids.copy_(time_ids.reshape(self._time_ids.shape))
-            self._text_embeds.copy_(text_embeds)
-        for buf, r in zip(self._res, additional_residuals or []):
-            buf.copy_(r)
-        self._launch()
-        return self._out
+            self._time_ids[:r].copy_(time_ids.reshape(r, -1))
+            self._text_embeds[:r].copy_(text_embeds)
+        if self._cond is not None:
+            if timestep_cond is None:
+                raise ValueError(f"this UNet has time_cond_proj_dim={self.engine.time_cond_dim}: pass timestep_cond")
+            self._cond[:r].copy_(timestep_cond)
+        for buf, res in zip(self._res, additional_residuals or []):
+            buf[:r].copy_(res)
+        self._launch(r)
+        return self._out[:r]
 
     def __call__(self, **kwargs):
         self._verify_inputs(**kwargs)
@@ -197,6 +229,8 @@ class UNetModel(B200Model):
         if self.engine.xl:
             self._to_device(kwargs["time_ids"], self._time_ids)
             self._to_device(kwargs["text_embeds"], self._text_embeds)
+        if self._cond is not None:
+            self._to_device(kwargs["timestep_cond"], self._cond)
         for i, buf in enumerate(self._res):
             self._to_device(kwargs[f"additional_residual_{i}"], buf)
         self._launch()

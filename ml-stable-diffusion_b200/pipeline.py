@@ -240,7 +240,29 @@ class B200StableDiffusionPipeline:
                    tokenizer=tokenizer, vae_encoder=venc, force_zeros_for_empty_prompt=unet.engine.xl,
                    scheduler_kwargs=scheduler_kwargs, safety_checker=checker)
 
-    _SCHEDULER_CLASS = {"PNDMScheduler": "PNDM", "DDIMScheduler": "DDIM", "DPMSolverMultistepScheduler": "DPMSolverMultistep"}
+    _SCHEDULER_CLASS = {"PNDMScheduler": "PNDM", "DDIMScheduler": "DDIM", "DPMSolverMultistepScheduler": "DPMSolverMultistep",
+                        "LCMScheduler": "LCM", "EulerDiscreteScheduler": "EulerDiscrete",
+                        "EulerAncestralDiscreteScheduler": "EulerAncestralDiscrete",
+                        "LMSDiscreteScheduler": "LMSDiscrete"}
+
+    @classmethod
+    def scheduler_from_config(cls, sched_cfg: dict) -> str:
+        """The scheduler a checkpoint's ``scheduler_config.json`` names (``_class_name``, PNDM when absent).  The Euler /
+        Euler-ancestral / LMS classes are taken from the checkpoint only with the ``"trailing"`` spacing the few-step
+        checkpoints ship (SD-Turbo, SDXL-Turbo, SDXL-Lightning); with any other spacing (SDXL-base's ``"leading"``
+        Euler) the caller chooses the sampler through ``scheduler_override``, as before."""
+        name = sched_cfg.get("_class_name", "PNDMScheduler")
+        sched = cls._SCHEDULER_CLASS.get(name)
+        if sched is None or (sched in S.SIGMA_SCHEDULERS and sched_cfg.get("timestep_spacing") != "trailing"):
+            why = "" if sched is None else f" with timestep_spacing={sched_cfg.get('timestep_spacing')!r}"
+            raise ValueError(f"scheduler {name} of the checkpoint{why} is not implemented as its default; pass "
+                             f"scheduler_override (one of {sorted(S.SCHEDULER_MAP)})")
+        return sched
+
+    def do_classifier_free_guidance(self, guidance_scale):
+        """diffusers' rule: classifier-free guidance runs iff guidance_scale > 1 and the UNet has no guidance
+        embedding (time_cond_proj_dim).  Otherwise the loop runs guidance-free, the UNet on the N prompt rows only."""
+        return guidance_scale > 1.0 and not self.unet.engine.time_cond_dim
 
     @classmethod
     def from_pretrained(cls, model_dir, images_per_call=1, device="cuda", height=None, width=None,
@@ -310,18 +332,15 @@ class B200StableDiffusionPipeline:
         sched = scheduler_override
         sched_kw = None
         sched_cfg = os.path.join(model_dir, "scheduler", "scheduler_config.json")
-        if sched in S.SIGMA_SCHEDULERS and os.path.exists(sched_cfg):
-            # SCHEDULER_MAP[name].from_config(pytorch_pipe.scheduler.config) (pipeline.py:672-676): spacing, offset
-            # and betas come from the checkpoint (SDXL: "leading", offset 1)
-            with open(sched_cfg) as fh:
-                sched_kw = S.sigma_scheduler_kwargs(json.load(fh))
         if sched is None:
-            with open(os.path.join(model_dir, "scheduler", "scheduler_config.json")) as fh:
-                name = json.load(fh).get("_class_name", "PNDMScheduler")
-            if name not in cls._SCHEDULER_CLASS:
-                raise ValueError(f"scheduler {name} of the checkpoint is not implemented; pass scheduler_override "
-                                 f"(one of {sorted(S.SCHEDULER_MAP)})")
-            sched = cls._SCHEDULER_CLASS[name]
+            with open(sched_cfg) as fh:
+                sched = cls.scheduler_from_config(json.load(fh))
+        if sched in S.SIGMA_SCHEDULERS + ("LCM",) and os.path.exists(sched_cfg):
+            # SCHEDULER_MAP[name].from_config(pytorch_pipe.scheduler.config) (pipeline.py:672-676): spacing, offset
+            # and betas come from the checkpoint (SDXL: "leading", offset 1; Turbo / Lightning: "trailing")
+            with open(sched_cfg) as fh:
+                sc = json.load(fh)
+            sched_kw = S.lcm_scheduler_kwargs(sc) if sched == "LCM" else S.sigma_scheduler_kwargs(sc)
         if sched in S.PREDICTION_TYPE_SCHEDULERS and os.path.exists(sched_cfg):
             # SD 2.0 / 2.1 768-v checkpoints are v-prediction models ("prediction_type": "v_prediction"); diffusers
             # applies the key inside scheduler.step (pipeline.py:565-569), these schedulers take it in their plan
@@ -478,12 +497,13 @@ class B200StableDiffusionPipeline:
         if not self.controlnet:
             raise ValueError("Conditions for controlnet are given but the pipeline has no controlnet modules")
         total = None
+        r = sample.shape[0]  # the batch, or its first half in the guidance-free loop
         for module, cond in zip(self.controlnet, controlnet_cond):
-            module._sample.copy_(sample)
-            module._t.copy_(timestep)
-            module._ctx.copy_(encoder_hidden_states)
-            module._cond.copy_(cond)
-            outs = module.forward_device()
+            module._sample[:r].copy_(sample)
+            module._t[:r].copy_(timestep)
+            module._ctx[:r].copy_(encoder_hidden_states)
+            module._cond[:r].copy_(cond)
+            outs = module.forward_device(r)
             if total is None:
                 total = list(outs)
             else:
@@ -511,7 +531,7 @@ class B200StableDiffusionPipeline:
         return k
 
     def _loop_on_static_buffers(self, plan, guidance_scale, ts_rows, use_controlnet=False, refiner_start_step=None,
-                                inpaint=None, blend=None):
+                                inpaint=None, blend=None, guided=True):
         """The whole N-step loop on static device buffers (no host-side tensor arguments): what the loop graph
         captures.  Prologue, once per prompt: cross-attention K/V of all blocks from the text states, the
         time-embedding biases of all ResNet blocks for ALL timesteps (`ts_rows`: each step's timestep repeated per
@@ -520,43 +540,55 @@ class B200StableDiffusionPipeline:
         input (fp16 NHWC, both CFG halves: pipeline.py:502 np.concatenate([latents] * 2)) -- no fill / copy /
         layout kernels in between.  ``inpaint`` ("blend" / "unet9", see ``_inpaint_kind``): "blend" runs the step
         kernel's blend with ``blend[i]`` = (a, b) of step i; "unet9" writes the five conditioning channels (mask,
-        masked image latents) into both halves of the first UNet input, which the step kernel never overwrites."""
+        masked image latents) into both halves of the first UNet input, which the step kernel never overwrites.
+        ``guided=False``: the guidance-free loop: every launch (K/V prologue, time table, UNet, ControlNets, step)
+        sees only the N prompt rows [0, N) of the static buffers; ``ts_rows`` holds N entries per step."""
         n = self.images_per_call
+        rows = self.unet.batch if guided else n
         rs = len(plan) if refiner_start_step is None else max(0, min(len(plan), refiner_start_step))
         # which UNet runs each step: the SDXL refiner takes over at refiner_start_step with its own conditioning
         # (StableDiffusionXLPipeline.swift:205-225); each model gets its per-prompt prologue and its own time table
         models = [self.unet if i < rs else self.unet_refiner for i in range(len(plan))]
         self._hist.zero_()
-        b = self.unet.batch
         tables = {}
         for m, lo, hi in ((self.unet, 0, rs), (self.unet_refiner, rs, len(plan))):
             if hi > lo:
-                m.prepare_prompt()
-                tables[id(m)] = (m.time_table(ts_rows[lo * b: hi * b]), lo)
+                m.prepare_prompt(rows)
+                tables[id(m)] = (m.time_table(ts_rows[lo * rows: hi * rows], rows), lo)
         first = models[0]
         x_in = self._latents
         if inpaint == "unet9":
             x_in = self._inpaint_bufs["unet_in"]
             x_in[:, :self.latent_channels].copy_(self._latents)
         L.nchw_to_nhwc(x_in, c_pad=first.engine.in_pad, out=first._x_nhwc[:n])
-        L.nchw_to_nhwc(x_in, c_pad=first.engine.in_pad, out=first._x_nhwc[n:])
+        if guided:
+            L.nchw_to_nhwc(x_in, c_pad=first.engine.in_pad, out=first._x_nhwc[n:])
         if use_controlnet:
-            self.prepare_controlnets(ts_rows)
+            self.prepare_controlnets(ts_rows, rows)
         for i, st in enumerate(plan):
             u = models[i]
             table, lo = tables[id(u)]
-            u._run_core(table[i - lo], self.controlnet_residuals(i) if use_controlnet else None)
+            u._run_core(table[i - lo], self.controlnet_residuals(i, rows=rows) if use_controlnet else None, rows)
             k = self._coeffs(st, guidance_scale)
             k.noise_pred_nhwc = 1
             nxt = models[i + 1] if i + 1 < len(plan) else u
-            self._step(st, k, u._out_nhwc, unet_in=nxt._x_nhwc, blend=blend[i] if blend else None)
+            self._step(st, k, u._out_nhwc[:rows], unet_in=nxt._x_nhwc, blend=blend[i] if blend else None,
+                       guided=guided)
 
-    def _step(self, st, k, noise_pred, unet_in=None, blend=None):
+    def _step(self, st, k, noise_pred, unet_in=None, blend=None, guided=True):
         """One fused guidance + scheduler update of the loop state, with the step's noise when the plan has some and
-        the inpainting blend with ``blend`` = (a, b) when given."""
-        if blend is not None:
+        the inpainting blend with ``blend`` = (a, b) when given.  ``guided=False``: ``noise_pred`` holds one
+        prediction per image and the step kernel's guidance-free mode runs."""
+        noised = st.noise_offset >= 0
+        if not guided:
             b = self._inpaint_bufs
-            noised = st.noise_offset >= 0
+            L.scheduler_step_guidance_free(
+                noise_pred, self._latents, k, st.noise_scale if noised else 0.0, self._noise_key if noised else None,
+                self._noise_base + st.noise_offset if noised else 0,
+                blend=(b["mask"], b["image_latents"], b["noise"], blend[0], blend[1]) if blend is not None else None,
+                hist=self._hist, denoised=self._denoised, unet_in=unet_in)
+        elif blend is not None:
+            b = self._inpaint_bufs
             L.cfg_scheduler_step_blend(noise_pred, self._latents, k, b["mask"], b["image_latents"], b["noise"],
                                        blend[0], blend[1], st.noise_scale if noised else 0.0,
                                        self._noise_key if noised else None,
@@ -613,50 +645,53 @@ class B200StableDiffusionPipeline:
     def set_control_conditions(self, controlnet_cond):
         """Copy the conditioning images (each (2B, 3, H, W)) into the ControlNets' static input buffers."""
         for module, cond in zip(self.controlnet, controlnet_cond):
-            module._cond.copy_(torch.as_tensor(cond))
+            cond = torch.as_tensor(cond)
+            module._cond[:cond.shape[0]].copy_(cond)
 
-    def prepare_controlnets(self, ts_rows):
+    def prepare_controlnets(self, ts_rows, rows=None):
         """Device-loop prologue of every ControlNet: text states, the embedding of its conditioning image (static
-        buffer `_cond`), time-embedding table."""
+        buffer `_cond`), time-embedding table (of the first ``rows`` images: the guidance-free loop)."""
         for module in self.controlnet:
             module._ctx.copy_(self.unet._ctx)
-            module.prepare_prompt(ts_rows)
+            module.prepare_prompt(ts_rows, rows)
 
-    def controlnet_residuals(self, step, _temb=None):
+    def controlnet_residuals(self, step, _temb=None, rows=None):
         """pipeline.py:259-284 inside the device loop: every ControlNet sees the UNet's input; residuals are summed."""
         total = None
+        x = self.unet._x_nhwc if rows is None else self.unet._x_nhwc[:rows]
         for module in self.controlnet:
-            outs = module.run_core(self.unet._x_nhwc, step)
+            outs = module.run_core(x, step)
             if total is None:
                 total = list(outs)
             else:
                 total = [L.add(acc, o) for acc, o in zip(total, outs)]
         return total
 
-    def _ts_rows(self, plan):
-        return torch.tensor([float(st.timestep) for st in plan for _ in range(self.unet.batch)], dtype=torch.float32,
-                            device=self.device)
+    def _ts_rows(self, plan, rows=None):
+        return torch.tensor([float(st.timestep) for st in plan for _ in range(rows or self.unet.batch)],
+                            dtype=torch.float32, device=self.device)
 
     def _loop_graph_for(self, key, plan, guidance_scale, use_controlnet=False, refiner_start_step=None, inpaint=None,
-                        blend=None):
+                        blend=None, guided=True):
         g = self._loop_graphs.get(key)
         if g is None:
             keep = self._latents.clone()
-            ts_rows = self._ts_rows(plan)
+            rows = self.unet.batch if guided else self.images_per_call
+            ts_rows = self._ts_rows(plan, rows)
             s = torch.cuda.Stream(device=self.device)  # eager warm-up off the capture: workspaces, weight tiling
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._loop_on_static_buffers(plan[:1], guidance_scale, ts_rows[: self.unet.batch], use_controlnet,
-                                             inpaint=inpaint, blend=blend[:1] if blend else None)
+                self._loop_on_static_buffers(plan[:1], guidance_scale, ts_rows[:rows], use_controlnet,
+                                             inpaint=inpaint, blend=blend[:1] if blend else None, guided=guided)
                 if refiner_start_step is not None and refiner_start_step < len(plan):  # warm the refiner's kernels too
-                    self._loop_on_static_buffers(plan[-1:], guidance_scale, ts_rows[-self.unet.batch:], use_controlnet, 0)
+                    self._loop_on_static_buffers(plan[-1:], guidance_scale, ts_rows[-rows:], use_controlnet, 0)
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
             self._latents.copy_(keep)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._loop_on_static_buffers(plan, guidance_scale, ts_rows, use_controlnet, refiner_start_step,
-                                             inpaint, blend)
+                                             inpaint, blend, guided)
             g._b200sd_keep = ts_rows
             self._latents.copy_(keep)  # capture does not execute, but keep the contract obvious
             if len(self._loop_graphs) >= 4:
@@ -680,17 +715,40 @@ class B200StableDiffusionPipeline:
         is drawn.
         ``inpaint`` (``InpaintInputs``): the latent mask and image latents of an inpainting call (``__call__`` with
         ``mask_image``); required for a 9-channel UNet.  They are copied into static buffers before the loop, so the
-        loop graph depends on the inpainting kind only, never on the mask or the images."""
+        loop graph depends on the inpainting kind only, never on the mask or the images.
+
+        Without classifier-free guidance (``do_classifier_free_guidance``: guidance_scale <= 1, or a guidance-embedding
+        UNet) the loop runs guidance-free: the UNet (still built at batch 2B) and the ControlNets run on B rows only.
+        ``text_embeddings``, ``time_ids`` and ``text_embeds`` may then have B rows, or 2B in the uncond-first layout,
+        whose second (prompt) half is taken.  A guidance-embedding UNet is conditioned on
+        ``unet.guidance_scale_embedding(guidance_scale)``."""
         sched = S.make_scheduler(self.scheduler_name, num_inference_steps, **self.scheduler_kwargs)
         plan = list(sched.plan(start=start_step)) if start_step else list(sched.plan())
         n = self.images_per_call
+        guided = self.do_classifier_free_guidance(guidance_scale)
+        rows = self.unet.batch if guided else n
+        if refiner is not None and not guided:
+            raise ValueError("the SDXL refiner hand-off runs with classifier-free guidance only (guidance_scale > 1)")
         kind = self._inpaint_kind(inpaint is not None, start_step, bool(controlnet_cond), refiner is not None)
         blend = None
         if kind is not None:
             self._set_inpaint_buffers(kind, inpaint)
             if kind == "blend":
                 blend = sched.blend_coeffs(start_step)
-        self._ctx.copy_(torch.as_tensor(text_embeddings), non_blocking=True)
+        if guided:
+            self._ctx.copy_(torch.as_tensor(text_embeddings), non_blocking=True)
+        else:
+            text_embeddings = torch.as_tensor(text_embeddings)
+            if text_embeddings.shape[0] not in (n, 2 * n):
+                raise ValueError(f"text_embeddings has {text_embeddings.shape[0]} rows, expected {n} or {2 * n}")
+            self._ctx[:n].copy_(text_embeddings[-n:], non_blocking=True)
+            if time_ids is not None:
+                time_ids = torch.as_tensor(time_ids).reshape(-1, self.unet._time_ids.shape[1])[-n:]
+            if text_embeds is not None:
+                text_embeds = torch.as_tensor(text_embeds)[-n:]
+        if self.unet.engine.time_cond_dim:
+            from .unet import guidance_scale_embedding
+            self.unet._cond[:n].copy_(guidance_scale_embedding(guidance_scale, self.unet.engine.time_cond_dim, n))
         self._latents.copy_(torch.as_tensor(latents), non_blocking=True)
         if sched.input_scale(0) != 1.0:
             self._latents.div_(sched.input_scale(0))
@@ -704,6 +762,8 @@ class B200StableDiffusionPipeline:
             return self._latents if s == 1.0 else self._latents * s
         if controlnet_cond:
             controlnet_cond = [torch.as_tensor(c).to(self.device, torch.float16) for c in controlnet_cond]
+            if not guided:  # the condition images of the B prompt rows (prepare_control_cond doubles them)
+                controlnet_cond = [c[-n:] for c in controlnet_cond]
         elif self.unet._res:
             # a UNet built with additional_residual inputs but called without conditions: the static residual buffers
             # would still hold the previous ControlNet call's last step (the reference cannot run this combination)
@@ -713,8 +773,8 @@ class B200StableDiffusionPipeline:
             u = self.unet
             u._ctx.copy_(self._ctx)
             if u.engine.xl:
-                u._time_ids.copy_(torch.as_tensor(time_ids).reshape(u._time_ids.shape))
-                u._text_embeds.copy_(torch.as_tensor(text_embeds))
+                u._time_ids[:rows].copy_(torch.as_tensor(time_ids).reshape(rows, -1))
+                u._text_embeds[:rows].copy_(torch.as_tensor(text_embeds))
             if controlnet_cond:
                 self.set_control_conditions(controlnet_cond)
             rstep = None
@@ -727,8 +787,9 @@ class B200StableDiffusionPipeline:
                 r._text_embeds.copy_(torch.as_tensor(refiner["text_embeds"]))
                 rstep = int(np.float32(len(plan)) * np.float32(refiner_start))  # Int(Float(timeSteps.count) * refinerStart)
             key = (self.scheduler_name, int(num_inference_steps), float(guidance_scale), int(start_step),
-                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base, kind)
-            self._loop_graph_for(key, plan, guidance_scale, bool(controlnet_cond), rstep, kind, blend).replay()
+                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base, guided,
+                   kind)
+            self._loop_graph_for(key, plan, guidance_scale, bool(controlnet_cond), rstep, kind, blend, guided).replay()
             return self._denoised if return_denoised else self._latents
         if refiner is not None:
             raise ValueError("the refiner hand-off runs in the device loop only (no callback / record)")
@@ -740,15 +801,17 @@ class B200StableDiffusionPipeline:
             if kind == "unet9":  # cat([latents, mask, masked_image_latents], 1), the same conditioning every step
                 x_in = self._inpaint_bufs["unet_in"]
                 x_in[:, :self.latent_channels].copy_(self._latents)
-            sample = torch.cat([x_in, x_in], 0)  # pipeline.py:502
+            sample = torch.cat([x_in, x_in], 0) if guided else x_in  # pipeline.py:502
             residuals = None
             if controlnet_cond:  # pipeline.py:515-529
-                residuals = self.run_controlnet(sample, self._t, self._ctx, controlnet_cond)
-            noise_pred = self.unet.forward_device(sample, self._t, self._ctx, time_ids, text_embeds, residuals)
+                residuals = self.run_controlnet(sample, self._t[:rows], self._ctx[:rows], controlnet_cond)
+            noise_pred = self.unet.forward_device(sample, self._t[:rows], self._ctx[:rows], time_ids, text_embeds,
+                                                  residuals, self.unet._cond[:rows] if self.unet._cond is not None
+                                                  else None)
             self._coeffs(st, guidance_scale, k)
             if record is not None:
                 eps_copy = noise_pred.clone()
-            self._step(st, k, noise_pred, blend=blend[i] if blend else None)
+            self._step(st, k, noise_pred, blend=blend[i] if blend else None, guided=guided)
             if record is not None:
                 record.append((st.timestep, eps_copy, x_space(i + 1).clone()))
             if callback is not None and i % callback_steps == 0:
@@ -838,7 +901,12 @@ class B200StableDiffusionPipeline:
         if len(prompts) != self.images_per_call:
             raise ValueError(f"this pipeline instance generates {self.images_per_call} image(s) per call, "
                              f"got {len(prompts)} prompt(s)")
-        do_cfg = guidance_scale > 1.0  # pipeline.py:443
+        do_cfg = self.do_classifier_free_guidance(guidance_scale)  # pipeline.py:443, and no guidance embedding
+        if self.scheduler_name == "LCM":
+            for name, v in (("mask_image", mask_image), ("starting_image", starting_image)):
+                if v is not None:
+                    raise ValueError(f"{name} is not supported with the LCM scheduler (its strength changes the "
+                                     f"timesteps themselves)")
         xl_pooled = None
         if prompt_embeds is not None:
             text_embeddings = prompt_embeds

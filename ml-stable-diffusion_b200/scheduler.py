@@ -456,6 +456,82 @@ class LMSDiscreteScheduler(_SigmaScheduler):
         st.push_eps_slot = i % 3
 
 
+class LCMScheduler(_Base):
+    """diffusers 0.30.2 ``LCMScheduler`` (latent consistency models), restated from its ``set_timesteps`` and ``step``.
+
+    Timesteps: with k = n_train // original_inference_steps, origin = (arange(1, original_inference_steps + 1) k - 1)
+    reversed, the n steps are origin[floor(linspace(0, len(origin), n, endpoint=False))] (4 of 50: 999, 759, 499, 259).
+    Step i at t, prev = timesteps[i + 1] (t itself on the last step), abar from diffusers' fp32 table:
+        s = timestep_scaling t,  c_skip = 0.25 / (s^2 + 0.25),  c_out = s / sqrt(s^2 + 0.25)      (sigma_data = 0.5)
+        x0 = (x - sqrt(1 - abar_t) eps) / sqrt(abar_t)    (v_prediction: x0 = sqrt(abar_t) x - sqrt(1 - abar_t) v)
+        denoised = c_out x0 + c_skip x
+        x' = sqrt(abar_prev) denoised + sqrt(1 - abar_prev) z   on every step but the last, where x' = denoised.
+    All of it is linear in (x, eps, z): the plan's x0 terms are ``denoised``, the noise is noise draw number i with
+    noise_scale sqrt(1 - abar_prev).  z is the in-kernel Philox stream keyed by the seed (as for Euler-ancestral), so
+    the images are not bit-compatible with diffusers' torch-generator noise.  No image-to-image schedule: LCM's
+    ``strength`` changes the timesteps themselves."""
+
+    def __init__(self, num_inference_steps, original_inference_steps=50, timestep_scaling=10.0,
+                 prediction_type="epsilon", num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012,
+                 beta_schedule="scaled_linear"):
+        super().__init__(num_inference_steps, num_train_timesteps, beta_start, beta_end, beta_schedule)
+        self.original_inference_steps = int(original_inference_steps)
+        if self.n > self.original_inference_steps:
+            raise ValueError(f"num_inference_steps={self.n} exceeds the LCM schedule's original_inference_steps="
+                             f"{self.original_inference_steps}")
+        self.timestep_scaling = float(timestep_scaling)
+        self.prediction_type = check_prediction_type(prediction_type)
+        self.abar = alphas_cumprod_diffusers(beta_start, beta_end, num_train_timesteps, beta_schedule).astype(np.float64)
+        k = self.n_train // self.original_inference_steps
+        origin = (np.arange(1, self.original_inference_steps + 1) * k - 1)[::-1]
+        idx = np.floor(np.linspace(0, len(origin), self.n, endpoint=False)).astype(np.int64)
+        self.lcm_timesteps = [int(t) for t in origin[idx]]
+
+    def plan(self, start=0):
+        if start:
+            raise ValueError("LCMScheduler has no image-to-image schedule")
+        ts = self.lcm_timesteps
+        out = []
+        for i, t in enumerate(ts):
+            last = i == len(ts) - 1
+            a_t = self.abar[t]
+            a_p = self.abar[t if last else ts[i + 1]]
+            s = t * self.timestep_scaling
+            c_skip = 0.25 / (s * s + 0.25)
+            c_out = s / math.sqrt(s * s + 0.25)
+            if self.prediction_type == "epsilon":
+                x0_x, x0_e = 1.0 / math.sqrt(a_t), -math.sqrt(1.0 - a_t) / math.sqrt(a_t)
+            else:
+                x0_x, x0_e = math.sqrt(a_t), -math.sqrt(1.0 - a_t)
+            d_x, d_e = c_out * x0_x + c_skip, c_out * x0_e
+            st = StepPlan(t, d_x, d_e, [0.0] * 4, d_x, d_e, [0.0] * 4)
+            if not last:
+                st.cx, st.ce = math.sqrt(a_p) * d_x, math.sqrt(a_p) * d_e
+                st.noise_scale, st.noise_offset = math.sqrt(1.0 - a_p), i
+            out.append(st)
+        return out
+
+
+def lcm_scheduler_kwargs(config: dict) -> dict:
+    """Constructor arguments of ``LCMScheduler`` from a checkpoint's ``scheduler_config.json``.  The options that make
+    the step non-linear (sample clipping, dynamic thresholding) or change the beta table (zero-SNR rescaling, trained
+    betas) raise a ValueError that names the key."""
+    unsupported = {
+        "clip_sample": bool,
+        "thresholding": bool,
+        "rescale_betas_zero_snr": bool,
+        "trained_betas": lambda v: v is not None,
+    }
+    for key, bad in unsupported.items():
+        if key in config and bad(config[key]):
+            raise ValueError(f"scheduler config {key}={config[key]!r} is not supported by the LCM scheduler")
+    if "prediction_type" in config:
+        check_prediction_type(config["prediction_type"])
+    used = ("original_inference_steps", "timestep_scaling", "prediction_type", "beta_start", "beta_end",
+            "beta_schedule", "num_train_timesteps")
+    return {key: config[key] for key in used if key in config}
+
+
 SCHEDULER_MAP = {
     "DDIM": DDIMScheduler,
     "DPMSolverMultistep": DPMSolverMultistepScheduler,
@@ -463,6 +539,7 @@ SCHEDULER_MAP = {
     "EulerDiscrete": EulerDiscreteScheduler,
     "EulerAncestralDiscrete": EulerAncestralDiscreteScheduler,
     "LMSDiscrete": LMSDiscreteScheduler,
+    "LCM": LCMScheduler,
 }
 
 #: the scheduler classes whose loop state is y = x / sqrt(sigma^2 + 1)

@@ -88,6 +88,19 @@ class _Packer:
         return self.f32(k) if k in self.sd else None
 
 
+def guidance_scale_embedding(guidance_scale, dim, batch=1):
+    """diffusers 0.30.2 ``get_guidance_scale_embedding`` (what a guidance-embedding UNet is conditioned on) in fp32:
+    w = (guidance_scale - 1) * 1000, f = exp(-arange(dim // 2) * log(10000) / (dim // 2 - 1)),
+    cat(sin(w f), cos(w f)), zero-padded to ``dim`` when it is odd.  -> fp32 CPU tensor [batch, dim]."""
+    half = dim // 2
+    w = torch.tensor(float(guidance_scale) - 1.0, dtype=torch.float32) * 1000.0
+    f = torch.exp(torch.arange(half, dtype=torch.float32) * -(torch.log(torch.tensor(10000.0)) / (half - 1)))
+    emb = torch.cat([torch.sin(w * f), torch.cos(w * f)])
+    if dim % 2:
+        emb = torch.nn.functional.pad(emb, (0, 1))
+    return emb[None].repeat(batch, 1)
+
+
 class UNetEngine:
     """Holds device-resident packed weights and issues the forward launch sequence."""
 
@@ -118,6 +131,8 @@ class UNetEngine:
         self.in_pad = max(8, (self.in_ch + 7) // 8 * 8)
         self.xl = cfg.get("addition_embed_type") == "text_time"
         self.support_controlnet = bool(cfg.get("support_controlnet", False))
+        # guidance-embedding (LCM) UNets: time_embedding takes a [B, time_cond_proj_dim] condition
+        self.time_cond_dim = int(cfg.get("time_cond_proj_dim") or 0)
         # Normalisation fusion level (B200SD_FUSED):
         #   "ln" (default)  LayerNorm folded into its consumer GEMM, row statistics from the producer's epilogue;
         #                   GroupNorm stays the one-launch cluster kernel in front of the 9-tap TMA convolution (the
@@ -294,6 +309,8 @@ class UNetEngine:
         w["conv_in"] = {"w": P.conv3("conv_in", pad_in=self.in_pad), "b": P.bias("conv_in")}
         w["time"] = {"l1": P.lin("time_embedding.linear_1"), "l1b": P.bias("time_embedding.linear_1"),
                      "l2": P.lin("time_embedding.linear_2"), "l2b": P.bias("time_embedding.linear_2")}
+        if self.time_cond_dim:
+            w["time"]["cond"] = P.lin("time_embedding.cond_proj")
         if self.xl:
             w["add"] = {"l1": P.lin("add_embedding.linear_1"), "l1b": P.bias("add_embedding.linear_1"),
                         "l2": P.lin("add_embedding.linear_2"), "l2b": P.bias("add_embedding.linear_2")}
@@ -663,12 +680,21 @@ class UNetEngine:
                              out=out)
 
     # ------------------------------------------------------------------ forward
-    def time_embedding(self, timesteps, time_ids=None, text_embeds=None):
-        """fp32 [B] -> per-image bias vectors of every ResNet block: fp32 [B, sum Cout]."""
+    def time_embedding(self, timesteps, time_ids=None, text_embeds=None, timestep_cond=None):
+        """fp32 [B] -> per-image bias vectors of every ResNet block: fp32 [B, sum Cout].  ``timestep_cond``: fp32
+        [B, time_cond_proj_dim], required by a guidance-embedding UNet: cond_proj(timestep_cond) is added to the
+        sinusoidal embedding before linear_1 (diffusers' TimestepEmbedding.forward)."""
         cfg = self.cfg
         tw = self.w["time"]
         t_emb = L.timestep_embedding(timesteps, self.boc[0], cfg.get("flip_sin_to_cos", True),
                                      cfg.get("freq_shift", 0))
+        if self.time_cond_dim:
+            if timestep_cond is None or tuple(timestep_cond.shape) != (timesteps.shape[0], self.time_cond_dim):
+                raise ValueError(f"this UNet has time_cond_proj_dim={self.time_cond_dim}: pass timestep_cond of shape "
+                                 f"{(timesteps.shape[0], self.time_cond_dim)}")
+            t_emb = t_emb + L.linear_small(timestep_cond.float().contiguous(), tw["cond"], None)
+        elif timestep_cond is not None:
+            raise ValueError("timestep_cond was given but the UNet has no time_cond_proj_dim")
         emb = L.linear_small(L.linear_small(t_emb, tw["l1"], tw["l1b"], act_out=True), tw["l2"], tw["l2b"])
         if self.xl:
             aw = self.w["add"]
@@ -685,15 +711,15 @@ class UNetEngine:
         return L.linear(ctx_tokens, self.kv_w, static_w=True, out=out) if self.kv_w is not None else None
 
     def forward(self, sample, timesteps, ctx_tokens, s_ctx, time_ids=None, text_embeds=None,
-                additional_residuals=None, temb_all=None, kv_all=None, out=None):
+                additional_residuals=None, temb_all=None, kv_all=None, out=None, timestep_cond=None):
         """sample: NHWC fp16 [B, H, W, in_pad]; timesteps fp32 [B]; ctx_tokens fp16 [B*s_ctx, D].
         additional_residuals: list of NHWC fp16 tensors (ControlNet, unet.py:1009-1022).
         temb_all / kv_all: precomputed time-embedding biases [B, sum Cout] / cross-attention keys and values (the
-        per-prompt prologue of the pipeline's loop); out: optional fp32 NHWC output buffer.
-        Returns noise_pred NHWC fp32 [B, H, W, out_ch]."""
+        per-prompt prologue of the pipeline's loop); out: optional fp32 NHWC output buffer.  timestep_cond: see
+        time_embedding.  Returns noise_pred NHWC fp32 [B, H, W, out_ch]."""
         batch = sample.shape[0]
         if temb_all is None:
-            temb_all = self.time_embedding(timesteps, time_ids, text_embeds)
+            temb_all = self.time_embedding(timesteps, time_ids, text_embeds, timestep_cond)
         if kv_all is None:
             kv_all = self.kv_project(ctx_tokens)
         if self.fused:

@@ -2,13 +2,19 @@
 
     python tools/model_bench.py --model sd15|sd21-base|sd21 [--reps 3]
     python tools/model_bench.py --inpaint [--rounds 5] [--reps 3]
+    python tools/model_bench.py --guidance-free --model sd21-base|sdxl-base [--rounds 5] [--reps 3]
 
 The workload is bench.py's: random-init weights, txt2img 512x512 at UNet batch 2 (uncond, cond), 20 DDIM steps, CFG
 7.5, the 20 steps (with the per-prompt prologue) captured as one CUDA graph by bench.LoopBench and timed with
 bench.timed_replays.  ``sd21`` (SD 2.0 / 2.1 768-v) runs the same UNet at 768x768 (96x96 latents) with 20 DDIM
 v-prediction steps.  The attention time is the same loop captured with only the attention class launching
 (classes=2).  Prints one JSON line: iter/s, ms per step, attention ms per step, card name, power limit and the median
-SM clock while the loop ran."""
+SM clock while the loop ran.
+
+``--guidance-free`` (512x512, random-init weights): the pipeline's 20-step DDIM loop graph with CFG 7.5 (UNet batch 2)
+against the same loop guidance-free (guidance 1.0, UNet batch 1), and the whole ``__call__`` (text encoding, the loop,
+VAE decode; output_type "np") of a 1-step Euler-ancestral (trailing) call at guidance 0 and a 4-step LCM call (the
+UNet with time_cond_proj_dim=256), alternated ``--rounds`` times.  One JSON line per mode."""
 import argparse
 import json
 import os
@@ -74,13 +80,92 @@ def inpaint_modes(args, dev):
                           "sm_mhz": clocks.get("sm_mhz"), "clock_events": clocks.get("reasons")}), flush=True)
 
 
+def guidance_free_modes(args, dev):
+    import time
+
+    import numpy as np
+
+    from b200sd import config as C
+    from b200sd.pipeline import B200StableDiffusionPipeline as P
+
+    model = args.model
+    base = {"sd21-base": C.SD21_BASE_UNET, "sdxl-base": C.SDXL_BASE_UNET}[model]
+    ddim = P.from_random_init(model, device=dev, seed=1, scheduler="DDIM")
+    turbo = P.from_random_init(model, device=dev, seed=1, scheduler="EulerAncestralDiscrete",
+                               scheduler_kwargs={"timestep_spacing": "trailing"})
+    lcm = P.from_random_init(model, device=dev, seed=1, scheduler="LCM",
+                             unet_cfg=dict(base, time_cond_proj_dim=256))
+    g = torch.Generator().manual_seed(93)
+    d_ctx = ddim.unet._ctx.shape[1]
+    emb = torch.cat([torch.zeros(1, d_ctx, 1, 77), torch.randn(1, d_ctx, 1, 77, generator=g)]).half()
+    lat = torch.randn(1, 4, 64, 64, generator=g).half().float()
+    kw = {}
+    if ddim.xl:
+        kw = dict(time_ids=torch.tensor([[512.0, 512.0, 0.0, 0.0, 512.0, 512.0]] * 2),
+                  text_embeds=torch.randn(2, 1280, generator=g))
+    n = bench.N_STEPS_IMG
+    graphs = {}
+    for mode, gs in (("ddim20-cfg-b2", 7.5), ("ddim20-guidance-free-b1", 1.0)):
+        before = set(ddim._loop_graphs)
+        ddim.denoise(emb, lat, n, gs, **kw)
+        key, = set(ddim._loop_graphs) - before
+        graphs[mode] = ddim._loop_graphs[key]
+    calls = {"euler-a-trailing-1step-call": lambda: turbo("a cat", num_inference_steps=1, guidance_scale=0.0, seed=1,
+                                                         output_type="np"),
+             "lcm-4step-call": lambda: lcm("a cat", num_inference_steps=4, guidance_scale=8.0, seed=1,
+                                           output_type="np")}
+    for fn in calls.values():  # warm-up: loop graphs, workspaces
+        fn()
+        fn()
+    sync = torch.cuda.synchronize
+    times = {m: [] for m in list(graphs) + list(calls)}
+    sampler = bench.ClockSampler(0)
+    sampler.start()
+    for _ in range(args.rounds):
+        for mode, graph in graphs.items():
+            times[mode].append(bench.timed_replays(graph, args.reps, sync) / n)
+        for mode, fn in calls.items():
+            ms = []
+            for _ in range(args.reps):
+                sync()
+                t0 = time.perf_counter()
+                fn()
+                sync()
+                ms.append((time.perf_counter() - t0) * 1e3)
+            times[mode].append(float(np.median(ms)))
+    clocks = sampler.stop()
+    for mode, ms in times.items():
+        med = float(np.median(ms))
+        rec = {"model": model, "mode": mode, "workload": "512x512, random-init weights, fp16"}
+        if mode in graphs:
+            rec.update(iter_per_s=round(1e3 / med, 2), ms_per_step=round(med, 4),
+                       ms_per_step_rounds=[round(v, 4) for v in ms])
+        else:
+            rec.update(ms_per_call=round(med, 3), ms_per_call_rounds=[round(v, 3) for v in ms])
+        rec.update(card=torch.cuda.get_device_name(dev), power_limit_w=power_limit_w(0), sm_mhz=clocks.get("sm_mhz"),
+                   clock_events=clocks.get("reasons"))
+        print(json.dumps(rec), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
-    ap.add_argument("--model", choices=("sd15", "sd21-base", "sd21"), default="sd15")
+    ap.add_argument("--model", choices=("sd15", "sd21-base", "sd21", "sdxl-base"), default="sd15",
+                    help="sdxl-base: --guidance-free only")
     ap.add_argument("--reps", type=int, default=3, help="replays of the 20-step graph per measurement")
     ap.add_argument("--inpaint", action="store_true", help="SD-1.5: text-to-image vs the two inpainting loops")
-    ap.add_argument("--rounds", type=int, default=5, help="--inpaint: alternated measurements per mode")
+    ap.add_argument("--rounds", type=int, default=5, help="--inpaint / --guidance-free: alternated measurements per mode")
+    ap.add_argument("--guidance-free", action="store_true",
+                    help="--model sd21-base | sdxl-base: the CFG loop against the guidance-free one, Turbo / LCM calls")
     args = ap.parse_args()
+    if args.guidance_free:
+        if args.model not in ("sd21-base", "sdxl-base"):
+            ap.error("--guidance-free runs --model sd21-base or sdxl-base")
+        dev = torch.device("cuda", 0)
+        torch.cuda.set_device(dev)
+        guidance_free_modes(args, dev)
+        return
+    if args.model == "sdxl-base":
+        ap.error("--model sdxl-base runs with --guidance-free only")
     if args.inpaint:
         dev = torch.device("cuda", 0)
         torch.cuda.set_device(dev)
