@@ -310,6 +310,14 @@ int b200sd_upsample2x_s8(const void* in, void* out, int32_t n, int32_t h, int32_
 int b200sd_absmax_f16(const void* x, size_t numel, float* slot, void* stream);
 /* out = a + b (fp16; ControlNet residual injection unet.py:1009-1022) */
 int b200sd_add(const void* a, const void* b, void* out, size_t numel, void* stream);
+/* ControlNet residual injection with per-net conditioning scales, in diffusers' fp16 operation order:
+ *   t = fp16(s_0 * r_0);  t = fp16(t + fp16(s_k * r_k)) for k = 1 .. n_res-1;  out = fp16(skip + t)
+ * res: host array of n_res (1 .. B200SD_MAX_CONTROLNETS) device pointers to fp16 tensors of numel elements; scales:
+ * fp32 device array [n_res], read by the kernel (a captured graph replays with the values current at replay); skip:
+ * fp16 [numel] or NULL (then out = t).  out may alias skip.  At every scale equal to 1.0 the result is b200sd_add's. */
+#define B200SD_MAX_CONTROLNETS 8
+int b200sd_control_inject(const void* skip, const void* const* res, const float* scales, int32_t n_res, void* out,
+                          size_t numel, void* stream);
 /* BC1S fp16/fp32 context (B, D, 1, S) -> token-major fp16 [B*S, D] */
 int b200sd_ctx_to_tokens(const void* in, int32_t in_f32, void* out, int32_t b, int32_t d, int32_t s,
                          void* stream);

@@ -151,6 +151,29 @@ TINY_CONTROLNET = dict(
     conditioning_embedding_out_channels=(16, 32, 96, 256),
 )
 
+# ControlNet for SDXL-base (diffusers/controlnet-canny-sdxl-1.0, controlnet-depth-sdxl-1.0): the encoder half of
+# SDXL_BASE_UNET with its text_time add-embedding; the mid block takes the last level's depth (10), as diffusers'
+# ControlNetModel builds it from transformer_layers_per_block[-1].  9 down residuals + 1 mid residual, the shapes of the
+# SDXL UNet's skip connections.
+SDXL_CONTROLNET = dict(
+    in_channels=4, block_out_channels=(320, 640, 1280), layers_per_block=2,
+    down_block_types=("DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D"),
+    attention_head_dim=(5, 10, 20), cross_attention_dim=2048, norm_num_groups=32, norm_eps=1e-5,
+    flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=(1, 2, 10),
+    addition_embed_type="text_time", addition_time_embed_dim=256, projection_class_embeddings_input_dim=2816,
+    conditioning_embedding_out_channels=(16, 32, 96, 256),
+)
+
+# the encoder half of TINY_XL_UNET (depth-2 mid block)
+TINY_XL_CONTROLNET = dict(
+    in_channels=4, block_out_channels=(64, 128), layers_per_block=2,
+    down_block_types=("DownBlock2D", "CrossAttnDownBlock2D"),
+    attention_head_dim=(1, 2), cross_attention_dim=96, norm_num_groups=32, norm_eps=1e-5,
+    flip_sin_to_cos=True, freq_shift=0, transformer_layers_per_block=(1, 2),
+    addition_embed_type="text_time", addition_time_embed_dim=32, projection_class_embeddings_input_dim=64 + 6 * 32,
+    conditioning_embedding_out_channels=(16, 32, 96, 256),
+)
+
 SD_VAE = dict(latent_channels=4, out_channels=3, block_out_channels=(128, 256, 512, 512),
               layers_per_block=2, norm_num_groups=32, scaling_factor=0.18215)
 
@@ -254,7 +277,9 @@ def unet_param_shapes(cfg) -> "OrderedDict[str, tuple]":
 
 
 def controlnet_param_shapes(cfg) -> "OrderedDict[str, tuple]":
-    """name -> shape for the reference ``ControlNetModel`` (controlnet.py:49-189)."""
+    """name -> shape for the reference ``ControlNetModel`` (controlnet.py:49-189), and for diffusers' ControlNetModel
+    where the reference has no counterpart: the ``add_embedding`` of a ``text_time`` (SDXL) config and a mid block of
+    depth ``transformer_layers_per_block[-1]`` (1 for every SD 1.x / 2.x ControlNet)."""
     sh = OrderedDict()
     boc = list(cfg["block_out_channels"])
     nb = len(boc)
@@ -265,6 +290,9 @@ def controlnet_param_shapes(cfg) -> "OrderedDict[str, tuple]":
     _conv(sh, "conv_in", boc[0], cfg.get("in_channels", 4), 3)
     _conv(sh, "time_embedding.linear_1", temb, boc[0], 1)
     _conv(sh, "time_embedding.linear_2", temb, temb, 1)
+    if cfg.get("addition_embed_type") == "text_time":
+        _conv(sh, "add_embedding.linear_1", temb, cfg["projection_class_embeddings_input_dim"], 1)
+        _conv(sh, "add_embedding.linear_2", temb, temb, 1)
     ce = list(cfg.get("conditioning_embedding_out_channels", (16, 32, 96, 256)))
     _conv(sh, "controlnet_cond_embedding.conv_in", ce[0], 3, 3)
     for i in range(len(ce) - 1):
@@ -288,9 +316,31 @@ def controlnet_param_shapes(cfg) -> "OrderedDict[str, tuple]":
             _conv(sh, f"controlnet_down_blocks.{k}", out, out, 1)
     _conv(sh, "controlnet_mid_block", boc[-1], boc[-1], 1)
     _resnet(sh, "mid_block.resnets.0", boc[-1], boc[-1], temb)
-    _transformer(sh, "mid_block.attentions.0", boc[-1], ctx, 1)  # controlnet.py:168-180: default depth 1
+    _transformer(sh, "mid_block.attentions.0", boc[-1], ctx, depth[-1])
     _resnet(sh, "mid_block.resnets.1", boc[-1], boc[-1], temb)
     return sh
+
+
+def check_controlnet_matches_unet(unet_cfg, controlnet_cfg, which="ControlNet"):
+    """ValueError naming the first field in which a ControlNet cannot drive the UNet: its residuals must have the
+    shapes of the UNet's skip connections (block_out_channels, down_block_types, layers_per_block), it must read the
+    same text states (cross_attention_dim) and the same add-embedding inputs (addition_embed_type and, for text_time,
+    projection_class_embeddings_input_dim).  Pooled-condition ControlNets (global_pool_conditions) are not
+    implemented."""
+    if controlnet_cfg.get("global_pool_conditions"):
+        raise ValueError(f"{which}: global_pool_conditions=True (pooled residuals) is not supported")
+    norm = {"block_out_channels": lambda v: tuple(int(c) for c in v), "down_block_types": lambda v: tuple(v),
+            "layers_per_block": int, "cross_attention_dim": int}
+    defaults = {"layers_per_block": 2, "addition_embed_type": None}
+    fields = ["cross_attention_dim", "block_out_channels", "down_block_types", "layers_per_block", "addition_embed_type"]
+    if unet_cfg.get("addition_embed_type") == "text_time":
+        fields.append("projection_class_embeddings_input_dim")
+    for f in fields:
+        u, c = unet_cfg.get(f, defaults.get(f)), controlnet_cfg.get(f, defaults.get(f))
+        if f in norm and u is not None and c is not None:
+            u, c = norm[f](u), norm[f](c)
+        if u != c:
+            raise ValueError(f"{which} does not match the UNet: {f} is {c!r}, the UNet's is {u!r}")
 
 
 def vae_decoder_param_shapes(cfg) -> "OrderedDict[str, tuple]":

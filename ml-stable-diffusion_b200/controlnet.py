@@ -2,7 +2,9 @@
 8-conv conditioning embedder (reference ``python_coreml_stable_diffusion/controlnet.py:15-250``), with the
 reference's model-call contract (``pipeline.py:259-284``: ``sample, timestep, encoder_hidden_states,
 controlnet_cond`` -> ``additional_residual_i``).  Re-uses ``UNetEngine``'s packed blocks; the conditioning
-embedder's SiLU is fused into the conv epilogue (``act=1``)."""
+embedder's SiLU is fused into the conv epilogue (``act=1``).  An SDXL ControlNet (``addition_embed_type="text_time"``,
+config.SDXL_CONTROLNET) adds the UNet's ``add_embedding`` of ``time_ids`` / ``text_embeds`` to its time embedding, as
+diffusers' ControlNetModel does; the reference's ControlNetModel has no such input."""
 from __future__ import annotations
 
 import numpy as np
@@ -20,8 +22,9 @@ class ControlNetEngine(UNetEngine):
         # the encoder half is built by the UNet packer: give it no up path and no output head
         self._ce_channels = list(cfg.get("conditioning_embedding_out_channels", (16, 32, 96, 256)))
         self._full_sd = state_dict
-        # mid block transformer depth is 1 regardless of transformer_layers_per_block (controlnet.py:168-180)
-        ucfg = dict(cfg, up_block_types=(), out_channels=cfg.get("in_channels", 4), mid_block_transformer_layers=1)
+        # the mid block's transformer depth is transformer_layers_per_block[-1] (diffusers' ControlNetModel): 1 for every
+        # SD 1.x / 2.x ControlNet, 10 for SDXL's
+        ucfg = dict(cfg, up_block_types=(), out_channels=cfg.get("in_channels", 4))
         super().__init__(ucfg, state_dict, device)
 
     def _pack(self, sd):
@@ -60,13 +63,15 @@ class ControlNetEngine(UNetEngine):
             x = L.conv3x3(x, e["w"], e["b"], stride=e["stride"], act=e["act"])
         return x
 
-    def forward(self, sample, timesteps, ctx_tokens, s_ctx, cond_nhwc, temb_all=None, kv_all=None, emb=None):
-        """Returns the list of NHWC fp16 residuals: 12 (or fewer) down residuals + the mid residual.
+    def forward(self, sample, timesteps, ctx_tokens, s_ctx, cond_nhwc, temb_all=None, kv_all=None, emb=None,
+                time_ids=None, text_embeds=None):
+        """Returns the list of NHWC fp16 residuals: 12 (SDXL: 9, or fewer) down residuals + the mid residual.
         temb_all / kv_all / emb: precomputed time-embedding biases, cross-attention K/V and conditioning embedding
-        (constant over a denoising loop: the pipeline's per-prompt prologue)."""
+        (constant over a denoising loop: the pipeline's per-prompt prologue).  time_ids / text_embeds: the add-embedding
+        inputs of a text_time ControlNet, the rows the UNet gets."""
         batch = sample.shape[0]
         if temb_all is None:
-            temb_all = self.time_embedding(timesteps)
+            temb_all = self.time_embedding(timesteps, time_ids, text_embeds)
         if kv_all is None:
             kv_all = self.kv_project(ctx_tokens)
         e = self.embed_condition(cond_nhwc) if emb is None else emb
@@ -116,8 +121,9 @@ class ControlNetEngine(UNetEngine):
 
 
 class ControlNetModel(B200Model):
-    """``controlnet(sample, timestep, encoder_hidden_states, controlnet_cond) -> {"additional_residual_i": ...}``
-    (pipeline.py:259-284, torch2coreml.py:1382-1412)."""
+    """``controlnet(sample, timestep, encoder_hidden_states[, time_ids, text_embeds], controlnet_cond) ->
+    {"additional_residual_i": ...}`` (pipeline.py:259-284, torch2coreml.py:1382-1412).  ``time_ids`` / ``text_embeds``
+    (named and shaped as on UNetModel): text_time (SDXL) ControlNets only."""
 
     def __init__(self, cfg, state_dict, batch=2, height=64, width=64, seq_len=77, device="cuda", io_dtype=np.float16,
                  use_cuda_graph=True):
@@ -135,12 +141,20 @@ class ControlNetModel(B200Model):
             "encoder_hidden_states": {"shape": (batch, cfg["cross_attention_dim"], 1, seq_len), "dtype": dt},
             "controlnet_cond": {"shape": (batch, 3, height * 8, width * 8), "dtype": dt},
         }
+        if e.xl:
+            nid = int(cfg.get("num_time_ids", 6))
+            spec["time_ids"] = {"shape": (batch, nid), "dtype": dt}
+            spec["text_embeds"] = {"shape": (batch, cfg["projection_class_embeddings_input_dim"]
+                                             - nid * cfg["addition_time_embed_dim"]), "dtype": dt}
         super().__init__(spec, device)
         dev = self.device
         self._sample = torch.zeros(spec["sample"]["shape"], dtype=torch.float32, device=dev)
         self._t = torch.zeros(batch, dtype=torch.float32, device=dev)
         self._ctx = torch.zeros(spec["encoder_hidden_states"]["shape"], dtype=torch.float16, device=dev)
         self._cond = torch.zeros(spec["controlnet_cond"]["shape"], dtype=torch.float16, device=dev)
+        self._time_ids = torch.zeros(spec["time_ids"]["shape"], dtype=torch.float32, device=dev) if e.xl else None
+        self._text_embeds = (torch.zeros(spec["text_embeds"]["shape"], dtype=torch.float32, device=dev) if e.xl
+                             else None)
         self._kv_all = (torch.zeros(batch * seq_len, e.kv_total, dtype=torch.float16, device=dev)
                         if e.kv_w is not None else None)
         self._emb = None     # conditioning embedding of `_cond` (device loop prologue)
@@ -150,16 +164,21 @@ class ControlNetModel(B200Model):
     def prepare_prompt(self, ts_rows, rows=None):
         """Everything that does not change over a denoising loop: cross-attention K/V from `_ctx`, the embedding of
         the conditioning image `_cond` (the reference recomputes it every step, pipeline.py:516-522), the
-        time-embedding biases of all steps.  ``rows``: the first ``rows`` images only (the guidance-free loop);
-        ``ts_rows`` then holds ``rows`` entries per step."""
+        time-embedding biases of all steps (a text_time ControlNet: with the add-embedding of `_time_ids` /
+        `_text_embeds`).  ``rows``: the first ``rows`` images only (the guidance-free loop); ``ts_rows`` then holds
+        ``rows`` entries per step."""
         e, b = self.engine, rows or self.batch
         if self._kv_all is not None:
             e.kv_project(L.ctx_to_tokens(self._ctx[:b]), out=self._kv_all[:b * self.seq])
         self._emb = e.embed_condition(L.nchw_to_nhwc(self._cond[:b], c_pad=8))
         n_steps = ts_rows.shape[0] // b
         per = max(1, 32 // b)
-        parts = [e.time_embedding(ts_rows[s0 * b:(s0 + min(per, n_steps - s0)) * b].contiguous())
-                 for s0 in range(0, n_steps, per)]
+        parts = []
+        for s0 in range(0, n_steps, per):
+            k = min(per, n_steps - s0)
+            tid = self._time_ids[:b].repeat(k, 1) if e.xl else None
+            te = self._text_embeds[:b].repeat(k, 1) if e.xl else None
+            parts.append(e.time_embedding(ts_rows[s0 * b:(s0 + k) * b].contiguous(), tid, te))
         self._table = torch.cat(parts, 0).reshape(n_steps, b, -1)
 
     def run_core(self, x_nhwc, step):
@@ -175,7 +194,9 @@ class ControlNetModel(B200Model):
         x = L.nchw_to_nhwc(self._sample[:r], c_pad=e.in_pad)
         ctx = L.ctx_to_tokens(self._ctx[:r])
         cond = L.nchw_to_nhwc(self._cond[:r], c_pad=8)
-        return e.forward(x, self._t[:r], ctx, self.seq, cond)
+        tid = self._time_ids[:r] if e.xl else None
+        te = self._text_embeds[:r] if e.xl else None
+        return e.forward(x, self._t[:r], ctx, self.seq, cond, time_ids=tid, text_embeds=te)
 
     def forward_device(self, rows=None):
         """Static input buffers -> list of NHWC fp16 residuals.  With CUDA graphs the list is a set of static
@@ -209,6 +230,9 @@ class ControlNetModel(B200Model):
         self._to_device(kwargs["timestep"], self._t)
         self._to_device(kwargs["encoder_hidden_states"], self._ctx)
         self._to_device(kwargs["controlnet_cond"], self._cond)
+        if self.engine.xl:
+            self._to_device(kwargs["time_ids"], self._time_ids)
+            self._to_device(kwargs["text_embeds"], self._text_embeds)
         outs = self.forward_device()
         res = {}
         for i, o in enumerate(outs):

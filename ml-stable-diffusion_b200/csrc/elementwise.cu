@@ -168,6 +168,67 @@ __global__ void add_kernel(const __half2* __restrict__ a, const __half2* __restr
     }
 }
 
+// ---- ControlNet residual injection: out = skip + sum_k scales[k] * res[k] ------------------------------------------
+// diffusers' fp16 operation order (ControlNetModel's conditioning_scale, MultiControlNetModel's sum, the UNet's add):
+// t = fp16(s_0 r_0), t = fp16(t + fp16(s_k r_k)) for each following net, out = fp16(skip + t).  Each product and sum
+// is computed in fp32 and rounded to fp16, as torch does for an fp16 tensor op.  At s = 1 the product is exact, so one
+// net gives fp16(skip + r_0) and two give fp16(skip + fp16(r_0 + r_1)): b200sd_add's bits.  The scales are read from
+// device memory, so a captured graph sees new values on replay.  skip == nullptr: out = t.
+struct ControlResiduals {
+    const __half* r[B200SD_MAX_CONTROLNETS];
+};
+
+__device__ __forceinline__ float control_inject_one(const __half* skip, const ControlResiduals& res, const float* s,
+                                                    int n_res, size_t i) {
+    float t = __half2float(__float2half_rn(s[0] * __half2float(res.r[0][i])));
+    for (int k = 1; k < n_res; ++k)
+        t = __half2float(__float2half_rn(t + __half2float(__float2half_rn(s[k] * __half2float(res.r[k][i])))));
+    if (skip) t = __half2float(__float2half_rn(__half2float(skip[i]) + t));
+    return t;
+}
+
+// vec: every pointer is 16-byte aligned, so numel / 8 groups of eight go through 16-byte loads and stores; the tail
+// (and everything when vec is 0) is done one element per thread
+__global__ void control_inject_kernel(const __half* skip, ControlResiduals res, const float* __restrict__ scales,
+                                      int n_res, __half* out, size_t numel, int vec) {
+    pdl_trigger();  // no large shared memory here: dependents may start their prologue at once
+    pdl_wait();
+    float s[B200SD_MAX_CONTROLNETS];
+#pragma unroll
+    for (int k = 0; k < B200SD_MAX_CONTROLNETS; ++k) s[k] = k < n_res ? scales[k] : 0.f;
+    const size_t n8 = vec ? numel / 8 : 0;
+    const size_t tid = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+    const size_t step = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t v = tid; v < n8; v += step) {
+        float t[8];
+        {
+            const uint4 a = reinterpret_cast<const uint4*>(res.r[0])[v];
+            const __half* h = reinterpret_cast<const __half*>(&a);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) t[j] = __half2float(__float2half_rn(s[0] * __half2float(h[j])));
+        }
+        for (int k = 1; k < n_res; ++k) {
+            const uint4 a = reinterpret_cast<const uint4*>(res.r[k])[v];
+            const __half* h = reinterpret_cast<const __half*>(&a);
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                t[j] = __half2float(__float2half_rn(t[j] + __half2float(__float2half_rn(s[k] * __half2float(h[j])))));
+        }
+        if (skip) {
+            const uint4 a = reinterpret_cast<const uint4*>(skip)[v];
+            const __half* h = reinterpret_cast<const __half*>(&a);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) t[j] = __half2float(h[j]) + t[j];
+        }
+        uint4 o;
+        __half* oh = reinterpret_cast<__half*>(&o);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) oh[j] = __float2half_rn(t[j]);
+        reinterpret_cast<uint4*>(out)[v] = o;
+    }
+    for (size_t i = n8 * 8 + tid; i < numel; i += step) out[i] = __float2half_rn(control_inject_one(skip, res, s, n_res, i));
+}
+
 // ---- small-M linear: one warp per output column, all M rows at once (M <= 8) -------------------
 // The (optionally SiLU-activated) input rows are staged in shared memory ONCE per block -- every column warp used to
 // re-read and re-activate them (the 20 800-column time-embedding projection was MUFU-bound on 20 800 redundant SiLU
@@ -549,6 +610,29 @@ extern "C" int b200sd_add(const void* a, const void* b, void* out, size_t numel,
     B200SD_CHECK_CUDA(launch_kernel(add_kernel, dim3(grid_for(numel / 2, 256)), dim3(256), 0, stream, reinterpret_cast<const __half2*>(a),
                                                              reinterpret_cast<const __half2*>(b),
                                                              reinterpret_cast<__half2*>(out), numel / 2));
+    B200SD_CHECK_CUDA(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+extern "C" int b200sd_control_inject(const void* skip, const void* const* res, const float* scales, int32_t n_res,
+                                     void* out, size_t numel, void* stream_) {
+    if (!b200sd::launch_class_enabled(8)) return 0;  // bench.py's per-class timing graphs
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    B200SD_REQUIRE(res && scales && out && numel > 0, "b200sd_control_inject: null pointer or empty tensor");
+    B200SD_REQUIRE(n_res >= 1 && n_res <= B200SD_MAX_CONTROLNETS, "b200sd_control_inject: n_res=%d must be in [1, %d]",
+                   n_res, B200SD_MAX_CONTROLNETS);
+    ControlResiduals r{};
+    bool aligned = reinterpret_cast<uintptr_t>(out) % 16 == 0 && reinterpret_cast<uintptr_t>(skip) % 16 == 0;
+    for (int k = 0; k < n_res; ++k) {
+        B200SD_REQUIRE(res[k], "b200sd_control_inject: res[%d] is null", k);
+        r.r[k] = static_cast<const __half*>(res[k]);
+        aligned = aligned && reinterpret_cast<uintptr_t>(res[k]) % 16 == 0;
+    }
+    const size_t work = aligned ? numel / 8 + numel % 8 : numel;
+    B200SD_CHECK_CUDA(launch_kernel(control_inject_kernel, dim3(grid_for(work, 256)), dim3(256), 0, stream,
+                                    static_cast<const __half*>(skip), r, scales, static_cast<int>(n_res),
+                                    static_cast<__half*>(out), numel, static_cast<int>(aligned)));
     B200SD_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return 0;

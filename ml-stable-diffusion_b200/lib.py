@@ -111,6 +111,8 @@ _SIGNATURES = {
     "b200sd_upsample2x": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p]),
     "b200sd_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200sd_control_inject": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p,
+                                        C.c_size_t, C.c_void_p]),
     # W8A8 (int8 wgmma) 3x3 convolution and its operand producers
     "b200sd_gemm_s8": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p, C.c_void_p]),
     "b200sd_gemm_lut": (C.c_int, [C.POINTER(GemmArgs), C.POINTER(LutArgs), C.c_void_p]),
@@ -987,6 +989,34 @@ def add(a, b, out=None):
     if out is None:
         out = torch.empty_like(a)
     _check(load().b200sd_add(_ptr(a), _ptr(b), _ptr(out), a.numel(), _stream()), "b200sd_add")
+    return out
+
+
+MAX_CONTROLNETS = 8  # B200SD_MAX_CONTROLNETS
+
+
+def control_inject(skip, residuals, scales, out=None):
+    """ControlNet residual injection, one launch whatever the number of nets: out = fp16(skip + t) with
+    t = fp16(s_0 r_0), t = fp16(t + fp16(s_k r_k)) -- diffusers' fp16 order for conditioning_scale, several ControlNets
+    and the UNet's add.  ``skip`` None: out = t.  ``residuals``: fp16 tensors shaped like ``skip``; ``scales``: fp32 CUDA
+    tensor [len(residuals)], read by the kernel, so a captured graph replays with the values it holds then."""
+    n = len(residuals)
+    if not 1 <= n <= MAX_CONTROLNETS:
+        raise B200SDError(f"control_inject: {n} residuals, at most {MAX_CONTROLNETS}")
+    ref = residuals[0] if skip is None else skip
+    _req(ref, torch.float16, "control_inject skip")
+    for r in residuals:
+        _req(r, torch.float16, "control_inject residual")
+        if r.shape != ref.shape:
+            raise B200SDError(f"control_inject: residual of shape {tuple(r.shape)}, expected {tuple(ref.shape)}")
+    _req(scales, torch.float32, "control_inject scales")
+    if scales.numel() < n:
+        raise B200SDError(f"control_inject: {scales.numel()} scales for {n} residuals")
+    if out is None:
+        out = torch.empty_like(ref)
+    ptrs = (C.c_void_p * n)(*[r.data_ptr() for r in residuals])
+    _check(load().b200sd_control_inject(_ptr(skip), ptrs, _ptr(scales), n, _ptr(out), ref.numel(), _stream()),
+           "b200sd_control_inject")
     return out
 
 

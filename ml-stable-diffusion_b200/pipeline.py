@@ -27,6 +27,7 @@ from . import config as C
 from . import lib as L
 from . import scheduler as S
 from .model import UNetModel
+from .unet import ControlResiduals
 from .vae import VAEDecoderModel
 
 
@@ -42,6 +43,40 @@ def vae_dtype(unet_cfg: dict, vae_cfg: dict):
 
 #: the schedulers whose truncated schedule (inpainting at strength < 1) diffusers 0.30.2 runs as ``plan(start)``
 INPAINT_STRENGTH_SCHEDULERS = ("DDIM", "DPMSolverMultistep")
+
+
+def _per_net(value, n_nets, name):
+    """A float, or one per ControlNet -> list of n_nets floats (ValueError naming ``name`` on a wrong length)."""
+    vals = list(value) if isinstance(value, (list, tuple, np.ndarray)) else [value] * n_nets
+    if len(vals) != n_nets:
+        raise ValueError(f"{name} has {len(vals)} values for {n_nets} ControlNet(s)")
+    return [float(v) for v in vals]
+
+
+def controlnet_arguments(n_nets, controlnet_conditioning_scale=1.0, control_guidance_start=0.0,
+                         control_guidance_end=1.0, guess_mode=False):
+    """Checks the ControlNet arguments of ``__call__`` as diffusers' check_inputs does -> (scales, starts, ends), one
+    float per net.  Scales must be finite; every window must satisfy 0 <= start < end <= 1.  guess_mode is not
+    implemented."""
+    if guess_mode:
+        raise ValueError("guess_mode=True is not implemented")
+    scales = _per_net(controlnet_conditioning_scale, n_nets, "controlnet_conditioning_scale")
+    if not all(np.isfinite(scales)):
+        raise ValueError(f"controlnet_conditioning_scale must be finite, got {scales}")
+    starts = _per_net(control_guidance_start, n_nets, "control_guidance_start")
+    ends = _per_net(control_guidance_end, n_nets, "control_guidance_end")
+    for s, e in zip(starts, ends):
+        if not (0.0 <= s < e <= 1.0):
+            raise ValueError(f"control_guidance_start / control_guidance_end: need 0 <= start < end <= 1, got start={s} "
+                             f"end={e}")
+    return scales, starts, ends
+
+
+def controlnet_keep(n_steps, starts, ends):
+    """diffusers' controlnet_keep over the ``n_steps`` executed steps (after an image-to-image start): net k runs at
+    step i unless i / n_steps < start_k or (i + 1) / n_steps > end_k.  -> per step, the tuple of the nets that run."""
+    return [tuple(k for k, (s, e) in enumerate(zip(starts, ends)) if not (i / n_steps < s or (i + 1) / n_steps > e))
+            for i in range(n_steps)]
 
 
 def prepare_mask_and_masked_image(image, mask):
@@ -140,6 +175,18 @@ class B200StableDiffusionPipeline:
         self.controlnet = list(controlnet) if controlnet else None  # pipeline.py:66,106: Optional[List[model]]
         if self.controlnet and not unet.engine.support_controlnet:
             raise ValueError("the UNet was not built with support_controlnet=True (no additional_residual inputs)")
+        if self.controlnet:
+            if unet_refiner is not None:
+                raise ValueError("ControlNet cannot be combined with the SDXL refiner")
+            if len(self.controlnet) > L.MAX_CONTROLNETS:
+                raise ValueError(f"at most {L.MAX_CONTROLNETS} ControlNets, got {len(self.controlnet)}")
+            for k, net in enumerate(self.controlnet):
+                C.check_controlnet_matches_unet(unet.engine.cfg, net.engine.cfg, f"ControlNet {k}")
+            # conditioning scales on the device, one fp32 array per set of nets that runs at some step (the loop graph
+            # reads them, so a new scale replays the same graph); the set of all nets exists from the start
+            self._all_nets = tuple(range(len(self.controlnet)))
+            self._control_scale_bufs = {self._all_nets: torch.ones(len(self.controlnet), dtype=torch.float32,
+                                                                   device=unet.device)}
         self.vae_decoder = vae_decoder
         self.scheduler_name = scheduler
         # this class mirrors the reference's PYTHON pipeline, whose DPM-Solver++ is diffusers 0.30.2
@@ -289,7 +336,16 @@ class B200StableDiffusionPipeline:
 
         ucfg = K.read_config(model_dir, "unet")
         vcfg = K.read_config(model_dir, "vae")
+        ccfgs = []
         if controlnet_dirs:
+            if refiner_dir:
+                raise ValueError("ControlNet cannot be combined with the SDXL refiner")
+            for k, d in enumerate(controlnet_dirs):  # checked before any weights are read
+                with open(os.path.join(d, "config.json")) as fh:
+                    ccfg = {k2: (tuple(v) if isinstance(v, list) else v) for k2, v in json.load(fh).items()
+                            if not k2.startswith("_")}
+                C.check_controlnet_matches_unet(ucfg, ccfg, f"ControlNet {k} ({d})")
+                ccfgs.append(ccfg)
             ucfg = dict(ucfg, support_controlnet=True)
         f = 2 ** (len(vcfg["block_out_channels"]) - 1)
         size = ucfg.get("sample_size", 64)
@@ -352,9 +408,7 @@ class B200StableDiffusionPipeline:
         if controlnet_dirs:
             from .controlnet import ControlNetModel
             nets = []
-            for d in controlnet_dirs:
-                with open(os.path.join(d, "config.json")) as fh:
-                    ccfg = {k: (tuple(v) if isinstance(v, list) else v) for k, v in json.load(fh).items() if not k.startswith("_")}
+            for d, ccfg in zip(controlnet_dirs, ccfgs):
                 nets.append(ControlNetModel(ccfg, K.load_component(d, "controlnet", ccfg), batch=2 * images_per_call,
                                             height=h, width=w, device=device))
         refiner = None
@@ -491,25 +545,32 @@ class B200StableDiffusionPipeline:
             out.append(cond)
         return out
 
-    def run_controlnet(self, sample, timestep, encoder_hidden_states, controlnet_cond):
-        """pipeline.py:259-284 on the device: every ControlNet sees the same UNet inputs; their residuals are
-        summed (fp16, like the reference's in-place numpy add).  Returns NCHW views of NHWC fp16 tensors."""
+    def run_controlnet(self, sample, timestep, encoder_hidden_states, controlnet_cond, nets=None, time_ids=None,
+                       text_embeds=None):
+        """pipeline.py:259-284 on the device: every ControlNet in ``nets`` (indices; default all) sees the same UNet
+        inputs (``time_ids`` / ``text_embeds``: those of an SDXL UNet); their residuals are scaled and summed in
+        diffusers' fp16 order (one launch per residual, the scales of ``_control_scale_bufs[nets]``).  Returns NCHW
+        views of NHWC fp16 tensors, or None when ``nets`` is empty."""
         if not self.controlnet:
             raise ValueError("Conditions for controlnet are given but the pipeline has no controlnet modules")
-        total = None
+        nets = self._all_nets if nets is None else tuple(nets)
+        if not nets:
+            return None
         r = sample.shape[0]  # the batch, or its first half in the guidance-free loop
-        for module, cond in zip(self.controlnet, controlnet_cond):
+        outs = []
+        for k in nets:
+            module, cond = self.controlnet[k], controlnet_cond[k]
             module._sample[:r].copy_(sample)
             module._t[:r].copy_(timestep)
             module._ctx[:r].copy_(encoder_hidden_states)
             module._cond[:r].copy_(cond)
-            outs = module.forward_device(r)
-            if total is None:
-                total = list(outs)
-            else:
-                for acc, o in zip(total, outs):
-                    L.add(acc, o, out=acc)
-        return [r.permute(0, 3, 1, 2) for r in total]
+            if module.engine.xl:
+                module._time_ids[:r].copy_(torch.as_tensor(time_ids).reshape(r, -1))
+                module._text_embeds[:r].copy_(torch.as_tensor(text_embeds))
+            outs.append(module.forward_device(r))
+        scales = self._control_scale_bufs[nets]
+        total = [L.control_inject(None, [o[i] for o in outs], scales) for i in range(len(outs[0]))]
+        return [t.permute(0, 3, 1, 2) for t in total]
 
     @staticmethod
     def numpy_to_pil(images):
@@ -549,6 +610,8 @@ class B200StableDiffusionPipeline:
         # which UNet runs each step: the SDXL refiner takes over at refiner_start_step with its own conditioning
         # (StableDiffusionXLPipeline.swift:205-225); each model gets its per-prompt prologue and its own time table
         models = [self.unet if i < rs else self.unet_refiner for i in range(len(plan))]
+        # use_controlnet: False, or per step the tuple of ControlNets that run (controlnet_keep)
+        keep = use_controlnet if isinstance(use_controlnet, (list, tuple)) else [None] * len(plan)
         self._hist.zero_()
         tables = {}
         for m, lo, hi in ((self.unet, 0, rs), (self.unet_refiner, rs, len(plan))):
@@ -568,7 +631,8 @@ class B200StableDiffusionPipeline:
         for i, st in enumerate(plan):
             u = models[i]
             table, lo = tables[id(u)]
-            u._run_core(table[i - lo], self.controlnet_residuals(i, rows=rows) if use_controlnet else None, rows)
+            u._run_core(table[i - lo], self.controlnet_residuals(i, rows=rows, nets=keep[i]) if use_controlnet else None,
+                        rows)
             k = self._coeffs(st, guidance_scale)
             k.noise_pred_nhwc = 1
             nxt = models[i + 1] if i + 1 < len(plan) else u
@@ -642,6 +706,18 @@ class B200StableDiffusionPipeline:
             b["unet_in"][:, c:c + 1].copy_(mask)
             b["unet_in"][:, c + 1:].copy_(as_dev(inp.masked_image_latents, (n, self.unet.in_channels - c - 1, h, w)))
 
+    def set_control_scales(self, scales, keep=None):
+        """Write the conditioning scales (one float per net) into the device arrays the loop reads: one per set of
+        nets in ``keep`` (per-step tuples, controlnet_keep), allocated on first use, and the set of all nets."""
+        sets = {self._all_nets} | set(keep or ())
+        for nets in sets:
+            if not nets:
+                continue
+            buf = self._control_scale_bufs.get(nets)
+            if buf is None:
+                buf = self._control_scale_bufs[nets] = torch.empty(len(nets), dtype=torch.float32, device=self.device)
+            buf.copy_(torch.tensor([scales[k] for k in nets], dtype=torch.float32))
+
     def set_control_conditions(self, controlnet_cond):
         """Copy the conditioning images (each (2B, 3, H, W)) into the ControlNets' static input buffers."""
         for module, cond in zip(self.controlnet, controlnet_cond):
@@ -653,19 +729,20 @@ class B200StableDiffusionPipeline:
         buffer `_cond`), time-embedding table (of the first ``rows`` images: the guidance-free loop)."""
         for module in self.controlnet:
             module._ctx.copy_(self.unet._ctx)
+            if module.engine.xl:  # the add-embedding rows the UNet gets (the negative pooled embedding on uncond rows)
+                module._time_ids.copy_(self.unet._time_ids)
+                module._text_embeds.copy_(self.unet._text_embeds)
             module.prepare_prompt(ts_rows, rows)
 
-    def controlnet_residuals(self, step, _temb=None, rows=None):
-        """pipeline.py:259-284 inside the device loop: every ControlNet sees the UNet's input; residuals are summed."""
-        total = None
+    def controlnet_residuals(self, step, _temb=None, rows=None, nets=None):
+        """pipeline.py:259-284 inside the device loop: the ControlNets ``nets`` (indices; default all) see the UNet's
+        input.  -> ControlResiduals for the UNet, which scales and sums them as it injects them, or None when ``nets``
+        is empty."""
+        nets = self._all_nets if nets is None else tuple(nets)
+        if not nets:
+            return None
         x = self.unet._x_nhwc if rows is None else self.unet._x_nhwc[:rows]
-        for module in self.controlnet:
-            outs = module.run_core(x, step)
-            if total is None:
-                total = list(outs)
-            else:
-                total = [L.add(acc, o) for acc, o in zip(total, outs)]
-        return total
+        return ControlResiduals([self.controlnet[k].run_core(x, step) for k in nets], self._control_scale_bufs[nets])
 
     def _ts_rows(self, plan, rows=None):
         return torch.tensor([float(st.timestep) for st in plan for _ in range(rows or self.unet.batch)],
@@ -681,7 +758,9 @@ class B200StableDiffusionPipeline:
             s = torch.cuda.Stream(device=self.device)  # eager warm-up off the capture: workspaces, weight tiling
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._loop_on_static_buffers(plan[:1], guidance_scale, ts_rows[:rows], use_controlnet,
+                # every ControlNet runs in the warm-up step, whichever steps it is kept at
+                self._loop_on_static_buffers(plan[:1], guidance_scale, ts_rows[:rows],
+                                             [self._all_nets] if use_controlnet else False,
                                              inpaint=inpaint, blend=blend[:1] if blend else None, guided=guided)
                 if refiner_start_step is not None and refiner_start_step < len(plan):  # warm the refiner's kernels too
                     self._loop_on_static_buffers(plan[-1:], guidance_scale, ts_rows[-rows:], use_controlnet, 0)
@@ -702,7 +781,7 @@ class B200StableDiffusionPipeline:
     def denoise(self, text_embeddings, latents, num_inference_steps, guidance_scale, callback=None,
                 callback_steps=1, time_ids=None, text_embeds=None, return_denoised=False, record=None,
                 controlnet_cond=None, start_step=0, refiner=None, refiner_start=0.8, noise_key=None, noise_offset=0,
-                inpaint=None):
+                inpaint=None, controlnet_conditioning_scale=1.0, control_guidance_start=0.0, control_guidance_end=1.0):
         """Runs the N-step loop (from ``start_step``: image-to-image) entirely on the device.  ``text_embeddings`` (2B, D, 1, S) and ``latents``
         (B, C, h, w) may be numpy (copied once, before the loop) or CUDA tensors.  ``record`` (a list) receives
         (timestep, noise_pred, latents_after_step) clones per step -- a debugging / testing aid.  Without
@@ -716,6 +795,10 @@ class B200StableDiffusionPipeline:
         ``inpaint`` (``InpaintInputs``): the latent mask and image latents of an inpainting call (``__call__`` with
         ``mask_image``); required for a 9-channel UNet.  They are copied into static buffers before the loop, so the
         loop graph depends on the inpainting kind only, never on the mask or the images.
+        ``controlnet_conditioning_scale`` / ``control_guidance_start`` / ``control_guidance_end``: a float or one per
+        ControlNet (controlnet_arguments); net k runs at the steps controlnet_keep gives and is not launched at the
+        others.  The loop graph is keyed by those per-step sets of nets, not by the scales, which it reads on the
+        device.
 
         Without classifier-free guidance (``do_classifier_free_guidance``: guidance_scale <= 1, or a guidance-embedding
         UNet) the loop runs guidance-free: the UNet (still built at batch 2B) and the ControlNets run on B rows only.
@@ -760,7 +843,14 @@ class B200StableDiffusionPipeline:
         def x_space(i):  # latents after i steps, in x-space
             s = sched.input_scale(i)
             return self._latents if s == 1.0 else self._latents * s
+        keep = None
         if controlnet_cond:
+            if len(controlnet_cond) != len(self.controlnet):
+                raise ValueError(f"{len(controlnet_cond)} conditioning images for {len(self.controlnet)} ControlNet(s)")
+            scales, starts, ends = controlnet_arguments(len(self.controlnet), controlnet_conditioning_scale,
+                                                        control_guidance_start, control_guidance_end)
+            keep = controlnet_keep(len(plan), starts, ends)
+            self.set_control_scales(scales, keep)
             controlnet_cond = [torch.as_tensor(c).to(self.device, torch.float16) for c in controlnet_cond]
             if not guided:  # the condition images of the B prompt rows (prepare_control_cond doubles them)
                 controlnet_cond = [c[-n:] for c in controlnet_cond]
@@ -787,9 +877,9 @@ class B200StableDiffusionPipeline:
                 r._text_embeds.copy_(torch.as_tensor(refiner["text_embeds"]))
                 rstep = int(np.float32(len(plan)) * np.float32(refiner_start))  # Int(Float(timeSteps.count) * refinerStart)
             key = (self.scheduler_name, int(num_inference_steps), float(guidance_scale), int(start_step),
-                   bool(controlnet_cond), tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base, guided,
-                   kind)
-            self._loop_graph_for(key, plan, guidance_scale, bool(controlnet_cond), rstep, kind, blend, guided).replay()
+                   tuple(keep) if keep else None, tuple(sorted(self.scheduler_kwargs.items())), rstep, self._noise_base,
+                   guided, kind)
+            self._loop_graph_for(key, plan, guidance_scale, keep or False, rstep, kind, blend, guided).replay()
             return self._denoised if return_denoised else self._latents
         if refiner is not None:
             raise ValueError("the refiner hand-off runs in the device loop only (no callback / record)")
@@ -804,7 +894,11 @@ class B200StableDiffusionPipeline:
             sample = torch.cat([x_in, x_in], 0) if guided else x_in  # pipeline.py:502
             residuals = None
             if controlnet_cond:  # pipeline.py:515-529
-                residuals = self.run_controlnet(sample, self._t[:rows], self._ctx[:rows], controlnet_cond)
+                residuals = self.run_controlnet(sample, self._t[:rows], self._ctx[:rows], controlnet_cond, keep[i],
+                                                time_ids, text_embeds)
+                if residuals is None:  # no net runs at this step: nothing is injected
+                    for buf in self.unet._res:
+                        buf[:rows].zero_()
             noise_pred = self.unet.forward_device(sample, self._t[:rows], self._ctx[:rows], time_ids, text_embeds,
                                                   residuals, self.unet._cond[:rows] if self.unet._cond is not None
                                                   else None)
@@ -875,7 +969,8 @@ class B200StableDiffusionPipeline:
                  original_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
                  target_size: Optional[Tuple[int, int]] = None, unet_batch_one=False, prompt_embeds=None,
                  starting_image=None, strength=None, seed=None, rng="numpy", refiner_start=0.8, aesthetic_score=6.0,
-                 negative_aesthetic_score=2.5, mask_image=None, **kwargs):
+                 negative_aesthetic_score=2.5, mask_image=None, controlnet_conditioning_scale=1.0,
+                 control_guidance_start=0.0, control_guidance_end=1.0, guess_mode=False, **kwargs):
         """``starting_image`` ((B, 3, H, W) in [-1, 1], the vae_encoder input) + ``strength`` (default 0.5) select the
         Swift pipeline's image-to-image mode (StableDiffusionPipeline.swift:250-262, 361-378): the encoded image is
         noised to timestep ``timeSteps[startStep]`` and only the remaining steps run.
@@ -886,8 +981,15 @@ class B200StableDiffusionPipeline:
         4-channel UNet keeps the unmasked region by blending the noised image latents back in after every step, so
         the unmasked latents end exactly on the image latents.  Draws from the global numpy stream, after the latent
         noise: the encoder noise of the full image (4-channel UNet, or strength < 1), then that of the masked image
-        (9-channel UNet)."""
+        (9-channel UNet).
+
+        ControlNet (``controlnet_cond``: one (3, H, W) image per net), as diffusers' ControlNet pipelines:
+        ``controlnet_conditioning_scale`` multiplies each net's residuals (a float or one per net; SDXL ControlNets are
+        usually run at 0.5), and net k runs only at the steps inside its window [``control_guidance_start``,
+        ``control_guidance_end``] (fractions of the executed steps).  ``guess_mode`` is not implemented."""
         self.check_inputs(prompt, height, width, callback_steps)
+        if guess_mode:
+            raise ValueError("guess_mode=True is not implemented")
         height = height or self.height
         width = width or self.width
         if (height, width) != (self.height, self.width):
@@ -896,6 +998,9 @@ class B200StableDiffusionPipeline:
             raise ValueError("only eta = 0 (deterministic DDIM) is implemented")
         if controlnet_cond and not self.controlnet:
             raise ValueError("Conditions for controlnet are given but the pipeline has no controlnet modules")
+        if controlnet_cond:
+            controlnet_arguments(len(self.controlnet), controlnet_conditioning_scale, control_guidance_start,
+                                 control_guidance_end)
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
         prompts = [p for p in prompts for _ in range(num_images_per_prompt)]
         if len(prompts) != self.images_per_call:
@@ -1007,7 +1112,9 @@ class B200StableDiffusionPipeline:
         final = self.denoise(text_embeddings, lat, num_inference_steps, guidance_scale, callback, callback_steps,
                              time_ids, text_embeds, controlnet_cond=controlnet_cond or None, start_step=start_step,
                              refiner=refiner, refiner_start=refiner_start, noise_key=noise_key,
-                             noise_offset=noise_offset, inpaint=inpaint)
+                             noise_offset=noise_offset, inpaint=inpaint,
+                             controlnet_conditioning_scale=controlnet_conditioning_scale,
+                             control_guidance_start=control_guidance_start, control_guidance_end=control_guidance_end)
         image, has_nsfw = self.decode_and_check(final)  # the only device->host copies of the result
         if output_type == "pil":
             image = self.numpy_to_pil(image)

@@ -21,6 +21,7 @@ from __future__ import annotations
 
 import enum
 import os
+from typing import NamedTuple
 
 import torch
 
@@ -86,6 +87,15 @@ class _Packer:
     def bias(self, key):
         k = key + ".bias"
         return self.f32(k) if k in self.sd else None
+
+
+class ControlResiduals(NamedTuple):
+    """The residuals of one or more ControlNets and their conditioning scales, as UNetEngine.forward injects them: one
+    b200sd_control_inject launch per skip connection and one for the mid block, whatever the number of nets.
+    ``nets[k][i]``: residual i (NHWC fp16, controlnet.py:218-229 order) of net k; ``scales``: fp32 CUDA tensor
+    [len(nets)], read by the kernel at run time (a captured graph replays with the values the tensor holds then)."""
+    nets: list
+    scales: torch.Tensor
 
 
 def guidance_scale_embedding(guidance_scale, dim, batch=1):
@@ -170,6 +180,7 @@ class UNetEngine:
             if os.environ.get("B200SD_STAGED", "0") == "1":
                 raise ValueError("palettization cannot be combined with B200SD_STAGED=1 (the staged epilogue)")
         L.reserve_attention_workspace(self.dev, max(c // h for c, h in zip(boc, self.heads)))
+        self._unit_scale = torch.ones(1, dtype=torch.float32, device=self.dev)  # one pre-summed residual set
         self._pack(state_dict)
 
     def _require_default_level(self, what):
@@ -457,6 +468,19 @@ class UNetEngine:
         if self.calib is not None and name in self.calib:
             L.absmax(L.layer_norm(tok, gamma, beta), self.calib[name])
 
+    # ------------------------------------------------------------------ ControlNet residuals
+    def _control(self, additional_residuals):
+        """forward's additional_residuals -> ControlResiduals (None stays None): a plain list of tensors is one
+        pre-summed set at scale 1 (UNetModel's additional_residual_i inputs, the C handle)."""
+        if additional_residuals is None or isinstance(additional_residuals, ControlResiduals):
+            return additional_residuals
+        return ControlResiduals([list(additional_residuals)], self._unit_scale)
+
+    @staticmethod
+    def _inject(ctrl, x, i):
+        """x + sum_k scale_k * residual i of net k (one launch)."""
+        return L.control_inject(x, [n[i] for n in ctrl.nets], ctrl.scales)
+
     # ------------------------------------------------------------------ blocks
     def _resnet(self, p, x, x1, temb_all):
         r = self.w[p]
@@ -646,13 +670,14 @@ class UNetEngine:
                 x = L.conv3x3(x, d["w"], d["b"], stride=2, stats=st if self.fuse_gn else None)
                 xs = st.get("chan")
                 skips.append((x, xs))
-        if additional_residuals is not None:  # the sums have no producer-side statistics: standalone GroupNorm there
-            skips = [(L.add(s, r), None) for (s, _), r in zip(skips, additional_residuals[:-1])]
+        ctrl = self._control(additional_residuals)
+        if ctrl is not None:  # the sums have no producer-side statistics: standalone GroupNorm there
+            skips = [(self._inject(ctrl, s, i), None) for i, (s, _) in enumerate(skips)]
         x, xs = self._resnet_f("mid_block.resnets.0", x, xs, None, None, temb_all)
         x, xs = self._transformer_f("mid_block.attentions.0", x, xs, kv_all, batch, self.heads[-1], s_ctx)
         x, xs = self._resnet_f("mid_block.resnets.1", x, xs, None, None, temb_all)
-        if additional_residuals is not None:
-            x, xs = L.add(x, additional_residuals[-1]), None
+        if ctrl is not None:
+            x, xs = self._inject(ctrl, x, -1), None
         rheads = self.heads[::-1]
         for i, typ in enumerate(self.up_types):
             for j in range(self.lpb + 1):
@@ -713,7 +738,8 @@ class UNetEngine:
     def forward(self, sample, timesteps, ctx_tokens, s_ctx, time_ids=None, text_embeds=None,
                 additional_residuals=None, temb_all=None, kv_all=None, out=None, timestep_cond=None):
         """sample: NHWC fp16 [B, H, W, in_pad]; timesteps fp32 [B]; ctx_tokens fp16 [B*s_ctx, D].
-        additional_residuals: list of NHWC fp16 tensors (ControlNet, unet.py:1009-1022).
+        additional_residuals: list of NHWC fp16 tensors (ControlNet, unet.py:1009-1022), or ControlResiduals: the
+        residuals of several ControlNets with their conditioning scales, summed in diffusers' fp16 order.
         temb_all / kv_all: precomputed time-embedding biases [B, sum Cout] / cross-attention keys and values (the
         per-prompt prologue of the pipeline's loop); out: optional fp32 NHWC output buffer.  timestep_cond: see
         time_embedding.  Returns noise_pred NHWC fp32 [B, H, W, out_ch]."""
@@ -736,13 +762,14 @@ class UNetEngine:
                 d = self.w[f"down_blocks.{i}.downsamplers.0.conv"]
                 x = L.conv3x3(x, d["w"], d["b"], stride=2)
                 skips.append(x)
-        if additional_residuals is not None:
-            skips = [L.add(s, r) for s, r in zip(skips, additional_residuals[:-1])]
+        ctrl = self._control(additional_residuals)
+        if ctrl is not None:
+            skips = [self._inject(ctrl, s, i) for i, s in enumerate(skips)]
         x = self._resnet("mid_block.resnets.0", x, None, temb_all)
         x = self._transformer("mid_block.attentions.0", x, kv_all, batch, self.heads[-1], s_ctx)
         x = self._resnet("mid_block.resnets.1", x, None, temb_all)
-        if additional_residuals is not None:
-            x = L.add(x, additional_residuals[-1])
+        if ctrl is not None:
+            x = self._inject(ctrl, x, -1)
         rheads = self.heads[::-1]
         for i, typ in enumerate(self.up_types):
             for j in range(self.lpb + 1):

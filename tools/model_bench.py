@@ -3,6 +3,7 @@
     python tools/model_bench.py --model sd15|sd21-base|sd21 [--reps 3]
     python tools/model_bench.py --inpaint [--rounds 5] [--reps 3]
     python tools/model_bench.py --guidance-free --model sd21-base|sdxl-base [--rounds 5] [--reps 3]
+    python tools/model_bench.py --controlnet [--rounds 5] [--reps 3]
 
 The workload is bench.py's: random-init weights, txt2img 512x512 at UNet batch 2 (uncond, cond), 20 DDIM steps, CFG
 7.5, the 20 steps (with the per-prompt prologue) captured as one CUDA graph by bench.LoopBench and timed with
@@ -14,7 +15,12 @@ SM clock while the loop ran.
 ``--guidance-free`` (512x512, random-init weights): the pipeline's 20-step DDIM loop graph with CFG 7.5 (UNet batch 2)
 against the same loop guidance-free (guidance 1.0, UNet batch 1), and the whole ``__call__`` (text encoding, the loop,
 VAE decode; output_type "np") of a 1-step Euler-ancestral (trailing) call at guidance 0 and a 4-step LCM call (the
-UNet with time_cond_proj_dim=256), alternated ``--rounds`` times.  One JSON line per mode."""
+UNet with time_cond_proj_dim=256), alternated ``--rounds`` times.  One JSON line per mode.
+
+``--controlnet``: SDXL-base at 1024x1024 (random-init weights), the pipeline's 20-step DDIM loop graph at CFG 5 (UNet
+batch 2) with 0, 1 and 2 random-init SDXL ControlNets (config.SDXL_CONTROLNET, scale 0.5) running at every step,
+alternated ``--rounds`` times, and one SDXL ControlNet forward at batch 2 alone (its own CUDA graph, CUDA events).
+One JSON line: ms per step of each loop, the ControlNet forward, and the 1-net loop less the 0-net loop."""
 import argparse
 import json
 import os
@@ -147,6 +153,59 @@ def guidance_free_modes(args, dev):
         print(json.dumps(rec), flush=True)
 
 
+def controlnet_modes(args, dev):
+    import numpy as np
+
+    from b200sd import config as C
+    from b200sd.pipeline import B200StableDiffusionPipeline as P
+
+    two = P.from_random_init("sdxl-base", device=dev, seed=1, scheduler="DDIM", height=1024, width=1024,
+                             controlnet_cfgs=[C.SDXL_CONTROLNET] * 2)
+    one = P(two.unet, two.vae_decoder, scheduler="DDIM", xl=True, controlnet=two.controlnet[:1])
+    g = torch.Generator().manual_seed(93)
+    emb = torch.cat([torch.zeros(1, 2048, 1, 77), torch.randn(1, 2048, 1, 77, generator=g)]).half()
+    lat = torch.randn(1, 4, 128, 128, generator=g).half().float()
+    kw = dict(time_ids=torch.tensor([[1024.0, 1024.0, 0.0, 0.0, 1024.0, 1024.0]] * 2),
+              text_embeds=torch.randn(2, 1280, generator=g))
+    cond = [torch.rand(2, 3, 1024, 1024, generator=g).half() for _ in range(2)]
+    n = bench.N_STEPS_IMG
+    graphs = {}
+    for mode, pipe, cc in (("0-controlnets", two, None), ("1-controlnet", one, cond[:1]), ("2-controlnets", two, cond)):
+        before = set(pipe._loop_graphs)
+        pipe.denoise(emb, lat, n, 5.0, controlnet_cond=cc, controlnet_conditioning_scale=0.5, **kw)
+        key, = set(pipe._loop_graphs) - before
+        graphs[mode] = pipe._loop_graphs[key]
+    # one ControlNet forward alone: the model's own graph on the static inputs the last loop left behind
+    cn = two.controlnet[0]
+    cn.forward_device()
+    sync = torch.cuda.synchronize
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    times = {m: [] for m in list(graphs) + ["controlnet-forward"]}
+    sampler = bench.ClockSampler(0)
+    sampler.start()
+    for _ in range(args.rounds):
+        for mode, graph in graphs.items():
+            times[mode].append(bench.timed_replays(graph, args.reps, sync) / n)
+        sync()
+        e0.record()
+        for _ in range(n * args.reps):
+            cn.forward_device()
+        e1.record()
+        sync()
+        times["controlnet-forward"].append(e0.elapsed_time(e1) / (n * args.reps))
+    clocks = sampler.stop()
+    med = {m: float(np.median(v)) for m, v in times.items()}
+    print(json.dumps({"model": "sdxl-base + SDXL ControlNet",
+                      "workload": "1024x1024, random-init weights, UNet / ControlNet batch 2, 20 DDIM steps, CFG 5, "
+                                  "conditioning scale 0.5, fp16, pipeline loop graph",
+                      "ms_per_step": {m: round(v, 4) for m, v in med.items()},
+                      "ms_per_step_rounds": {m: [round(x, 4) for x in v] for m, v in times.items()},
+                      "controlnet_cost_in_loop_ms": round(med["1-controlnet"] - med["0-controlnets"], 4),
+                      "second_controlnet_cost_in_loop_ms": round(med["2-controlnets"] - med["1-controlnet"], 4),
+                      "card": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0),
+                      "sm_mhz": clocks.get("sm_mhz"), "clock_events": clocks.get("reasons")}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--model", choices=("sd15", "sd21-base", "sd21", "sdxl-base"), default="sd15",
@@ -156,7 +215,14 @@ def main():
     ap.add_argument("--rounds", type=int, default=5, help="--inpaint / --guidance-free: alternated measurements per mode")
     ap.add_argument("--guidance-free", action="store_true",
                     help="--model sd21-base | sdxl-base: the CFG loop against the guidance-free one, Turbo / LCM calls")
+    ap.add_argument("--controlnet", action="store_true",
+                    help="SDXL-base 1024x1024: the loop with 0, 1 and 2 SDXL ControlNets, one ControlNet forward alone")
     args = ap.parse_args()
+    if args.controlnet:
+        dev = torch.device("cuda", 0)
+        torch.cuda.set_device(dev)
+        controlnet_modes(args, dev)
+        return
     if args.guidance_free:
         if args.model not in ("sd21-base", "sdxl-base"):
             ap.error("--guidance-free runs --model sd21-base or sdxl-base")
